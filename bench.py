@@ -65,11 +65,36 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM 3.35 TB/s HBM3), not measured"
+
+
+DUMP_CHAINS = 512          # chains sampled per output by --dump-outputs (d = 4: 40 MB of float32 in all)
+
+
+def dump_chain_index(batch, n=DUMP_CHAINS, seed=2024):
+    """The fixed, seeded sample of chains --dump-outputs writes (sorted; all chains when the batch is smaller)."""
+    if batch <= n:
+        return np.arange(batch)
+    return np.sort(np.random.default_rng(seed).choice(batch, n, replace=False))
+
+
+def take_chains(t, idx):
+    """Device tensor [..., batch] -> host float32 array [..., len(idx)] of the sampled chains."""
+    import torch
+    return t[..., torch.as_tensor(idx, device=t.device)].float().cpu().numpy()
+
+
+def write_outputs(dump_dir, arrays):
+    """--dump-outputs: one DIR/<name>.npy per output (float32 or float64)."""
+    os.makedirs(dump_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(dump_dir, name + ".npy"), a)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -228,6 +253,9 @@ def bench_other_config(args, ctx, dev, emit):
         def step():
             ctx.lgssm(y, **md, smooth=True, out_mean=mean, out_cov=cov, asynchronous=True)
         ms, launches, clocks = timed(step)
+        if args.dump_outputs:        # covariances are chain independent (shared model): a few chains of them suffice
+            idx = dump_chain_index(batch, 64)
+            write_outputs(args.dump_outputs, {"mean": take_chains(mean, idx), "cov": take_chains(cov, idx[:2])})
         for _ in range(3):
             step(); parts.append(ctx.profile_last_ms())
         sweep_ms, gain_ms = float(np.mean([p[0] for p in parts])), float(np.mean([p[1] for p in parts]))
@@ -246,7 +274,7 @@ def bench_other_config(args, ctx, dev, emit):
                             "frac": cov_bytes / (bcast_ms * 1e-3) / 1e9 / peak, "traffic": None, "peak_source": peak_src,
                             "kernel_ms": bcast_ms, "algorithmic_bytes_per_launch": cov_bytes,
                             "whole_step_frac": algo / (ms * 1e-3) / 1e9 / peak,
-                            "breakdown_ms": {"gain_tables_fp64": gain_ms, "mean_sweep_tcgen05": sweep_ms, "covariance_broadcast": bcast_ms},
+                            "breakdown_ms": {"gain_tables_fp64": gain_ms, "mean_sweep_wgmma": sweep_ms, "covariance_broadcast": bcast_ms},
                             "mean_sweep_TFLOPs": 8 * d * d * T * batch / (sweep_ms * 1e-3) / 1e12},
                "e2e": None, "e2e_note": "not measured for this config: the contract output alone is 67 GB of pinned host memory",
                "gpu_launches": int(launches), "clocks": clocks}
@@ -257,6 +285,8 @@ def bench_other_config(args, ctx, dev, emit):
     yh = (torch.randn(T, batch, device=dev, generator=g).cumsum(0) * 0.5).contiguous()
     outb = torch.empty(T, 4, batch, device=dev)
     ms, launches, clocks = timed(lambda: ctx.hgf_filter(yh, iters=iters, out=outb))
+    if args.dump_outputs:
+        write_outputs(args.dump_outputs, {"posteriors": take_chains(outb, dump_chain_index(batch, 2048))})
     msgs = 6 * iters * T * batch
     # end to end: host observations in, host posteriors out through the same entry point
     yhh = torch.empty(T, batch).pin_memory(); yhh.copy_(yh)
@@ -284,7 +314,7 @@ def bench_other_config(args, ctx, dev, emit):
                         "frac": io / (ms * 1e-3) / 1e9 / peak, "traffic": None, "peak_source": peak_src, "kernel_ms": ms,
                         "algorithmic_bytes_per_launch": io,
                         "note": "SFU / FP32-issue bound (652 ex2 + ~5 k FMA per 20 B of I/O): the HBM fraction is not the meaningful "
-                                "ceiling here (SURVEY.md 8d); see profiles/ for the pipe utilisation"},
+                                "ceiling here (SURVEY.md 8d)"},
            "e2e": {"value": msgs / (e_ms * 1e-3), "unit": "messages/s", "ms_per_step": e_ms, "h2d_bytes_per_step": int(yhh.numel() * 4),
                    "d2h_bytes_per_step": int(outh.numel() * 4)},
            "gpu_launches": int(launches), "clocks": clocks}
@@ -313,6 +343,9 @@ def main():
                     help="BASELINE.json configs[] index: 1 = headline (d=4, batch 65536), 2 = d=64 batch 4096 (tensor-core family), "
                          "3 = HGF T=1000 batch 32768, 20 VMP iterations")
     ap.add_argument("--sweep-variant", type=int, default=0, help="RXG_OPT_SWEEP_VARIANT (0 auto, 1 stash, 2 checkpoint, 3/4 time-segmented)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the posteriors of the last step (a fixed, seeded sample of chains) "
+                         "as DIR/<name>.npy, so that two builds can be compared output for output")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -402,10 +435,18 @@ def main():
         sampler.start()
     msgs = MSG_PER_STEP * T * batch * world
     gather = None
+    dump_idx = dump_chain_index(batch * world) if args.dump_outputs else None
     if world == 1:
         ms_per_step, launches = timed(step, args.steps)
+        if rank == 0 and args.dump_outputs:
+            write_outputs(args.dump_outputs, {"mean": take_chains(mean, dump_idx), "cov": take_chains(cov, dump_idx)})
     else:
         ms_per_step, launches = timed(lambda: step_gather(False), args.steps)          # contract: full gather in the step
+        if rank == 0 and args.dump_outputs:      # the gathered posteriors [G][T][...][batch] as seen by rank 0
+            parts = [(r, dump_idx[dump_idx // batch == r] - r * batch) for r in range(world)]
+            write_outputs(args.dump_outputs, {
+                "mean": np.concatenate([take_chains(grp.mean[r], i) for r, i in parts], axis=-1),
+                "cov": np.concatenate([take_chains(grp.cov[r], i) for r, i in parts], axis=-1)})
         ms_rep, l_rep = timed(lambda: step_gather(True), args.steps)
         ms_sweep, _ = timed(step, args.steps)
         slab = (mean.numel() + cov.numel()) * 4
@@ -432,8 +473,8 @@ def main():
                                        "covariance slabs replicated locally during the sweep; buffers bit-identical (asserted)"},
             "sweep_only": {"ms_per_step": ms_sweep, "value": msgs / (ms_sweep * 1e-3),
                            "note": "no gather (round-1 headline); NOT the contract at N > 1"},
-            "nvlink_floor_ms": {"full": (world - 1) * slab / 770e9 * 1e3, "replicated_cov": (world - 1) * mean.numel() * 4 / 770e9 * 1e3,
-                                "note": "bytes that must arrive per GPU / 770 GB/s measured peer bandwidth (B200_PROFILING.md)"},
+            "nvlink_floor_ms": {"full": (world - 1) * slab / 450e9 * 1e3, "replicated_cov": (world - 1) * mean.numel() * 4 / 450e9 * 1e3,
+                                "note": "bytes that must arrive per GPU / 450 GB/s (H100 SXM data sheet: 900 GB/s NVLink, both directions)"},
         }
         # the round-1 design for comparison: sweep, then ncclAllGather of the finished posteriors (into the same buffers)
         try:

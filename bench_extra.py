@@ -115,7 +115,7 @@ def main():
             mean = torch.empty(T, d, b, device="cuda"); cov = torch.empty(T, d, d, b, device="cuda")
             ms = timed(lambda: ctx.lgssm(y, **md, smooth=True, out_mean=mean, out_cov=cov, mask=mk), warm=1, reps=2)
             print(json.dumps({"what": "lgssm smooth, per-chain missing data, generic one-CTA-per-chain kernel (CUDA cores)", "d": d, "T": T,
-                              "batch": b, "ms": ms, "messages_per_s": 6 * T * b / ms * 1e3, "us_per_chain_step": ms * 1e3 / (T * b) * min(b, 148 * (2 if d <= 32 else 1))}))
+                              "batch": b, "ms": ms, "messages_per_s": 6 * T * b / ms * 1e3, "us_per_chain_step": ms * 1e3 / (T * b) * min(b, 132 * (2 if d <= 32 else 1))}))
             del y, mk, mean, cov
         yw = torch.randn(1500, 2, 32768, device="cuda", generator=g)
         ms = timed(lambda: ctx.mv_iid_wishart_vmp(yw, iterations=10), warm=2, reps=3)
@@ -146,7 +146,7 @@ def main():
                     a, bb = ctx.profile_last_ms(); sw.append(a); gn.append(bb)
                 ms = timed(run, warm=2, reps=3)
                 print(json.dumps({"what": "lgssm smooth, large-state family (shared model, cov de-duplicated)", "d": d, "T": T, "batch": b,
-                                  "sweep": "tcgen05 3xTF32 (umma_ky + lgssm_umma_sweep)" if no_umma == "0" else "FP32 pipe (lgssm_block_sweep)",
+                                  "sweep": "wgmma 3xTF32 (umma_ky + lgssm_umma_sweep)" if no_umma == "0" else "FP32 pipe (lgssm_block_sweep)",
                                   "ms": ms, "sweep_ms": float(np.mean(sw[-3:])), "gain_tables_ms": float(np.mean(gn[-3:])),
                                   "messages_per_s": 6 * T * b / ms * 1e3,
                                   "sweep_TFLOPs": 8 * d * d * T * b / (float(np.mean(sw[-3:])) * 1e-3) / 1e12}))

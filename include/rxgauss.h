@@ -1,4 +1,4 @@
-/* rxgauss.h -- C ABI of librxgauss: B200 (sm_100a) kernels for the Gaussian message-passing hot
+/* rxgauss.h -- C ABI of librxgauss: H100 (sm_90a) kernels for the Gaussian message-passing hot
  * path of RxInfer.jl's infer().
  *
  * This header is the drop-in boundary.  Every entry point replaces one piece of the reference's
@@ -72,7 +72,7 @@ enum rxg_flags {
 typedef enum rxg_option {
     RXG_OPT_GAIN_SEQ = 0,          /* 1: sequential Riccati gain kernels (cross-check of the time-parallel scan)   */
     RXG_OPT_LARGE_SEQ = 1,         /* 1: sequential gain kernels of the large-state family (cross-check)            */
-    RXG_OPT_NO_UMMA = 2,           /* 1: d >= 16 mean recursions on the FP32 pipe instead of tcgen05 (cross-check)  */
+    RXG_OPT_NO_UMMA = 2,           /* 1: d >= 16 mean recursions on the FP32 pipe instead of wgmma (cross-check)    */
     RXG_OPT_SWEEP_VARIANT = 3,     /* shared-model sweep: 0 auto, 1 stash, 3 time-segmented (experimental, slower)  */
     RXG_OPT_FORCE_CPT = 4,         /* chains per thread of the shared-model sweep (0 = auto)                        */
     RXG_OPT_HOST_THREADS = 5,      /* host threads of the host-side covariance broadcast (0 = auto)                 */
@@ -373,8 +373,8 @@ int rxg_stream_vmp_gamma_f32(rxg_ctx*, int T, int64_t batch, int iters, float w,
                              const float* prev, const float* y, float* out, float* free_energy,
                              unsigned flags);
 
-/* Diagnostic: D[128][64] = A[128][128] * B[64][128]' on the tcgen05 tensor pipe (kind::tf32, 3xTF32
- * split, TMEM accumulator), row-major device arrays.  Validates the hand-written UMMA descriptors
+/* Diagnostic: D[128][64] = A[128][128] * B[64][128]' on the tensor cores (wgmma tf32, 3xTF32 split,
+ * register accumulator), row-major device arrays.  Validates the hand-written wgmma descriptors
  * used by the large-state family; no reference counterpart.                                     */
 int rxg_selftest_umma_f32(rxg_ctx*, const float* A, const float* B, float* D, unsigned flags);
 /* Same for every operand shape the sweeps issue: D[128][n] = A[128][k] * B[n][k]' with

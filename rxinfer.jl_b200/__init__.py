@@ -1,4 +1,4 @@
-"""rxinfer.jl_b200 -- B200-native (sm_100a) Gaussian message-passing hot path of RxInfer.jl.
+"""rxinfer.jl_b200 -- H100-native (sm_90a) Gaussian message-passing hot path of RxInfer.jl.
 
 Contents: ``csrc/`` (CUDA kernels + the C ABI of ``librxgauss.so``, header in ``include/rxgauss.h``),
 this host-side mirror of the reference interface (``infer``, ``call_rule``, distribution

@@ -129,7 +129,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python rxinfer.jl_b200/build.py` "
-            "(nvcc, sm_100a).  There is no CPU fallback for the hot path.")
+            "(nvcc, sm_90a).  There is no CPU fallback for the hot path.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         try:

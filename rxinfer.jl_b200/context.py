@@ -477,7 +477,7 @@ class Context:
         return mz, vz
 
     def selftest_umma(self, A, B):
-        """D[128, n] = A[128, k] @ B[n, k].T on the tcgen05 tensor pipe (3xTF32), for the sweeps' operand shapes."""
+        """D[128, n] = A[128, k] @ B[n, k].T on the tensor cores (wgmma, 3xTF32), for the sweeps' operand shapes."""
         self._dev(A, B)
         n, k = B.shape
         D = self.empty(128, n)

@@ -14,8 +14,7 @@
 //   backward  elements (E_k, L_k) = (G_k, Sigma_f,k - G_k Sigma_p,k+1 G_k'):
 //               a_i (x) a_j = ( E_i E_j,  E_i L_j E_i' + L_i );  suffix(a_k..a_T).L = smoothed cov
 //
-// Depth is O(T / 1024 + log 1024) combines instead of O(T) Riccati steps (T = 1000: ~25 us
-// instead of ~1.8 ms on B200).  The sequential kernels in rxg_lgssm.cu remain as the
+// Depth is O(T / 1024 + log 1024) combines instead of O(T) Riccati steps.  The sequential kernels in rxg_lgssm.cu remain as the
 // cross-check (RXG_GAIN_SEQ=1).
 #pragma once
 #include <cooperative_groups.h>

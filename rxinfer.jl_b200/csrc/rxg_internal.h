@@ -18,7 +18,7 @@ struct rxg_ctx {
     void* stage = nullptr;
     size_t stage_bytes = 0;
     long long launches = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     bool gh_ready = false;
     // optional per-kernel timing of the last fused sweep (bench.py roofline leg)
     bool profile = false;
@@ -139,7 +139,7 @@ int rules_large_convert(rxg_ctx* ctx, int64_t n, int d, int k, const float* cons
 // rxg_lgssm_large.cu
 int lgssm_large_dispatch(rxg_ctx* ctx, LgssmCall& c);
 bool lgssm_large_supported(int d, int m);
-// rxg_umma_sweep.cu (d = 16 / 32 / 64 mean recursions on tcgen05)
+// rxg_umma_sweep.cu (d = 16 / 32 / 64 mean recursions on the tensor cores, wgmma)
 int launch_umma_sweep(rxg_ctx* ctx, int d, bool smooth, const float* recFE, const float* recG, const float* recK,
                       const float* m0, const float* m0c, const float* y, float* mean, int T, int64_t batch);
 

@@ -404,7 +404,7 @@ static int launch_shared(rxg_ctx* ctx, LgssmCall& c, const ModelF<D, M>& mdl, co
     bool has_u = false;
     for (int i = 0; i < D; ++i) has_u |= (mdl.u[i] != 0.f);
     // checkpoint + recompute instead of the forward->backward stash (RXG_NO_CKPT=1: A/B switch)
-    bool ckpt = c.smooth && (D * D <= 16) && (CPT == 2);   // with one chain per thread the stash path is faster (B200: 1.85 vs 2.06 ms)
+    bool ckpt = c.smooth && (D * D <= 16) && (CPT == 2);   // with one chain per thread the stash path is faster
     if (ctx->opt[RXG_OPT_SWEEP_VARIANT] == 1) ckpt = false;                     // stash variant (A/B switch)
     // fused all-gather: only the headline variant (smoothing, no evidence, no offset) has a PEER instantiation;
     // everything else leaves fused_peer_stores false and the caller pushes the finished slab
@@ -544,8 +544,7 @@ static int run_shared_family(rxg_ctx* ctx, LgssmCall& c) {
     }
     const bool al16 = (((uintptr_t)c.y | (uintptr_t)c.mean | (uintptr_t)c.cov | (uintptr_t)c.nle | (uintptr_t)c.mean0_chain) & 15) == 0;
     // chains per thread: keep >= ~2 resident warps per SM sub-partition
-    // Wider per-thread vectors cut the number of (128-byte-per-warp) store instructions per byte;
-    // B200, d = m = 4, T = 1000, batch 65 536: CPT 1 / 2 / 4 = 1.85 / 1.50 / 1.58 ms (262 144: 2 beats 4 too).
+    // Wider per-thread vectors cut the number of (128-byte-per-warp) store instructions per byte.
     int cpt = (c.batch >= (int64_t)ctx->sm_count * 64 * 2) ? 2 : 1;
     if (ctx->opt[RXG_OPT_FORCE_CPT] > 0) cpt = (int)ctx->opt[RXG_OPT_FORCE_CPT];      // test / tuning override
     if (D * M > 16 && cpt > 2) cpt = 2;                              // register budget for d = 6

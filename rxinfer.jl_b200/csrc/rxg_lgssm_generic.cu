@@ -10,9 +10,8 @@
 // one Cholesky per direction).  All matrices live in shared memory (row-major, leading dimension n + 1), every
 // operation is block-cooperative over 256 threads; the filtered (mu, Sigma) are stashed in the output buffers and
 // overwritten by the smoothed ones on the way back.  fp32 storage and arithmetic like the register kernels.
-// Throughput is that of a CUDA-core fallback: measured on B200 (T = 1000, smoothing, 20 % missing data) d = 16: 20 us per
-// step and chain (2048 chains in 140 ms), d = 64: 390 us (512 chains in 1.35 s) -- ~800 barrier-separated phases per step
-// with little work each; a variant with block-parallel triangular solves (two barriers per row) was slower (451 us).
+// Throughput is that of a CUDA-core fallback: ~800 barrier-separated phases per step with little work each; a variant
+// with block-parallel triangular solves (two barriers per row) was slower.
 // The shared-model gain-table families remain the fast path; a tensor-core per-chain recursion is the open item.
 #include <math.h>
 

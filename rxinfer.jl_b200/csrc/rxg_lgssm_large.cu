@@ -10,8 +10,8 @@
 //      GEMMs per step,  X <- [F_t | K_t] [X ; Y_t]  and  X <- [E_t | G_t] [mu_f,t ; X],
 //      executed by lgssm_block_sweep with the per-step gain block streamed through shared memory
 //      (cp.async, double buffered) and a 4 x 2 register tile per thread.
-// For d >= 16 the mean recursions run on the tensor cores (rxg_umma_sweep.cu: tcgen05 kind::tf32, 3xTF32 split,
-// TMEM accumulators, TMA bulk copies of the gain records); lgssm_block_sweep is the d = 8 path and the
+// For d >= 16 the mean recursions run on the tensor cores (rxg_umma_sweep.cu: wgmma tf32, 3xTF32 split,
+// register accumulators, TMA bulk copies of the gain records); lgssm_block_sweep is the d = 8 path and the
 // RXG_OPT_NO_UMMA cross-check.  The family also produces neg_log_evidence (large_evidence_kernel).
 #include <math.h>
 
@@ -123,7 +123,7 @@ struct LargeWs {
     float *ss, *sf;                          // [T][D*D] smoothed / filtered covariance (fp32)
     int* flag;
     int b_identity;                          // B == I: skip the two B products
-    // tensor-core sweep (rxg_umma_sweep.cu): per-step gain blocks split tf32 hi | lo in the canonical UMMA
+    // tensor-core sweep (rxg_umma_sweep.cu): per-step gain blocks split tf32 hi | lo in the canonical
     // K-major layout (K = D), or null:  recFE[t] = [F_t ; E_{t-1}] (2D x D),  recG[t] = G_t,  recK[t] = K_t (D x D)
     float *recFE, *recG, *recK;
     // evidence (optional): evT[t][(D+M)][M] = [-(L_t^-1 B A) | L_t^-1]' (k-major, like fwdT) with S_t = L_t L_t',
@@ -228,7 +228,7 @@ __global__ void __launch_bounds__(256) large_gain_tables(LargeWs w, int T, int t
     float* ft = w.fwdT + (size_t)t * (D + M) * D;
     const bool pred = (t > 0) || transition_first;
     // tensor-core sweep: emit a D x D block W(r, k) = srcT[k][r] into rows [row0, row0 + D) of a record whose hi part
-    // starts at rec_hi and lo part at rec_lo (canonical K-major UMMA layout with K = D, rxg_umma.cuh)
+    // starts at rec_hi and lo part at rec_lo (canonical K-major layout with K = D, rxg_umma.cuh)
     auto emit_umma = [&](float* rec_hi, float* rec_lo, const float* srcT, int row0) {
         for (int idx = threadIdx.x; idx < D * D; idx += blockDim.x) {
             const int k = idx / D, r = idx % D;
@@ -935,7 +935,7 @@ static int run_large(rxg_ctx* ctx, LgssmCall& c) {
     }
     const unsigned blocks = (unsigned)((c.batch + NB - 1) / NB);
     auto sweep = [&](bool smooth) -> int {
-        if (use_umma)   // tensor-pipe sweep (tcgen05 kind::tf32, 3xTF32): 128 chains per CTA; u_t = K_t y_t pre-pass + recursion
+        if (use_umma)   // tensor-pipe sweep (wgmma tf32, 3xTF32): 64 chains per CTA; u_t = K_t y_t pre-pass + recursion
             return launch_umma_sweep(ctx, D, smooth, w.recFE, w.recG, w.recK, dm0, c.mean0_chain, c.y, c.mean, c.T, c.batch);
         if (smooth) lgssm_block_sweep<D, M, NB, true><<<blocks, (D / 4) * (NB / 2), smw, ctx->stream>>>(w.fwdT, w.bwdT, dm0, c.mean0_chain, c.y, c.mean, c.T, c.batch);
         else        lgssm_block_sweep<D, M, NB, false><<<blocks, (D / 4) * (NB / 2), smw, ctx->stream>>>(w.fwdT, w.bwdT, dm0, c.mean0_chain, c.y, c.mean, c.T, c.batch);
@@ -965,9 +965,8 @@ static int run_large(rxg_ctx* ctx, LgssmCall& c) {
     }
     if (ctx->profile) cudaEventRecord(ctx->ev[2], ctx->stream);
     // Per-chain covariance output (the contract): T d^2 rows broadcast over the batch -- 67 GB at configs[2], pure HBM
-    // writes at the write roofline (8.9 ms).  Measured in round 2: running it on a side stream concurrently with the mean
-    // sweeps gains nothing (20.96 -> 21.0 ms): the broadcast streams through L2 and evicts the per-step gain records that
-    // all chain tiles of the latency-bound tcgen05 sweep share, which then slows from 5.5 to 14.3 ms.  Sequential it is.
+    // writes.  It runs after the mean sweeps, not beside them: the broadcast streams through L2 and would evict the
+    // per-step gain records that all chain tiles of the latency-bound tensor-core sweep share.
     if (c.cov) {
         const float* tab = c.smooth ? w.ss : w.sf;
         if (c.flags & RXG_COV_SHARED_OUT) {

@@ -18,14 +18,14 @@
 // Compared with lgssm_shared_kernel (one thread walks all T steps): no forward->backward stash or checkpoint at
 // all, no dependent chain longer than 16 steps, 64 loads in flight per thread instead of 4-8, and the second read of
 // y happens ~one tile lifetime after the first, from a working set of (CTAs x 32 chains x T x 4m bytes) = 76 MB at
-// the headline config -- inside the 126 MB L2 when the y lines are loaded evict_last in pass A, evict_first in pass B
+// the headline config -- more than the H100's 50 MB L2, so the reuse is partial even when the y lines are loaded evict_last in pass A, evict_first in pass B
 // and the 80 B/step of posterior stores are evict_first (createpolicy + .L2::cache_hint).  DRAM traffic per
-// (chain, step) then is 4 (m + d + d^2) = the algorithmic 96 B at d = m = 4 (checkpoint kernel: 114 B).
-// STATUS (B200, round 2): EXPERIMENTAL, not the default (RXG_OPT_SWEEP_VARIANT = 3 selects it; parity tests keep it honest).
-// Measured at the headline config: 1.96 ms (+ 0.28 ms for seg_tables_kernel) against 1.35 ms for lgssm_shared_kernel.
+// (chain, step) then is 4 (m + d + d^2) = the algorithmic 96 B at d = m = 4 (checkpoint kernel: ~115 B).
+// STATUS: EXPERIMENTAL, not the default (RXG_OPT_SWEEP_VARIANT = 3 selects it; parity tests keep it honest).
+// It measured slower than lgssm_shared_kernel at the headline config.
 // Two lessons recorded in DESIGN.md: (1) these sweeps are instruction-cache sensitive -- a first version with per-store
-// peer loops was 31 K instructions and took 8.2 ms, this one is 5.1 K (lgssm_shared_kernel: 3.4 K; the same effect took
-// that kernel from 1.35 to 2.25 ms when peer loops grew it to 11 K); (2) with y[T][m][batch] a CTA that owns 32 chains for
+// peer loops was 31 K instructions, this one is 5.1 K (lgssm_shared_kernel: 3.4 K; the same effect slowed that kernel by
+// two thirds when peer loops grew it to 11 K); (2) with y[T][m][batch] a CTA that owns 32 chains for
 // all T gathers 128-byte pieces 256 KB apart, and once the CTAs drift apart in time the DRAM pages and the output rows
 // are no longer shared between neighbouring CTAs -- the lock-step walk of lgssm_shared_kernel (all CTAs at the same t)
 // is what keeps its accesses row-coherent.  The L2 reuse the design aims at needs chain tiles that are wide in memory

@@ -1,6 +1,6 @@
 // lgssm_shared_kernel: the mean-only forward/backward sweep of the shared-model path.
 //
-// One warp = one CTA = 32 x CPT chains, so CTAs spread over the 148 SMs to within one warp and no
+// One warp = one CTA = 32 x CPT chains, so CTAs spread over the 132 SMs to within one warp and no
 // block-wide barrier is ever needed.  Per (chain, step) the sweep moves
 //     forward : read y_t (m)            write filtered mean (d)      [stash, in post_mean]
 //     backward: read filtered mean (d)  write smoothed mean (d) + smoothed covariance (d*d)
@@ -122,7 +122,7 @@ __device__ __forceinline__ void peer_store(const PeerOut& po, int write_cov, int
 
 // PEER: the final posteriors are also stored to the peer ranks' gathered buffers (fused all-gather, rxg_peer.cu).
 // A separate instantiation, because the kernel is instruction-cache sensitive: the loops over peers inside the
-// unrolled step bodies took the single-GPU kernel from 3.4 K to 11 K instructions and from 1.35 to 2.25 ms on B200.
+// unrolled step bodies took the single-GPU kernel from 3.4 K to 11 K instructions.
 template <int D, int M, int CPT, int PF, bool SMOOTH, bool EVID, bool OFFSET, bool CKPT, bool PEER = false>
 __global__ void __launch_bounds__(32, 16 / CPT)   // CPT=1: <= 128 regs so ~14 warps/SM stay resident; wider CPT trades warps for ILP
 lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __restrict__ fwd_tab,
@@ -131,12 +131,15 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
                     float* __restrict__ nle, int T, int64_t batch, int transition_first,
                     int write_cov, const float* __restrict__ mu0c, const __grid_constant__ PeerOut po) {
     using TB = Tab<D, M>;
-    constexpr int TC = 4 * PF;                                   // table chunk, in time steps
-    constexpr int REC_MAX = TB::FWD_REC > TB::BWD_REC ? TB::FWD_REC : TB::BWD_REC;
     // CKPT (smoothing only): the forward pass keeps one filtered mean per TC-step chunk; the backward
     // pass re-reads y and recomputes the chunk's filtered means into s_f (lane-contiguous, private
     // to each thread), which replaces the 2 x 4d bytes/step stash by 4m bytes/step of y re-read.
     constexpr bool CK = SMOOTH && CKPT && (D * D <= 16);   // larger states exceed the static smem budget: stash path
+    // table chunk, in time steps.  With CK, 12-step chunks keep the static shared memory at 22.6 KB (d = m = 4, CPT = 2),
+    // so 9 CTAs fit in an SM and a 65 536-chain grid (1024 one-warp CTAs) is resident in one wave on 132 SMs; 16-step
+    // chunks (30.2 KB, 7 CTAs per SM) leave a second wave of 100 CTAs.
+    constexpr int TC = CK ? 3 * PF : 4 * PF;
+    constexpr int REC_MAX = TB::FWD_REC > TB::BWD_REC ? TB::FWD_REC : TB::BWD_REC;
     __shared__ __align__(16) float s_tab[2][TC * (CK ? (TB::FWD_REC + TB::BWD_REC) : REC_MAX)];
     __shared__ float s_f[CK ? TC * D * CPT * 32 : 1];
 

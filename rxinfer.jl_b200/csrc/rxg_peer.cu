@@ -1,8 +1,8 @@
 // Peer-mapped all-gather of posterior marginals over NVLink / NVSwitch -- no NCCL on the data path.
 //
-// north_star: "the batch dimension shards across the 8xB200 box with one all-gather of posterior marginals at
+// north_star: "the batch dimension shards across the GPUs of one node with one all-gather of posterior marginals at
 // the end".  A separate collective after the sweep costs (G-1)/G of the gathered bytes over NVLink AFTER the
-// compute has finished (round 1: 54.8 ms of ncclAllGather behind a 1.47 ms sweep at 8 GPUs).  Here every rank
+// compute has finished.  Here every rank
 // maps its peers' gathered buffers (CUDA IPC, NVLink P2P) and
 //   * the fused smoothing sweep stores each smoothed mean (and, for the literal full gather, each covariance)
 //     straight into all G gathered buffers while the backward recursion is still running (st.global on peer
@@ -319,11 +319,7 @@ int rxg_lgssm_smooth_gather_f32(rxg_ctx* ctx, int d, int m, int T, int64_t batch
             pc[np] = (gathered_cov && !replicate) ? gathered_cov[g] + r * slab_c : nullptr;
             ++np;
         }
-    // Fused in-kernel peer stores (default) or push-after-sweep (RXG_OPT_GATHER_MODE = 2, kept for comparison).  Measured
-    // (B200, 65 536 chains per GPU, profiles/r2_bench_{2,8}gpu*.json): replicated covariances G = 2: fused 2.64 ms, push
-    // 3.61 ms; G = 8: fused 15.4 ms, push 16.4 ms (the 7.3 GB of means leave at ~480 GB/s either way while the local
-    // covariance replication writes 29 GB into the same HBM).  Full gather G = 2: 7.84 vs 8.98 ms; G = 8: 54.3 ms fused vs
-    // 55.8 ms sweep + ncclAllGather (NVLink bound: 47.7 ms).
+    // Fused in-kernel peer stores (default) or push-after-sweep (RXG_OPT_GATHER_MODE = 2, kept for comparison).
     const long long gmode = ctx->opt[RXG_OPT_GATHER_MODE];
     const bool fuse = gmode != 2;
     if (fuse) {

@@ -8,7 +8,7 @@
 //                     [d] x [d n], and for a fixed first index the slab [c][n] is a [d] x [n] matrix.  One thread = one
 //                     column, A' staged in shared memory and read as float4 (4 FMAs per LDS), up to 64 accumulators in
 //                     registers.  CUDA cores: 2 M K flops per K + M floats of traffic = 16 flop/B at d = 64, i.e. FP32-issue
-//                     bound (the tcgen05 version of this product is what DESIGN.md section 7 lists next);
+//                     bound (a tensor-core version of this product is what DESIGN.md section 7 lists next);
 //   * k_cholinv_warp  FastCholesky.cholinv twin (every `mean_cov` / `weightedmean_precision` / *(:in) / marginal of the
 //                     reference): one warp = one message, the matrix in shared memory (row stride d + 1: conflict-free for
 //                     lane-per-row and lane-per-column access), left-looking Cholesky with lane-per-row, L^-1 by forward

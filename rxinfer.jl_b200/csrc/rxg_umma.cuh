@@ -1,12 +1,15 @@
-// Minimal hand-written tcgen05 / TMEM building blocks (sm_100a inline PTX) for the large-state
-// sweep GEMM: UMMA shared-memory descriptors for the canonical K-major no-swizzle layout, the
-// kind::tf32 instruction descriptor, TMEM alloc / load, commit + mbarrier.
+// Minimal hand-written Hopper tensor-core building blocks (sm_90a inline PTX) for the large-state sweep GEMM:
+// wgmma shared-memory descriptors for the canonical K-major no-swizzle layout, wgmma.mma_async kind tf32 with
+// register accumulators, mbarrier + TMA bulk copies.
 //
-// Canonical K-major, SWIZZLE_NONE operand layout (units of 16 bytes; cute/atom/mma_traits_sm100.hpp
-// "LayoutType::INTERLEAVE : ((8,n),2):((1,SBO),LBO)"): a core matrix is 8 rows x 16 bytes stored
+// Canonical K-major, SWIZZLE_NONE operand layout (units of 16 bytes; cute/atom/mma_traits_sm90_gmma.hpp
+// "LayoutType::INTERLEAVE : ((8,m),(T,2k)):((1T,SBO),(1,LBO))"): a core matrix is 8 rows x 16 bytes stored
 // contiguously (128 B); core matrices adjacent along K are LBO bytes apart, adjacent 8-row groups
 // SBO bytes apart.  For fp32/tf32 one 16-byte row piece holds 4 elements and one MMA consumes
 // K = 8 (two core matrices along K).
+//
+// Accumulator fragment of wgmma m64nNk8 (f32): thread i of the warpgroup (warp w = i / 32, lane l) holds
+// d[4j + 2h + e] = D(16 w + l / 4 + 8 h, 8 j + 2 (l % 4) + e),  j < N / 8, h, e in {0, 1}.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -26,113 +29,50 @@ __device__ __forceinline__ uint64_t smem_desc(uint32_t smem_addr, uint32_t lbo, 
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);            // start address       bits [0,14)
     d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;            // leading byte offset bits [16,30)
     d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;            // stride byte offset  bits [32,46)
-    d |= (uint64_t)1 << 46;                                // descriptor version (Blackwell)
-    return d;                                              // base offset 0, lbo mode 0, SWIZZLE_NONE
-}
-// kind::tf32, fp32 accumulate, A and B K-major
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+    return d;                                              // base offset 0, layout type 0 = SWIZZLE_NONE
 }
 
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]' (tf32 in, fp32 accumulate), A and B K-major in shared memory.
+// accumulate = 0 ignores the previous contents of d.
+template <int N>
+__device__ __forceinline__ void mma_tf32(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+
+template <>
+__device__ __forceinline__ void mma_tf32<16>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void commit(uint64_t* mbar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                     (uint32_t)__cvta_generic_to_shared(mbar))
-                 : "memory");
+
+template <>
+__device__ __forceinline__ void mma_tf32<32>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {   // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     (uint32_t)__cvta_generic_to_shared(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {        // same warp as alloc
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// pin accumulator registers behind the wait: the compiler must not read them before wgmma_wait_all()
+__device__ __forceinline__ void fence_reg(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* mbar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(mbar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* mbar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t"
-        "}\n" ::"r"((uint32_t)__cvta_generic_to_shared(mbar)),
-        "r"(parity)
-        : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives row (lane_base + i)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-// Split-phase variant: issue several loads, wait once (tmem_ld_wait), then pin the destination registers behind
-// the wait (tmem_ld_fence16) so that the compiler cannot hoist their uses above it.
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_fence16(uint32_t* r) {
-    asm volatile("" : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                      "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :
-                 : "memory");
-}
-// NC = 16 or 32 columns
-template <int NC>
-__device__ __forceinline__ void tmem_ldn(uint32_t taddr, float* v) {
-    if (NC == 32) tmem_ld32(taddr, v); else tmem_ld16(taddr, v);
 }
 
 // ---- TMA bulk copy (1-D, no tensor map): global -> shared, completion on an mbarrier (complete_tx)

@@ -1,7 +1,7 @@
 # RxGaussB200.jl -- the Julia side of the drop-in: routes the batched Gaussian hot path of RxInfer's `infer`
 # to librxgauss.so (include/rxgauss.h) through plain `ccall`.  No CUDA.jl, no code generation: device memory,
 # copies and peer mapping all go through the C ABI (rxg_device_alloc / rxg_memcpy_* / rxg_peer_*), the kernels
-# are the hand-written sm_100a ones in csrc/.
+# are the hand-written sm_90a ones in csrc/.
 #
 # Layers (each usable on its own):
 #   1. `Lib`      one thin wrapper per export of include/rxgauss.h (every export is bound: tests/test_julia_shim.py

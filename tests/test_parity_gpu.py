@@ -443,7 +443,7 @@ def test_large_state_doubling_vs_sequential(ctx, monkeypatch, d, T):
 
 @pytest.mark.parametrize("d,T,batch", [(16, 90, 300), (32, 70, 129), (64, 50, 257)])
 def test_large_state_tensor_core_vs_fp32_pipe(ctx, monkeypatch, d, T, batch):
-    """d >= 16: the mean recursions run on tcgen05 (u_t = K_t y_t pre-pass + [F;E] / G recursion, 3xTF32);
+    """d >= 16: the mean recursions run on the tensor cores (wgmma; u_t = K_t y_t pre-pass + [F;E] / G recursion, 3xTF32);
     RXG_NO_UMMA=1 runs the same tables through the FP32-pipe block sweep.  Ragged last chain tile, several
     time slices in the pre-pass; smoothing and filtering; both against each other and the oracle."""
     mod = f32_model(lgssm.dense_model(d, seed=5))

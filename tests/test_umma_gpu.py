@@ -1,4 +1,4 @@
-"""tcgen05 / TMEM plumbing self-test: D[128, n] = A[128, k] B[n, k]' on the tensor pipe with the 3xTF32 split must
+"""wgmma descriptor / fragment plumbing self-test: D[128, n] = A[128, k] B[n, k]' on the tensor pipe with the 3xTF32 split must
 match the fp64 product to fp32-level accuracy, for every operand shape the large-state sweeps issue
 (K-major canonical layout with K = 16 / 32 / 64 / 128, N = 16 ... 128)."""
 import numpy as np

@@ -11,9 +11,8 @@ from oracle import hgf, vmp
 from util import rel_l2
 
 pytestmark = pytest.mark.gpu
-# GPU (fp32) vs oracle (fp64) bounds, relative L2 over all (t, chain) -- all inside the contract's 1e-5.  Measured on B200
-# (round 2, after psi / det of the GCV joint were put in cancellation-free closed form): m_x 6.7e-8, v_x 9.1e-8,
-# m_z 3.0e-7, v_z 4.2e-7 (T = 300); at configs[3] size (T = 1000, batch 32 768, 20 iterations): 6.5e-8, 3.3e-7, 6.3e-7, 9.1e-7.
+# GPU (fp32) vs oracle (fp64) bounds, relative L2 over all (t, chain) -- all inside the contract's 1e-5 (psi / det of the
+# GCV joint are in cancellation-free closed form).
 # Round 1 needed 1e-4 / 2e-3 / 5e-3 / 5e-3.
 HGF_TOL = {"m_x": 1e-6, "v_x": 2e-6, "m_z": 5e-6, "v_z": 5e-6}
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -67,7 +66,7 @@ def test_hgf_free_energy_vs_oracle_and_chunks(ctx):
     assert fe.shape == (120, 8, 96)
     err = np.abs(fe - fe_ref)
     print("hgf free energy: max abs err", err.max(), "mean abs err", err.mean(), "scale", np.abs(fe_ref).mean())
-    assert err.max() < 2e-4 and err.mean() < 1e-5          # measured on B200: 2.0e-5 / 4.7e-7
+    assert err.max() < 2e-4 and err.mean() < 1e-5
     plain = ctx.hgf_filter(dev(y), iters=8)
     assert torch.equal(plain, out)                              # the FE variant does not perturb the posteriors
     o1, f1 = ctx.hgf_filter(dev(y[:50]), iters=8, want_free_energy=True)
