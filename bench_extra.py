@@ -3,12 +3,14 @@
 the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >= 3 warm-ups.
 
   python bench_extra.py [--which per_chain,filter,hgf,rules,vmp,scaling_T]
+  python bench_extra.py --which predict      (opt-in: observation predictions / forecasts after the smoother)
 """
 from __future__ import annotations
 
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 import numpy as np
@@ -33,6 +35,55 @@ def timed(fn, warm=3, reps=5):
     return e0.elapsed_time(e1) / reps
 
 
+def gpu_name_and_power_limit():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        name, plim = (x.strip() for x in out.split(",")[:2])
+        return name, plim
+    except Exception:
+        return torch.cuda.get_device_name(0), "unknown"
+
+
+def bench_predict(ctx, peak):
+    """Smoother alone vs smoother + predictions (rxg_lgssm_smooth_predict_f32); the post-pass time is the difference of the
+    two (CUDA events, same inputs, alternated).  Algorithmic bytes of the post-pass means: read y (4 m, observed steps only)
+    and mu (4 d), write y_hat (4 m) per (chain, step); forecast rows read and write the state (8 d) and write y_hat (4 m)."""
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(11)
+    nb = notebook_model_f32()
+    dn = dense_model_f32(64)
+    cases = [("config-2 size, shared model, H = 0", nb, 1000, 65536, 0, None),
+             ("config-2 size, shared model, H = 100, last 100 steps missing (shared mask)", nb, 1000, 65536, 100, "tail"),
+             ("d = 64 dense model, H = 0 (left-GEMM route)", dn, 1000, 4096, 0, None)]
+    for name, mod, T, batch, H, mk in cases:
+        d, m = mod["A"].shape[0], mod["B"].shape[0]
+        y = torch.randn(T, m, batch, device="cuda", generator=g) * 3.3
+        mask = None
+        if mk == "tail":
+            mask = np.ones(T, dtype=np.uint8); mask[-100:] = 0
+        args = [mod[k] for k in ("A", "B", "P", "Q", "m0", "S0")]
+        smooth = lambda: ctx.lgssm(y, *args, mask=mask, cov_shared_out=mask is None)
+        # with a mask the smoother writes per-chain covariances: there the post-pass is timed for the prediction means
+        # only (no per-chain prediction or state-forecast covariance broadcast, state forecasts in library scratch)
+        pred = lambda: ctx.lgssm_predict(y, *args, horizon=H, mask=mask, cov_shared_out=mask is None,
+                                         want_pred_cov=mask is None, want_forecast_states=H > 0 and mask is None)
+        ts, tp = [], []
+        for _ in range(3):
+            ts.append(timed(smooth)); tp.append(timed(pred))
+        ms_s, ms_p = float(np.median(ts)), float(np.median(tp))
+        nobs = T - (100 if mk == "tail" else 0)
+        byts = 4 * batch * (nobs * (d + 2 * m) + (T - nobs) * (d + m) + H * (2 * d + m + d))
+        post = ms_p - ms_s
+        print(json.dumps({"what": "lgssm smooth + predictions: " + name, "d": d, "m": m, "T": T, "H": H, "batch": batch,
+                          "smoother_ms": ms_s, "smoother_plus_predict_ms": ms_p, "postpass_ms": post,
+                          "postpass_algorithmic_GB": byts / 1e9,
+                          "postpass_frac_of_peak_hbm": (byts / (post * 1e-3)) / (peak * 1e9) if post > 0 else None,
+                          "peak_hbm_gbs": peak, "gpu": gname, "power_limit": plim}), flush=True)
+        del y
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -40,6 +91,8 @@ def main():
     which = set(args.which.split(","))
     ctx = rx.Context(0)
     peak, _ = peaks()
+    if "predict" in which:
+        bench_predict(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

@@ -297,6 +297,30 @@ int rxg_lgssm_smooth_f32(rxg_ctx*, int d, int m, int T, int64_t batch, const flo
                          const float* S0, const float* u, const float* y, const uint8_t* ymask,
                          float* post_mean, float* post_cov, float* neg_log_evidence,
                          int32_t* status, unsigned flags);
+/* Smoothing sweep + predictive distributions of the observations (result.predictions)
+ * [ref: predictvars and the automatic predictions for data containing `missing`, src/inference/batch.jl:203-246;
+ *  tested in test/inference/prediction_tests.jl:193-420].  The prediction for y[t] is the reference's message
+ * toward y[t]: the cavity fwd_t x bwd_t passed through *(:out) with B and MvNormalMeanCovariance(:out) with Q.
+ * With the smoothed posterior (mu_s, S_s) and D_t = Q - B S_s[t] B' (formed and factorised in fp64):
+ *     missing y[t]:   N(B mu_s[t], B S_s[t] B' + Q)
+ *     observed y[t]:  N(y_t - Q D_t^-1 (y_t - B mu_s[t]), Q D_t^-1 Q)
+ *     forecast k = 1..H from (x_0, S_0) = (mu_s[T-1], S_s[T-1]):  x_k = A x_{k-1} + u, S_k = A S_{k-1} A' + P,
+ *                     prediction N(B x_k, B S_k B' + Q)  (== the smoother on y padded with H missing steps)
+ * Arguments shared with rxg_lgssm_smooth_f32 mean the same, and post_mean / post_cov / neg_log_evidence are
+ * bit-identical to its outputs.  Outputs: pred_mean[T+H][m][batch] (rows T.. are the forecasts), pred_cov
+ * [T+H][m][m][batch] ([T+H][m][m] with RXG_COV_SHARED_OUT) or NULL, fc_mean[H][d][batch] (state forecasts) or
+ * NULL, fc_cov[H][d][d][batch] ([H][d][d] with RXG_COV_SHARED_OUT) or NULL.  post_cov may be NULL (shared model,
+ * no per-chain mask) only at the register-resident shapes, whose own covariance table then feeds the post-pass; other
+ * shapes return RXG_ERR_UNSUPPORTED before anything runs.  Device pointers only
+ * (RXG_ERR_UNSUPPORTED otherwise); H < 0 or pred_mean NULL -> RXG_ERR_BAD_ARG; a chain whose D_t is not SPD gets
+ * RXG_ERR_NOT_SPD in status[b] (shared model: every chain, and the call returns RXG_ERR_NOT_SPD).  As for the
+ * smoother, y at masked steps is ignored but must be finite.                                     */
+int rxg_lgssm_smooth_predict_f32(rxg_ctx*, int d, int m, int T, int H, int64_t batch, const float* A,
+                                 const float* B, const float* P, const float* Q, const float* m0,
+                                 const float* S0, const float* u, const float* y, const uint8_t* ymask,
+                                 float* post_mean, float* post_cov, float* neg_log_evidence,
+                                 float* pred_mean, float* pred_cov, float* fc_mean, float* fc_cov,
+                                 int32_t* status, unsigned flags);
 /* Forward half only (filtering) -- what the streaming engine computes per datum with
  * @autoupdates x_min_t_mean, x_min_t_cov = mean_cov(q(x_t))
  * [ref: src/inference/streaming.jl:344-388; src/inference/autoupdates.jl:614-659; ipynb:199-216]. */

@@ -17,7 +17,8 @@ def __getattr__(name):   # lazy: these import torch
         from . import context
         return getattr(context, name)
     if name in ("infer", "InferenceResult", "linear_gaussian_ssm_smoothing", "linear_gaussian_ssm_filtering",
-                "hgf", "univariate_lgssm_gamma_precision", "kalman_gamma_streaming", "latent_autoregressive", "default_context"):
+                "hgf", "univariate_lgssm_gamma_precision", "kalman_gamma_streaming", "latent_autoregressive", "default_context",
+                "KeepLast", "KeepEach"):
         from . import inference
         return getattr(inference, name)
     if name in ("call_rule", "prod", "RuleMethodError"):

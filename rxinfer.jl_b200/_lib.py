@@ -74,6 +74,8 @@ SIGNATURES = {
     "rxg_marginalrule_gcv_yx_f32": (c_int, [c_void_p, c_int64, fp, fp, fp, fp, fp, fp, c_float, c_float, fp, fp, c_uint]),
     "rxg_rule_gcv_z_prod_f32": (c_int, [c_void_p, c_int64, fp, fp, fp, fp, c_float, c_float, fp, fp, c_uint]),
     "rxg_lgssm_smooth_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, fp, fp, fp, fp, fp, fp, fp, fp, u8p, fp, fp, fp, i32p, c_uint]),
+    "rxg_lgssm_smooth_predict_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int64, fp, fp, fp, fp, fp, fp, fp, fp, u8p, fp, fp, fp,
+                                             fp, fp, fp, fp, i32p, c_uint]),
     "rxg_lgssm_filter_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, fp, fp, fp, fp, fp, fp, fp, fp, u8p, fp, fp, fp, i32p, c_uint]),
     "rxg_lgssm_vmp_gamma_f32": (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_float, c_float, c_float, c_float, c_float, c_float, fp, fp, fp, fp, fp, c_uint]),
     "rxg_lgssm_vmp_gamma_fe_f32": (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_float, c_float, c_float, c_float, c_float, c_float, fp, fp, fp, fp, fp, fp, c_uint]),

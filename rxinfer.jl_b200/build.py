@@ -16,7 +16,7 @@ LGSSM_SHAPES = [(1, 1), (2, 1), (2, 2), (3, 3), (4, 1), (4, 2), (4, 4), (6, 6)]
 UNITS = ([("rxg_lgssm.cu", f"rxg_lgssm_d{d}m{m}", (f"-DRXG_INST_D={d}", f"-DRXG_INST_M={m}")) for d, m in reversed(LGSSM_SHAPES)] +
          [(s, s.replace(".cu", ""), ()) for s in
           ("rxg_lgssm_large.cu", "rxg_lgssm.cu", "rxg_umma_sweep.cu", "rxg_api.cu", "rxg_peer.cu", "rxg_rules.cu", "rxg_hgf.cu",
-           "rxg_lgssm_general.cu", "rxg_lgssm_generic.cu", "rxg_lar.cu", "rxg_rules_large.cu")] +
+           "rxg_lgssm_general.cu", "rxg_lgssm_generic.cu", "rxg_lar.cu", "rxg_rules_large.cu", "rxg_predict.cu")] +
          [("rxg_hostfill.cpp", "rxg_hostfill", ())])        # plain C++ (g++): host-side covariance broadcast
 SOURCES = sorted({u[0] for u in UNITS})
 HEADERS = ["rxg_internal.h", "rxg_linalg.cuh", "rxg_gain.cuh", "rxg_lgssm_common.cuh", "rxg_lgssm_shared.cuh", "rxg_lgssm_seg.cuh", "rxg_umma.cuh", "rxg_lar.cuh", os.path.join("..", "..", "include", "rxgauss.h")]

@@ -123,12 +123,10 @@ class Context:
         return torch.empty(*shape, dtype=dtype, device=f"cuda:{self.device}")
 
     # ------------------------------------------------------------------ fused sweeps
-    def lgssm(self, y, A, B, P, Q, m0, S0, *, u=None, smooth=True, mask=None, want_cov=True, want_evidence=False,
-              want_status=False, per_chain_model=False, force_per_chain_path=False, cov_shared_out=False,
-              transition_first=False, out_mean=None, out_cov=None, out_status=None, asynchronous=False):
-        """y[T, m, batch] (CUDA fp32, or pinned/pageable CPU fp32 for the host-pointer path)
-        -> dict(mean[T,d,batch], cov[T,d,d,batch] or [T,d,d], neg_log_evidence[batch], status[batch])."""
-        on_dev = y.is_cuda
+    def _sweep_args(self, y, A, B, P, Q, m0, S0, u, mask, on_dev, per_chain_model, force_per_chain_path, cov_shared_out,
+                    transition_first, asynchronous):
+        """Validation, flags and pointers shared by the fused LGSSM sweeps: returns (T, m, batch, d, flags, ptrs, mask,
+        mask_p, keep) -- ``mask`` the per-chain mask tensor or None, ``keep`` the host arrays that must outlive the call."""
         if y.dim() != 3:
             raise ValueError(f"y: expected [T, m, batch], got shape {tuple(y.shape)}")
         T, m, batch = y.shape
@@ -149,7 +147,7 @@ class Context:
             d = A.shape[0]
             self._dev(A, B, P, Q, m0, S0, u)
             ptrs = [_fp(x) for x in (A, B, P, Q, m0, S0, u)]
-            keep = None
+            keep = []
         else:
             d = np.asarray(A).shape[-1]
             keep = [_model32(x) for x in (A, B, P, Q, m0, S0)]
@@ -167,6 +165,21 @@ class Context:
             flags |= L.TRANSITION_FIRST
         if asynchronous:
             flags |= L.ASYNC
+        mask_p = ctypes.cast(c_void_p(mask.data_ptr()), L.u8p) if mask is not None else ctypes.cast(c_void_p(None), L.u8p)
+        if shared_mask is not None:
+            mask_p = shared_mask.ctypes.data_as(L.u8p)
+            keep.append(shared_mask)
+        return T, m, batch, d, flags, ptrs, mask, mask_p, keep
+
+    def lgssm(self, y, A, B, P, Q, m0, S0, *, u=None, smooth=True, mask=None, want_cov=True, want_evidence=False,
+              want_status=False, per_chain_model=False, force_per_chain_path=False, cov_shared_out=False,
+              transition_first=False, out_mean=None, out_cov=None, out_status=None, asynchronous=False):
+        """y[T, m, batch] (CUDA fp32, or pinned/pageable CPU fp32 for the host-pointer path)
+        -> dict(mean[T,d,batch], cov[T,d,d,batch] or [T,d,d], neg_log_evidence[batch], status[batch])."""
+        on_dev = y.is_cuda
+        T, m, batch, d, flags, ptrs, mask, mask_p, keep = self._sweep_args(
+            y, A, B, P, Q, m0, S0, u, mask, on_dev, per_chain_model, force_per_chain_path, cov_shared_out, transition_first,
+            asynchronous)
         mk = lambda *s, dt=torch.float32: (torch.empty(*s, dtype=dt, device=y.device) if on_dev
                                            else torch.empty(*s, dtype=dt).pin_memory())
         self._io(out_mean, "out_mean", on_dev, shape=(T, d, batch))
@@ -180,12 +193,42 @@ class Context:
         self._io(out_status, "out_status", on_dev, dtype=torch.int32, shape=(batch,))
         status = out_status if out_status is not None else (mk(batch, dt=torch.int32) if want_status else None)
         fn = self.lib.rxg_lgssm_smooth_f32 if smooth else self.lib.rxg_lgssm_filter_f32
-        mask_p = ctypes.cast(c_void_p(mask.data_ptr()), L.u8p) if mask is not None else ctypes.cast(c_void_p(None), L.u8p)
-        if shared_mask is not None:
-            mask_p = shared_mask.ctypes.data_as(L.u8p)
         st_p = ctypes.cast(c_void_p(status.data_ptr()), L.i32p) if status is not None else ctypes.cast(c_void_p(None), L.i32p)
         self._check(fn(self.h, d, m, T, batch, *ptrs, _fp(y), mask_p, _fp(mean), _fp(cov), _fp(nle), st_p, flags))
         return dict(mean=mean, cov=cov if (want_cov or need_cov) else None, neg_log_evidence=nle, status=status)
+
+    def lgssm_predict(self, y, A, B, P, Q, m0, S0, *, horizon=0, u=None, mask=None, want_cov=True, want_pred_cov=True,
+                      want_forecast_states=True, want_evidence=False, want_status=False, per_chain_model=False,
+                      force_per_chain_path=False, cov_shared_out=False, transition_first=False, asynchronous=False):
+        """Smoother + predictive distributions of the observations (``rxg_lgssm_smooth_predict_f32``).
+        y[T, m, batch] on this context's device; ``mask`` as for :meth:`lgssm` ([T, batch] per chain, or a [T] pattern
+        shared by every chain).  Returns dict(mean, cov, neg_log_evidence, status) as :meth:`lgssm` plus
+        pred_mean[T+H, m, batch], pred_cov[T+H, m, m, batch] (or [T+H, m, m] with ``cov_shared_out``), and the state
+        forecasts fc_mean[H, d, batch], fc_cov[H, d, d, batch] (or [H, d, d]); rows T.. of pred_* are the forecasts."""
+        if not y.is_cuda:
+            raise ValueError("lgssm_predict: y must be a CUDA tensor (the prediction entry takes device pointers)")
+        H = int(horizon)
+        if H < 0:
+            raise ValueError(f"horizon must be >= 0, got {horizon}")
+        T, m, batch, d, flags, ptrs, mask, mask_p, keep = self._sweep_args(
+            y, A, B, P, Q, m0, S0, u, mask, True, per_chain_model, force_per_chain_path, cov_shared_out, transition_first,
+            asynchronous)
+        mk = lambda *s, dt=torch.float32: torch.empty(*s, dtype=dt, device=y.device)
+        mean = mk(T, d, batch)
+        need_cov = want_cov or per_chain_model or force_per_chain_path or mask is not None
+        cov = (mk(T, d, d) if cov_shared_out else mk(T, d, d, batch)) if need_cov else None
+        nle = mk(batch) if want_evidence else None
+        status = mk(batch, dt=torch.int32) if want_status else None
+        pred_mean = mk(T + H, m, batch)
+        pred_cov = (mk(T + H, m, m) if cov_shared_out else mk(T + H, m, m, batch)) if want_pred_cov else None
+        fc_mean = mk(H, d, batch) if (H > 0 and want_forecast_states) else None
+        fc_cov = (mk(H, d, d) if cov_shared_out else mk(H, d, d, batch)) if (H > 0 and want_forecast_states) else None
+        st_p = ctypes.cast(c_void_p(status.data_ptr()), L.i32p) if status is not None else ctypes.cast(c_void_p(None), L.i32p)
+        self._check(self.lib.rxg_lgssm_smooth_predict_f32(self.h, d, m, T, H, batch, *ptrs, _fp(y), mask_p, _fp(mean), _fp(cov),
+                                                          _fp(nle), _fp(pred_mean), _fp(pred_cov), _fp(fc_mean), _fp(fc_cov),
+                                                          st_p, flags))
+        return dict(mean=mean, cov=cov if want_cov else None, neg_log_evidence=nle, status=status, pred_mean=pred_mean,
+                    pred_cov=pred_cov, fc_mean=fc_mean, fc_cov=fc_cov)
 
     def lgssm_filter_chunk(self, y, A, B, P, Q, prev_mean, carry_cov, *, u=None, want_evidence=False,
                            cov_shared_out=False, out_mean=None, out_cov=None):

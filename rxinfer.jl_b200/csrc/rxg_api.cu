@@ -113,6 +113,7 @@ int stage_shared_mask(rxg_ctx* ctx, int T, const uint8_t* host_mask, LgssmCall& 
 }
 void* workspace(rxg_ctx* ctx, size_t bytes) { return grow(ctx, &ctx->ws, &ctx->ws_bytes, bytes); }
 void* staging(rxg_ctx* ctx, size_t bytes) { return grow(ctx, &ctx->stage, &ctx->stage_bytes, bytes); }
+void* predict_scratch(rxg_ctx* ctx, size_t bytes) { return grow(ctx, &ctx->pred_buf, &ctx->pred_bytes, bytes); }
 
 }  // namespace rxg
 
@@ -192,6 +193,7 @@ int rxg_destroy(rxg_ctx* ctx) {
     if (ctx->d_bad) cudaFree(ctx->d_bad);
     for (int i = 0; i < 4; ++i) if (ctx->aux_buf[i]) cudaFree(ctx->aux_buf[i]);
     if (ctx->d_tmask) cudaFree(ctx->d_tmask);
+    if (ctx->pred_buf) cudaFree(ctx->pred_buf);
     if (ctx->h_bad) cudaFreeHost(ctx->h_bad);
     for (int i = 0; i < 4; ++i) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
     if (ctx->s_in) {
@@ -325,7 +327,7 @@ extern "C" int rxg_host_fill_threads(void) { return host_fill_threads(); }
 static int lgssm_entry(rxg_ctx* ctx, bool smooth, int d, int m, int T, int64_t batch, const float* A,
                        const float* B, const float* P, const float* Q, const float* m0, const float* S0,
                        const float* u, const float* y, const uint8_t* ymask, float* mean, float* cov, float* nle,
-                       int32_t* status, unsigned flags) {
+                       int32_t* status, unsigned flags, const PredictArgs* pred = nullptr) {
     if (!ctx) return RXG_ERR_BAD_ARG;
     if (d < 1 || m < 1 || T < 1 || batch < 1) return fail(ctx, RXG_ERR_BAD_ARG, "lgssm: d, m, T, batch must be >= 1");
     if (!A || !B || !P || !Q || !m0 || !S0 || !y || !mean) return fail(ctx, RXG_ERR_BAD_ARG, "lgssm: null pointer argument");
@@ -354,8 +356,11 @@ static int lgssm_entry(rxg_ctx* ctx, bool smooth, int d, int m, int T, int64_t b
         if (!cov && (ymask || per_chain_model || (flags & RXG_PATH_PER_CHAIN)))
             return fail(ctx, RXG_ERR_BAD_ARG, "lgssm: cov output required on the per-chain path");
         c.y = y; c.ymask = ymask; c.mean = mean; c.cov = cov; c.nle = nle; c.status = status;
+        // predictions without a covariance output: the family's own [T][d][d] table (where it keeps one) feeds the post-pass
+        if (pred && !cov) c.want_cov_table = true;
         int rc = begin_bad_flag(ctx);
         if (rc == RXG_OK) rc = lgssm_dispatch(ctx, c);
+        if (rc == RXG_OK && pred) rc = lgssm_predict_post(ctx, c, *pred);
         if (rc != RXG_OK) return rc;
         return end_bad_flag(ctx, !(flags & RXG_ASYNC));
     }
@@ -507,6 +512,28 @@ int rxg_lgssm_filter_f32(rxg_ctx* ctx, int d, int m, int T, int64_t batch, const
                          float* neg_log_evidence, int32_t* status, unsigned flags) {
     return lgssm_entry(ctx, false, d, m, T, batch, A, B, P, Q, m0, S0, u, y, ymask, filt_mean, filt_cov,
                        neg_log_evidence, status, flags);
+}
+
+// The smoothing sweep, unchanged (same dispatch, same outputs), followed by the prediction post-pass of rxg_predict.cu.
+int rxg_lgssm_smooth_predict_f32(rxg_ctx* ctx, int d, int m, int T, int H, int64_t batch, const float* A, const float* B,
+                                 const float* P, const float* Q, const float* m0, const float* S0, const float* u,
+                                 const float* y, const uint8_t* ymask, float* post_mean, float* post_cov,
+                                 float* neg_log_evidence, float* pred_mean, float* pred_cov, float* fc_mean, float* fc_cov,
+                                 int32_t* status, unsigned flags) {
+    if (!ctx) return RXG_ERR_BAD_ARG;
+    if (!(flags & RXG_PTR_DEVICE))
+        return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_smooth_predict takes device pointers (set RXG_PTR_DEVICE)");
+    if (H < 0) return fail(ctx, RXG_ERR_BAD_ARG, "lgssm_smooth_predict: the horizon H must be >= 0 (got %d)", H);
+    if (!pred_mean) return fail(ctx, RXG_ERR_BAD_ARG, "lgssm_smooth_predict: pred_mean is required");
+    // without post_cov the chain-independent route reads the family's own covariance table, which only the register-resident
+    // families keep: refuse the other shapes before anything runs
+    const bool per_chain_route = (flags & (RXG_MODEL_PER_CHAIN | RXG_PATH_PER_CHAIN)) || (ymask && !(flags & RXG_MASK_SHARED));
+    if (!post_cov && !per_chain_route && !lgssm_native_small(d, m))
+        return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_smooth_predict (d=%d, m=%d): this shape keeps no covariance table of its "
+                                              "own, pass post_cov", d, m);
+    const PredictArgs pa = {H, pred_mean, pred_cov, fc_mean, fc_cov};
+    return lgssm_entry(ctx, true, d, m, T, batch, A, B, P, Q, m0, S0, u, y, ymask, post_mean, post_cov,
+                       neg_log_evidence, status, flags, &pa);
 }
 
 // Streaming engine, one time-chunk.  The reference's streaming executor re-triggers a one-step graph per

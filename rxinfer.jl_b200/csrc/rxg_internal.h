@@ -55,6 +55,9 @@ struct rxg_ctx {
     size_t aux_bytes[4] = {0, 0, 0, 0};
     // persistent host threads of the host-side covariance broadcast
     void* fill_pool = nullptr;
+    // grow-only scratch of the prediction post-pass (model copies, per-step tables, forecast buffers)
+    void* pred_buf = nullptr;
+    size_t pred_bytes = 0;
 };
 
 namespace rxg {
@@ -64,6 +67,7 @@ int check_cuda(rxg_ctx* ctx, cudaError_t e, const char* what);
 // returns device pointer of >= bytes (grow-only); nullptr on failure (error recorded)
 void* workspace(rxg_ctx* ctx, size_t bytes);
 void* staging(rxg_ctx* ctx, size_t bytes);
+void* predict_scratch(rxg_ctx* ctx, size_t bytes);
 // device word that gain kernels OR a 1 into when a Cholesky pivot is non-positive (cleared by begin_bad_flag)
 int* bad_flag(rxg_ctx* ctx);
 int begin_bad_flag(rxg_ctx* ctx);                   // zero the flag on the ctx stream
@@ -123,6 +127,7 @@ int lgssm_dispatch_native(rxg_ctx* ctx, LgssmCall& c);
 // status[i] = RXG_ERR_NOT_SPD if the ctx's gain-table failure flag is set on the device, else RXG_OK
 int fill_status_from_flag(rxg_ctx* ctx, int32_t* status, int64_t n);
 bool lgssm_supported(int d, int m);
+bool lgssm_native_small(int d, int m);    // a register-resident family shape (keeps its own [T][d][d] covariance table)
 // rxg_rules_large.cu: Gaussian rule kernels for state sizes without a register-resident instantiation (d up to 64)
 bool rules_small(int d);
 bool rules_small2(int dout, int din);
@@ -134,8 +139,16 @@ int rules_large_mul_out(rxg_ctx* ctx, int64_t n, int dout, int din, const float*
                         float* mu_out, float* S_out);
 int rules_large_mul_in(rxg_ctx* ctx, int64_t n, int dout, int din, const float* A, const float* mu_out, const float* S_out,
                        float* xi_in, float* W_in, int32_t* status);
+int left_gemm_per_slice(rxg_ctx* ctx, int M, int K, int64_t N, const float* A, const float* X, float* Y, int64_t slices,
+                        int64_t x_slice, int64_t y_slice, int accumulate);
 int rules_large_convert(rxg_ctx* ctx, int64_t n, int d, int k, const float* const* v_list, const float* const* M_list,
                         float* vo, float* Mo, int32_t* status);
+// rxg_predict.cu: predictive distributions of the observations after a smoothing sweep (c = the call as dispatched)
+struct PredictArgs {
+    int H;
+    float *pred_mean, *pred_cov, *fc_mean, *fc_cov;
+};
+int lgssm_predict_post(rxg_ctx* ctx, const LgssmCall& c, const PredictArgs& p);
 // rxg_lgssm_large.cu
 int lgssm_large_dispatch(rxg_ctx* ctx, LgssmCall& c);
 bool lgssm_large_supported(int d, int m);

@@ -226,6 +226,7 @@ int embedded(rxg_ctx* ctx, LgssmCall& c, int D, int M) {
 int lgssm_generic_chain(rxg_ctx* ctx, const LgssmCall& c);   // rxg_lgssm_generic.cu
 
 bool lgssm_supported(int d, int m) { return d >= 1 && m >= 1 && d <= 64 && m <= 64; }
+bool lgssm_native_small(int d, int m) { return small_native(d, m); }
 
 int lgssm_dispatch(rxg_ctx* ctx, LgssmCall& c) {
     if (!lgssm_supported(c.d, c.m))

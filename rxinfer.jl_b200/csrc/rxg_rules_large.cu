@@ -35,16 +35,19 @@ k_ew(int64_t rows, int64_t n, const float* __restrict__ a, const float* __restri
 }
 
 // Y = op(A) X per batch slice (blockIdx.y): op(A) is M x K; transA = 0: A stored M x K row-major; 1: A stored K x M row-major.
+// MODE 0: one matrix for every slice; MODE 1: every slice its own matrix (A + slice * a_slice); MODE 2: as 1, and the
+// product is added to Y.  A template parameter, so that the MODE 0 instantiations of the rule kernels keep their registers.
 // A is staged per CTA (coalesced global reads; shared-memory row stride MMAX + 4 keeps the float4 reads aligned and the
 // transposing stores at 4-way instead of 32-way bank conflicts).  One thread = LG_NC columns (j, j + 128): every float4 of A'
 // read from shared memory feeds 4 * LG_NC FMAs -- with one column per thread the broadcast LDS.128 stream (16 per row at
 // M = 64, one shared-memory pipe for the four schedulers) costs as many cycles as the 64 FMAs it feeds.
 constexpr int LG_NC = 2;
-template <int MMAX>
+template <int MMAX, int MODE>
 __global__ void __launch_bounds__(128)
 k_left_gemm(int M, int K, int64_t N, const float* __restrict__ A, int transA, const float* __restrict__ X,
-            float* __restrict__ Y, int64_t x_slice, int64_t y_slice) {
+            float* __restrict__ Y, int64_t x_slice, int64_t y_slice, int64_t a_slice) {
     extern __shared__ __align__(16) float At[];                      // [K][LDA]: At[k][m] = op(A)(m, k), zero padded
+    if (MODE > 0) A += (int64_t)blockIdx.y * a_slice;
     constexpr int LDA = MMAX + 4;
     for (int idx = threadIdx.x; idx < K * LDA; idx += blockDim.x) At[idx] = 0.f;
     __syncthreads();
@@ -96,7 +99,7 @@ k_left_gemm(int M, int K, int64_t N, const float* __restrict__ A, int transA, co
         if (on[c]) {
 #pragma unroll
             for (int m = 0; m < MMAX; ++m)
-                if (m < M) Y[(int64_t)m * N + j[c]] = acc[c][m];
+                if (m < M) Y[(int64_t)m * N + j[c]] = MODE == 2 ? acc[c][m] + Y[(int64_t)m * N + j[c]] : acc[c][m];
         }
 }
 
@@ -236,15 +239,32 @@ static int ew(rxg_ctx* ctx, int64_t rows, int64_t n, const float* a, const float
     return check_cuda(ctx, cudaGetLastError(), "k_ew");
 }
 static int left_gemm(rxg_ctx* ctx, int M, int K, int64_t N, const float* A, int transA, const float* X, float* Y, int slices,
-                     int64_t x_slice, int64_t y_slice) {
+                     int64_t x_slice, int64_t y_slice, int64_t a_slice = 0, int accumulate = 0) {
     const dim3 grid((unsigned)((N + 128 * LG_NC - 1) / (128 * LG_NC)), (unsigned)slices);
     const int mmax = M <= 16 ? 16 : (M <= 32 ? 32 : 64);
     const size_t smem = (size_t)K * (mmax + 4) * sizeof(float);
-    if (mmax == 16) k_left_gemm<16><<<grid, 128, smem, ctx->stream>>>(M, K, N, A, transA, X, Y, x_slice, y_slice);
-    else if (mmax == 32) k_left_gemm<32><<<grid, 128, smem, ctx->stream>>>(M, K, N, A, transA, X, Y, x_slice, y_slice);
-    else k_left_gemm<64><<<grid, 128, smem, ctx->stream>>>(M, K, N, A, transA, X, Y, x_slice, y_slice);
+    const int mode = a_slice == 0 ? 0 : (accumulate ? 2 : 1);
+#define RXG_LG(MM, MO) k_left_gemm<MM, MO><<<grid, 128, smem, ctx->stream>>>(M, K, N, A, transA, X, Y, x_slice, y_slice, a_slice)
+#define RXG_LG_MODES(MM) do { if (mode == 0) RXG_LG(MM, 0); else if (mode == 1) RXG_LG(MM, 1); else RXG_LG(MM, 2); } while (0)
+    if (mmax == 16) RXG_LG_MODES(16);
+    else if (mmax == 32) RXG_LG_MODES(32);
+    else RXG_LG_MODES(64);
+#undef RXG_LG_MODES
+#undef RXG_LG
     ctx->launches += 1;
     return check_cuda(ctx, cudaGetLastError(), "k_left_gemm");
+}
+// Y[s] (+)= A[s] X[s] for `slices` slices with one row-major M x K matrix per slice (a_slice = M K); the grid's y dimension
+// caps one launch at 65 535 slices
+int left_gemm_per_slice(rxg_ctx* ctx, int M, int K, int64_t N, const float* A, const float* X, float* Y, int64_t slices,
+                        int64_t x_slice, int64_t y_slice, int accumulate) {
+    for (int64_t s0 = 0; s0 < slices; s0 += 65535) {
+        const int64_t ns = slices - s0 < 65535 ? slices - s0 : 65535;
+        int rc = left_gemm(ctx, M, K, N, A + s0 * M * K, 0, X + s0 * x_slice, Y + s0 * y_slice, (int)ns, x_slice, y_slice,
+                           (int64_t)M * K, accumulate);
+        if (rc != RXG_OK) return rc;
+    }
+    return RXG_OK;
 }
 static int cholinv_warp(rxg_ctx* ctx, int64_t n, int d, int k, const RuleList& in, float* vo, float* Mo, int32_t* status) {
     // 8 messages per CTA (one 32-byte sector per element) unless that leaves room for only one CTA per SM (d > 57): then 6,

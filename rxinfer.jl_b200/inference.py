@@ -16,6 +16,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
+from . import _lib as L
 from .context import Context
 from .distributions import GammaShapeRate, MvNormalMeanCovariance, NormalMeanVariance
 
@@ -35,6 +36,7 @@ class linear_gaussian_ssm_smoothing:
     per_chain: bool = False     # model matrices carry a trailing [batch] axis (CUDA tensors)
     u: object = None            # constant offset: x[t] ~ MvNormal(A x[t-1] + u, P)  (`+` with a PointMass)
     prior_on_previous_state: bool = False   # x_prior ~ x0; x[1] ~ N(A x_prior + u, P)  (mlgssm_test.jl:8-17)
+    horizon: int = 0            # forecast steps x[T+1..T+H], o[1..H] ~ N(B x[T+k], Q) (model_1, prediction_tests.jl:197-213)
 
 
 @dataclass
@@ -89,6 +91,32 @@ class latent_autoregressive:
     init_theta_precision: float = 1.0       # q(theta) = N(0, I / init_theta_precision)
 
 
+class KeepLast:
+    """``predictvars`` / ``returnvars`` marker: keep the result of the last iteration (the reference's ``KeepLast()``)."""
+
+    def __eq__(self, other):
+        return isinstance(other, KeepLast)
+
+    def __hash__(self):
+        return hash(KeepLast)
+
+    def __repr__(self):
+        return "KeepLast()"
+
+
+class KeepEach:
+    """``KeepEach()``: keep the result of every iteration.  Predictions per iteration are outside the batched hot path."""
+
+    def __eq__(self, other):
+        return isinstance(other, KeepEach)
+
+    def __hash__(self):
+        return hash(KeepEach)
+
+    def __repr__(self):
+        return "KeepEach()"
+
+
 @dataclass
 class InferenceResult:
     """``InferenceResult`` (/root/reference/src/inference/batch.jl:18-24)."""
@@ -97,9 +125,10 @@ class InferenceResult:
     model: object = None
     error: object = None
     history: dict = field(default_factory=dict)
+    predictions: dict = field(default_factory=dict)
 
 
-_UNSUPPORTED = ("constraints", "meta", "callbacks", "annotations", "predictvars", "events", "uselock",
+_UNSUPPORTED = ("constraints", "meta", "callbacks", "annotations", "events", "uselock",
                 "postprocess", "trace", "benchmark", "free_energy_diagnostics")
 _ctx_cache: dict = {}
 
@@ -113,11 +142,44 @@ def default_context(device=None) -> Context:
     return ctx
 
 
+def _predict_keys(predictvars, model, data):
+    """Which predictive distributions to return: ``predictvars`` normalised as the reference does
+    (src/inference/batch.jl:203-246) -- a bare ``KeepLast()`` stands for every data variable, and a ``y`` with missing
+    entries is always predicted.  Only ``KeepLast`` predictions of the LGSSM smoother's ``y`` (observations) and ``o``
+    (the ``horizon`` forecasts) run on the batched path; every other form raises ``NotImplementedError``."""
+    if isinstance(predictvars, (KeepLast, KeepEach)) and data is None:
+        raise ValueError(f"`predictvar` is specified as `{predictvars!r}`, but `data` is not provided. Make sure to provide "
+                         "`data` or specify `predictvars` explicitly.")       # the reference's error (batch.jl:210-213)
+    if not isinstance(model, linear_gaussian_ssm_smoothing) or isinstance(model, linear_gaussian_ssm_filtering):
+        raise NotImplementedError("predictvars: only the smoothing LGSSM predicts on the batched hot path; "
+                                  "run this call through stock ReactiveMP")
+    if data is None:
+        raise NotImplementedError("predictvars / horizon: predictions of the streaming engine (datastream) are outside the "
+                                  "batched hot path; pass `data`")
+    if isinstance(predictvars, KeepLast):
+        predictvars = {k: KeepLast() for k in data if k != "ymask"}
+    if not isinstance(predictvars, dict):
+        raise NotImplementedError(f"predictvars={predictvars!r}: expected KeepLast() or a dict of KeepLast() values; "
+                                  "run this call through stock ReactiveMP")
+    for k, v in predictvars.items():
+        if k not in ("y", "o"):
+            raise NotImplementedError(f"predictvars: {k!r} is not a data variable of the LGSSM (y, o)")
+        if not isinstance(v, KeepLast):
+            raise NotImplementedError(f"predictvars[{k!r}] = {v!r}: only KeepLast() predictions run on the batched path")
+    if "o" in predictvars and model.horizon <= 0:
+        raise ValueError("predictvars: 'o' (the forecasts) needs linear_gaussian_ssm_smoothing(..., horizon > 0)")
+    keys = set(predictvars)
+    mask = data.get("ymask")
+    if mask is not None and not bool((torch.as_tensor(mask) != 0).all()):
+        keys.add("y")                                  # data with missing entries are predicted (batch.jl:231-245)
+    return keys
+
+
 def infer(*, model, iterations=None, free_energy=False, returnvars=None, options=None,
           initialization=None, autoupdates=None, keephistory=None, historyvars=None,
           catch_exception=False, showprogress=False, session=None, warn=True, allow_node_contraction=False,
           context: Context | None = None, cov_shared_out=False, data=None, datastream=None, autostart=True,
-          batch=None, **kwargs):
+          batch=None, predictvars=None, **kwargs):
     """Batched ``infer``.  ``data = {"y": tensor[T, m, batch]}`` (CUDA fp32, or CPU for the
     host-staged path).  Returns ``posteriors["x"]`` as a batched ``MvNormalMeanCovariance``.
 
@@ -136,6 +198,12 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             raise NotImplementedError(f"options {sorted(bad)} are outside the batched hot path")
     if data is not None and datastream is not None:
         raise ValueError("`data` and `datastream` are mutually exclusive")    # reference: inference.jl argument check
+    horizon = getattr(model, "horizon", 0) if isinstance(model, linear_gaussian_ssm_smoothing) else 0
+    if isinstance(model, linear_gaussian_ssm_filtering) and horizon:
+        raise NotImplementedError("horizon > 0 belongs to the smoothing LGSSM")
+    predict = None
+    if predictvars is not None or horizon > 0:
+        predict = _predict_keys(predictvars if predictvars is not None else {}, model, data)
     if data is None:
         if datastream is None and autoupdates is None:
             raise ValueError("either `data` or `datastream` (or `autoupdates` for a push-driven engine) is required")
@@ -161,6 +229,29 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             if iterations not in (None, 1):
                 raise NotImplementedError("iterations > 1 on a tree-structured BP model is a no-op in the reference; "
                                           "KeepEach() results are outside the hot path")
+            if predict is not None:
+                r = ctx.lgssm_predict(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], horizon=horizon,
+                                      u=model.u, mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain,
+                                      cov_shared_out=cov_shared_out, transition_first=model.prior_on_previous_state,
+                                      want_status=True)
+                bad = r["status"] != 0
+                if bool(bad.any()):      # e.g. a chain whose D_t = Q - B S_s B' is not SPD has no usable prediction
+                    codes = sorted({L.STATUS_NAMES.get(int(c), str(int(c))) for c in r["status"][bad].unique().tolist()})
+                    raise L.RxGaussError(L.RXG_ERR_NOT_SPD if "NOT_SPD" in codes else int(r["status"][bad][0]),
+                                         f"predictions: {int(bad.sum())} of {bad.numel()} chains flagged {codes} (NOT_SPD: "
+                                         "Q - B S_s B' is not SPD, the observations dominate beyond the fp32 posterior "
+                                         "covariances)")
+                T = y.shape[0]
+                mean, cov = r["mean"], r["cov"]
+                if horizon > 0:          # posteriors["x"] covers x[1..T+H], as model_1's x covers n + 2 states
+                    mean, cov = torch.cat([mean, r["fc_mean"]]), torch.cat([cov, r["fc_cov"]])
+                preds = {}
+                if "y" in predict:
+                    preds["y"] = MvNormalMeanCovariance(r["pred_mean"][:T], r["pred_cov"][:T])
+                if "o" in predict:
+                    preds["o"] = MvNormalMeanCovariance(r["pred_mean"][T:], r["pred_cov"][T:])
+                return InferenceResult(posteriors={"x": MvNormalMeanCovariance(mean, cov)}, predictions=preds,
+                                       free_energy=r["neg_log_evidence"], model=model)
             r = ctx.lgssm(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], u=model.u, smooth=True, mask=mask,
                           want_evidence=free_energy, per_chain_model=model.per_chain, cov_shared_out=cov_shared_out,
                           transition_first=model.prior_on_previous_state)

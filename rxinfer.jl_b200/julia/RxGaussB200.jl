@@ -173,6 +173,10 @@ rule_gcv_z_prod(ctx, n, myx, Vyx, mzp, vzp, kappa, omega, mz, vz, fl) =
 const SWEEP = (Ptr{Cvoid}, Cint, Cint, Cint, Int64, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{UInt8}, F32P, F32P, F32P, Ptr{Int32}, Cuint)
 lgssm_smooth(ctx, d, m, T, batch, A, B, P, Q, m0, S0, u, y, mask, mean, cov, nle, st, fl) =
     check(ctx, ccall((:rxg_lgssm_smooth_f32, LIB), Cint, SWEEP, ctx.handle, d, m, T, batch, A, B, P, Q, m0, S0, u, y, mask, mean, cov, nle, st, fl))
+const PREDICT = (Ptr{Cvoid}, Cint, Cint, Cint, Cint, Int64, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{UInt8}, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Int32}, Cuint)
+lgssm_smooth_predict(ctx, d, m, T, H, batch, A, B, P, Q, m0, S0, u, y, mask, mean, cov, nle, pm, pc, fm, fc, st, fl) =
+    check(ctx, ccall((:rxg_lgssm_smooth_predict_f32, LIB), Cint, PREDICT, ctx.handle, d, m, T, H, batch, A, B, P, Q, m0, S0, u, y, mask,
+                     mean, cov, nle, pm, pc, fm, fc, st, fl))
 lgssm_filter(ctx, d, m, T, batch, A, B, P, Q, m0, S0, u, y, mask, mean, cov, nle, st, fl) =
     check(ctx, ccall((:rxg_lgssm_filter_f32, LIB), Cint, SWEEP, ctx.handle, d, m, T, batch, A, B, P, Q, m0, S0, u, y, mask, mean, cov, nle, st, fl))
 lgssm_filter_chunk(ctx, d, m, T, batch, A, B, P, Q, u, prev_mean, carry_cov, y, mean, cov, nle, fl) =
@@ -552,6 +556,48 @@ function sweep(ctx::Context, p::LGSSMPattern, y::Array{Float32, 3}; mask::Union{
     return mean, cov, free_energy ? nle : nothing, status ? st : nothing
 end
 
+"""
+    sweep_predict(ctx, p::LGSSMPattern, y; mask = nothing, free_energy = false)
+
+The smoothing sweep plus the predictive distributions of the observations (`rxg_lgssm_smooth_predict_f32`, device
+pointers): the reference's message toward every `y[t]` (`result.predictions[:y]`, src/inference/batch.jl:203-246).
+Returns `(mean[batch, d, T], cov[batch, d, d, T], neg_log_evidence or nothing, pred_mean[batch, m, T], pred_cov[batch, m, m, T])`.
+"""
+function sweep_predict(ctx::Context, p::LGSSMPattern, y::Array{Float32, 3}; mask::Union{Nothing, Matrix{UInt8}} = nothing,
+                       free_energy::Bool = false)
+    batch, m, T = size(y)
+    d = size(p.A, 1)
+    dy = upload(ctx, y)
+    dmask = mask === nothing ? C_NULL : Lib.device_alloc(ctx, sizeof(mask))
+    mask === nothing || GC.@preserve mask Lib.memcpy_h2d(ctx, dmask, Ptr{Cvoid}(pointer(mask)), sizeof(mask))
+    mean, cov = DeviceArray(ctx, batch, d, T), DeviceArray(ctx, batch, d, d, T)
+    pm, pc = DeviceArray(ctx, batch, m, T), DeviceArray(ctx, batch, m, m, T)
+    nle = free_energy ? DeviceArray(ctx, batch) : nothing
+    st = Lib.device_alloc(ctx, 4 * batch)
+    Ar, Br, Pr, Qr, S0r = rowmajor32(p.A), rowmajor32(p.B), rowmajor32(p.P), rowmajor32(p.Q), rowmajor32(p.S0)
+    m0r = rowmajor32(p.m0)
+    ur = p.u === nothing ? Float32[] : rowmajor32(p.u)
+    flags = RXG_PTR_DEVICE | (p.transition_first ? RXG_TRANSITION_FIRST : UInt32(0))
+    try
+        GC.@preserve Ar Br Pr Qr S0r m0r ur begin
+            Lib.lgssm_smooth_predict(ctx, d, m, T, 0, batch, pointer(Ar), pointer(Br), pointer(Pr), pointer(Qr), pointer(m0r),
+                                     pointer(S0r), p.u === nothing ? NULLF : pointer(ur), dy.ptr, Ptr{UInt8}(dmask), mean.ptr, cov.ptr,
+                                     nle === nothing ? NULLF : nle.ptr, pm.ptr, pc.ptr, NULLF, NULLF, Ptr{Int32}(st), flags)
+        end
+        # a chain whose Q - B S_s B' is not SPD (observations dominating beyond the fp32 posterior covariances) has no usable
+        # prediction: fail loudly instead of returning it
+        status = Vector{Int32}(undef, batch)
+        GC.@preserve status Lib.memcpy_d2h(ctx, Ptr{Cvoid}(pointer(status)), st, 4 * batch)
+        nbad = count(!=(RXG_OK), status)
+        nbad == 0 || throw(RxGaussError(first(filter(!=(RXG_OK), status)),
+                                        "predictions: $nbad of $batch chains flagged (RXG_ERR_NOT_SPD: Q - B S_s B' is not SPD)"))
+    finally
+        mask === nothing || Lib.device_free(ctx, dmask)
+        Lib.device_free(ctx, st)
+    end
+    return download(mean), download(cov), nle === nothing ? nothing : download(nle), download(pm), download(pc)
+end
+
 """HGF filter on host data `y[batch, T]`; returns `out[batch, 4, T]` = (m_x, v_x, m_z, v_z) and, on request, the
 Bethe free energy `[batch, iterations, T]` (its mean over T is `free_energy_history`, hgf_tests.jl:112-119)."""
 function hgf_filter(ctx::Context, p::HGFPattern, y::Matrix{Float32}; iterations::Integer = 1, free_energy::Bool = false)
@@ -736,7 +782,11 @@ function infer_batched(; model, data, iterations = nothing, free_energy = false,
     ys = data.y
     stock() = map(b -> RxInfer.infer(; model, data = (y = ys[b],), iterations, free_energy, constraints, initialization, returnvars, kwargs...),
                   collect(eachindex(ys)))
-    any(k -> haskey(kwargs, k), FALLBACK_KEYWORDS) && return stock()
+    # `predictvars = (y = KeepLast(),)` is the one prediction request of the fused path; any other form (forecast nodes, KeepEach,
+    # other variables) stays in the fallback list
+    pv = get(kwargs, :predictvars, nothing)
+    predict_y = pv isa NamedTuple && keys(pv) == (:y,) && pv.y isa RxInfer.KeepLast
+    any(k -> haskey(kwargs, k) && !(k === :predictvars && predict_y), FALLBACK_KEYWORDS) && return stock()
     (constraints === nothing && initialization === nothing) || return stock()      # BP on a tree needs neither
     (iterations === nothing || iterations == 1) || return stock()                  # KeepEach on BP is per-iteration output
     has_missing = any(s -> any(ismissing, s), ys)
@@ -744,7 +794,16 @@ function infer_batched(; model, data, iterations = nothing, free_energy = false,
     pattern === nothing && return stock()
     RxInfer.ReactiveMP.is_predefined_node(MvNormalMeanCovariance)                 # touches the node registry: fails early if RxInfer is broken
     y, mask = has_missing ? pack_missing(ys) : (pack(ys), nothing)
-    μ, Σ, F, _ = sweep(context, pattern, y; mask, free_energy = free_energy !== false)
+    # the reference predicts every data variable with missing entries (batch.jl:222-227) and what predictvars asks for
+    predictions = Dict{Symbol, Any}()
+    if has_missing || predict_y
+        μ, Σ, F, ŷ, Ŝ = sweep_predict(context, pattern, y; mask, free_energy = free_energy !== false)
+        predictions[:y] = materialize ?
+            [MvNormalMeanCovariance(Float64.(ŷ[b, :, t]), Float64.(Ŝ[b, :, :, t])) for t in 1:size(ŷ, 3), b in 1:size(ŷ, 1)] :
+            (mean = ŷ, cov = Ŝ)
+    else
+        μ, Σ, F, _ = sweep(context, pattern, y; mask, free_energy = free_energy !== false)
+    end
     batch, d, T = size(μ)
     posteriors = if materialize
         Dict(:x => [MvNormalMeanCovariance(Float64.(μ[b, :, t]), Float64.(Σ[b, :, :, t])) for t in 1:T, b in 1:batch])
@@ -752,7 +811,7 @@ function infer_batched(; model, data, iterations = nothing, free_energy = false,
         Dict(:x => (mean = μ, cov = Σ))                # structure of arrays: (batch, d, T) / (batch, d, d, T)
     end
     fe = free_energy === false ? nothing : Float64.(F)
-    return RxInfer.InferenceResult(posteriors, Dict{Symbol, Any}(), fe, model, nothing)
+    return RxInfer.InferenceResult(posteriors, predictions, fe, model, nothing)
 end
 
 # ---------------------------------------------------------------------------------------------- 5. streaming engine in time-chunks
