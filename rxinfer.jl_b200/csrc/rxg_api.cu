@@ -336,7 +336,10 @@ static int lgssm_entry(rxg_ctx* ctx, bool smooth, int d, int m, int T, int64_t b
     if (!lgssm_supported(d, m))
         return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm: d and m must be in 1..64 (got d=%d, m=%d)", d, m);
     const bool per_chain_model = (flags & RXG_MODEL_PER_CHAIN) != 0;
-    if ((flags & RXG_COV_SHARED_OUT) && (per_chain_model || (flags & RXG_PATH_PER_CHAIN) || ymask))
+    // a shared missing-data pattern (RXG_MASK_SHARED) keeps the covariances chain independent: only a per-chain mask
+    // rules the de-duplicated output out
+    const bool per_chain_mask = ymask && !(flags & RXG_MASK_SHARED);
+    if ((flags & RXG_COV_SHARED_OUT) && (per_chain_model || (flags & RXG_PATH_PER_CHAIN) || per_chain_mask))
         return fail(ctx, RXG_ERR_BAD_ARG, "lgssm: RXG_COV_SHARED_OUT needs the shared-model gain-table path");
     RXG_CUDA(ctx, cudaSetDevice(ctx->device));
 
