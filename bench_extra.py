@@ -4,6 +4,7 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
 
   python bench_extra.py [--which per_chain,filter,hgf,rules,vmp,scaling_T]
   python bench_extra.py --which predict      (opt-in: observation predictions / forecasts after the smoother)
+  python bench_extra.py --which inputs       (opt-in: known per-step inputs u[t], shared and per-chain sequences)
 """
 from __future__ import annotations
 
@@ -84,6 +85,59 @@ def bench_predict(ctx, peak):
         torch.cuda.empty_cache()
 
 
+def bench_inputs(ctx, peak):
+    """Smoothing with known per-step inputs at config-2 size (notebook model, d = m = 4, T = 1000, 65 536 chains): no input,
+    constant u, a shared sequence and a per-chain sequence (checkpoint and stash at CPT 2), each as kernel time (the
+    sweep kernel's CUDA events, rxg_profile_last_ms) and call time; plus the d = 64 linearity route at batch 4096.
+    Algorithmic bytes per (chain, step): read y (4 m) [+ u (4 d) for a per-chain sequence], write the smoothed mean (4 d)
+    and covariance (4 d^2)."""
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(12)
+    nb = notebook_model_f32()
+    dn = dense_model_f32(64)
+    cases = [("config-2, no input", nb, 65536, None, 0), ("config-2, constant u", nb, 65536, "const", 0),
+             ("config-2, shared sequence", nb, 65536, "shared", 0),
+             ("config-2, per-chain sequence, CPT 2 checkpoint", nb, 65536, "chain", 0),
+             ("config-2, per-chain sequence, CPT 2 stash", nb, 65536, "chain", 1),
+             ("d = 64 dense, per-chain sequence (linearity route)", dn, 4096, "chain", 0),
+             ("d = 64 dense, no input", dn, 4096, None, 0)]
+    T = 1000
+    for name, mod, batch, kind, variant in cases:
+        d, m = mod["A"].shape[0], mod["B"].shape[0]
+        y = torch.randn(T, m, batch, device="cuda", generator=g) * 3.3
+        args = [mod[k] for k in ("A", "B", "P", "Q", "m0", "S0")]
+        u = (0.3 * np.ones(d)).astype(np.float32) if kind == "const" else None
+        inputs = None
+        if kind == "shared":
+            inputs = (0.3 * np.random.default_rng(1).standard_normal((T, d))).astype(np.float32)
+        elif kind == "chain":
+            inputs = torch.randn(T, d, batch, device="cuda", generator=g) * 0.3
+        ctx.set_option("sweep_variant", variant)
+        out_mean = torch.empty(T, d, batch, device="cuda")
+        out_cov = torch.empty(T, d, d, batch, device="cuda")
+        call = lambda: ctx.lgssm(y, *args, u=u, inputs=inputs, out_mean=out_mean, out_cov=out_cov)
+        ctx.set_profiling(True)
+        call_ms, kern_ms = [], []
+        for _ in range(3):
+            call_ms.append(timed(call))
+            kms = []
+            for _ in range(5):
+                call()
+                kms.append(ctx.profile_last_ms()[0])
+            kern_ms.append(float(np.median(kms)))
+        ctx.set_profiling(False)
+        ctx.set_option("sweep_variant", 0)
+        kms, cms = float(np.median(kern_ms)), float(np.median(call_ms))
+        byts = 4 * T * batch * (m + d + d * d + (d if kind == "chain" else 0))
+        print(json.dumps({"what": "lgssm smoothing with inputs: " + name, "d": d, "m": m, "T": T, "batch": batch,
+                          "kernel_ms": kms, "call_ms": cms, "algorithmic_GB": byts / 1e9,
+                          "algorithmic_bytes_per_chain_step": byts / (T * batch),
+                          "kernel_frac_of_peak_hbm": (byts / (kms * 1e-3)) / (peak * 1e9),
+                          "peak_hbm_gbs": peak, "gpu": gname, "power_limit": plim}), flush=True)
+        del y, inputs, out_mean, out_cov
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -93,6 +147,8 @@ def main():
     peak, _ = peaks()
     if "predict" in which:
         bench_predict(ctx, peak)
+    if "inputs" in which:
+        bench_inputs(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

@@ -61,10 +61,18 @@ enum rxg_flags {
     RXG_TRANSITION_FIRST = 1u << 5, /* the prior sits one transition before the first datum      */
     RXG_COV_REPLICATE   = 1u << 6, /* all-gather: covariances are chain independent (shared model,
                                       no missing data) -- replicate them locally, gather only means */
-    RXG_MASK_SHARED     = 1u << 7  /* ymask is ONE pattern for all chains: a HOST array ymask[T] (like the model
+    RXG_MASK_SHARED     = 1u << 7, /* ymask is ONE pattern for all chains: a HOST array ymask[T] (like the model
                                       matrices).  The covariances stay chain independent, so the call stays on the
                                       gain-table path (a per-chain mask forces the per-chain covariance recursion,
                                       ~2.7x slower at d = 4).  y at masked steps is ignored but must be finite.   */
+    /* Known per-step inputs (control / exogenous terms): `u` is a SEQUENCE, x[t] ~ N(A x[t-1] + u[t], P).  Row t
+     * (0-based) enters the transition into x[t]; row 0 is read only with RXG_TRANSITION_FIRST.  A masked step still
+     * applies its input.  Inputs move only the means: covariances (and gain tables) are those of the call without
+     * inputs.  A constant offset has to be folded into the sequence by the caller.  Both flags together: BAD_ARG.  */
+    RXG_U_SEQ_SHARED    = 1u << 8, /* u is ONE sequence for every chain: a HOST array u[rows][d] (also with
+                                      RXG_MODEL_PER_CHAIN)                                                        */
+    RXG_U_SEQ_CHAIN     = 1u << 9  /* u is a DEVICE array u[rows][d][batch] (shared or per-chain model); needs
+                                      RXG_PTR_DEVICE (host-pointer calls return RXG_ERR_UNSUPPORTED)              */
 };
 
 /* Per-context options (rxg_set_option).  The RXG_* environment variables of the same name are read
@@ -286,6 +294,8 @@ int rxg_rule_gcv_z_prod_f32(rxg_ctx*, int64_t n, const float* m_yx, const float*
  *          [ref: missing data semantics docs/src/manuals/inference/static.md:98-125];
  *          A,B,P,Q,m0,S0,u row-major, shared HOST arrays (or device [..][batch] arrays with
  *          RXG_MODEL_PER_CHAIN).
+ *          With RXG_U_SEQ_SHARED / RXG_U_SEQ_CHAIN, u is a per-step input sequence of T rows instead
+ *          (u[T][d] host, or u[T][d][batch] device; see the flags): x[t] ~ N(A x[t-1] + u[t], P).
  * Outputs: post_mean[T][d][batch], post_cov[T][d][d][batch]  (== posteriors[:x], as
  *          MvNormalMeanCovariance) [ref: src/inference/batch.jl:475-481];
  *          neg_log_evidence[batch] or NULL (== Bethe free energy on this tree
@@ -314,7 +324,9 @@ int rxg_lgssm_smooth_f32(rxg_ctx*, int d, int m, int T, int64_t batch, const flo
  * shapes return RXG_ERR_UNSUPPORTED before anything runs.  Device pointers only
  * (RXG_ERR_UNSUPPORTED otherwise); H < 0 or pred_mean NULL -> RXG_ERR_BAD_ARG; a chain whose D_t is not SPD gets
  * RXG_ERR_NOT_SPD in status[b] (shared model: every chain, and the call returns RXG_ERR_NOT_SPD).  As for the
- * smoother, y at masked steps is ignored but must be finite.                                     */
+ * smoother, y at masked steps is ignored but must be finite.
+ * With RXG_U_SEQ_SHARED / RXG_U_SEQ_CHAIN the input sequence has T + H rows: forecast k = 1..H steps
+ * x_k = A x_{k-1} + u[T + k - 1].  The predictions at steps t < T depend only on (y, mu_s, S_s).  */
 int rxg_lgssm_smooth_predict_f32(rxg_ctx*, int d, int m, int T, int H, int64_t batch, const float* A,
                                  const float* B, const float* P, const float* Q, const float* m0,
                                  const float* S0, const float* u, const float* y, const uint8_t* ymask,
@@ -323,7 +335,8 @@ int rxg_lgssm_smooth_predict_f32(rxg_ctx*, int d, int m, int T, int H, int64_t b
                                  int32_t* status, unsigned flags);
 /* Forward half only (filtering) -- what the streaming engine computes per datum with
  * @autoupdates x_min_t_mean, x_min_t_cov = mean_cov(q(x_t))
- * [ref: src/inference/streaming.jl:344-388; src/inference/autoupdates.jl:614-659; ipynb:199-216]. */
+ * [ref: src/inference/streaming.jl:344-388; src/inference/autoupdates.jl:614-659; ipynb:199-216].
+ * RXG_U_SEQ_SHARED / RXG_U_SEQ_CHAIN as for rxg_lgssm_smooth_f32 (T rows).                        */
 int rxg_lgssm_filter_f32(rxg_ctx*, int d, int m, int T, int64_t batch, const float* A,
                          const float* B, const float* P, const float* Q, const float* m0,
                          const float* S0, const float* u, const float* y, const uint8_t* ymask,
@@ -373,7 +386,9 @@ int rxg_hgf_filter_fe_f32(rxg_ctx*, int T, int64_t batch, int iters, float kappa
  *                                       model);  out: covariance of q(x_{t0+Tc-1})
  * Model per datum: x_t ~ N(A x_{t-1} + u, P), y_t ~ N(B x_t, Q) (transition first).  Chunking is
  * exact: any split of the stream gives the same posteriors as one call (up to the fp32 rounding of
- * the carried covariance).  Shared model, no mask; device pointers; always synchronous.          */
+ * the carried covariance).  Shared model, no mask; device pointers; always synchronous.
+ * RXG_U_SEQ_SHARED / RXG_U_SEQ_CHAIN: u is the chunk's input sequence, Tc rows (u[Tc][d] host or
+ * u[Tc][d][batch] device); the chunk model is transition first, so row 0 is used.                 */
 int rxg_lgssm_filter_chunk_f32(rxg_ctx*, int d, int m, int Tc, int64_t batch, const float* A,
                                const float* B, const float* P, const float* Q, const float* u,
                                const float* prev_mean, float* carry_cov, const float* y,
@@ -469,7 +484,8 @@ int rxg_peer_allgather_f32(rxg_ctx*, int64_t n_local, const float* local, float*
  * RXG_COV_REPLICATE (shared model, no mask): only the means cross NVLink, the other ranks' covariance slabs are
  * replicated locally from the [T][d][d] table concurrently with the sweep (gathered_cov[g != rank] may be NULL);
  * the buffers end up bit-identical to the full gather.  neg_log_evidence / status are local ([b_local]).
- * A caller must not start the next gather into the same buffers before every rank has consumed the result.   */
+ * A caller must not start the next gather into the same buffers before every rank has consumed the result.
+ * RXG_U_SEQ_SHARED / RXG_U_SEQ_CHAIN are refused with RXG_ERR_UNSUPPORTED before anything runs.              */
 int rxg_lgssm_smooth_gather_f32(rxg_ctx*, int d, int m, int T, int64_t batch_local, const float* A,
                                 const float* B, const float* P, const float* Q, const float* m0,
                                 const float* S0, const float* u, const float* y, const uint8_t* ymask,

@@ -25,6 +25,8 @@ PATH_PER_CHAIN = 1 << 4
 TRANSITION_FIRST = 1 << 5
 COV_REPLICATE = 1 << 6
 MASK_SHARED = 1 << 7
+U_SEQ_SHARED = 1 << 8      # u is one input sequence for every chain, a host array [rows, d]
+U_SEQ_CHAIN = 1 << 9       # u is a per-chain input sequence, a device array [rows, d, batch]
 
 fp = POINTER(c_float)
 u8p = POINTER(c_uint8)

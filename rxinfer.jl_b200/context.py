@@ -123,8 +123,26 @@ class Context:
         return torch.empty(*shape, dtype=dtype, device=f"cuda:{self.device}")
 
     # ------------------------------------------------------------------ fused sweeps
+    def _inputs(self, inputs, u, rows, d, batch):
+        """Known per-step inputs (``inputs=``): a CPU / numpy [rows, d] array is one sequence for every chain
+        (RXG_U_SEQ_SHARED), a CUDA [rows, d, batch] tensor one per chain (RXG_U_SEQ_CHAIN).  Row t enters the transition
+        into x[t].  Returns (flag, pointer, kept array) or None."""
+        if inputs is None:
+            return None
+        if u is not None:
+            raise ValueError("pass either a constant offset u or an input sequence inputs, not both "
+                             "(fold the constant into the sequence)")
+        if isinstance(inputs, torch.Tensor) and inputs.is_cuda:
+            self._io(inputs, "inputs", True, shape=(rows, d, batch))
+            return L.U_SEQ_CHAIN, _fp(inputs), inputs
+        a = np.ascontiguousarray(np.asarray(inputs.cpu() if isinstance(inputs, torch.Tensor) else inputs, dtype=np.float32))
+        if a.shape != (rows, d):
+            raise ValueError(f"inputs: expected a host array of shape {(rows, d)} (or a CUDA tensor {(rows, d, batch)}), "
+                             f"got {a.shape}")
+        return L.U_SEQ_SHARED, a.ctypes.data_as(L.fp), a
+
     def _sweep_args(self, y, A, B, P, Q, m0, S0, u, mask, on_dev, per_chain_model, force_per_chain_path, cov_shared_out,
-                    transition_first, asynchronous):
+                    transition_first, asynchronous, inputs=None, input_rows=None):
         """Validation, flags and pointers shared by the fused LGSSM sweeps: returns (T, m, batch, d, flags, ptrs, mask,
         mask_p, keep) -- ``mask`` the per-chain mask tensor or None, ``keep`` the host arrays that must outlive the call."""
         if y.dim() != 3:
@@ -165,21 +183,28 @@ class Context:
             flags |= L.TRANSITION_FIRST
         if asynchronous:
             flags |= L.ASYNC
+        seq = self._inputs(inputs, u, T if input_rows is None else input_rows, d, batch)
+        if seq is not None:
+            flags |= seq[0]
+            ptrs[-1] = seq[1]
+            keep.append(seq[2])
         mask_p = ctypes.cast(c_void_p(mask.data_ptr()), L.u8p) if mask is not None else ctypes.cast(c_void_p(None), L.u8p)
         if shared_mask is not None:
             mask_p = shared_mask.ctypes.data_as(L.u8p)
             keep.append(shared_mask)
         return T, m, batch, d, flags, ptrs, mask, mask_p, keep
 
-    def lgssm(self, y, A, B, P, Q, m0, S0, *, u=None, smooth=True, mask=None, want_cov=True, want_evidence=False,
-              want_status=False, per_chain_model=False, force_per_chain_path=False, cov_shared_out=False,
+    def lgssm(self, y, A, B, P, Q, m0, S0, *, u=None, inputs=None, smooth=True, mask=None, want_cov=True,
+              want_evidence=False, want_status=False, per_chain_model=False, force_per_chain_path=False, cov_shared_out=False,
               transition_first=False, out_mean=None, out_cov=None, out_status=None, asynchronous=False):
         """y[T, m, batch] (CUDA fp32, or pinned/pageable CPU fp32 for the host-pointer path)
-        -> dict(mean[T,d,batch], cov[T,d,d,batch] or [T,d,d], neg_log_evidence[batch], status[batch])."""
+        -> dict(mean[T,d,batch], cov[T,d,d,batch] or [T,d,d], neg_log_evidence[batch], status[batch]).
+        ``inputs``: known per-step inputs, x[t] ~ N(A x[t-1] + inputs[t], P) -- a host [T, d] array shared by every
+        chain, or a CUDA [T, d, batch] tensor (device calls only); exclusive with ``u``."""
         on_dev = y.is_cuda
         T, m, batch, d, flags, ptrs, mask, mask_p, keep = self._sweep_args(
             y, A, B, P, Q, m0, S0, u, mask, on_dev, per_chain_model, force_per_chain_path, cov_shared_out, transition_first,
-            asynchronous)
+            asynchronous, inputs)
         mk = lambda *s, dt=torch.float32: (torch.empty(*s, dtype=dt, device=y.device) if on_dev
                                            else torch.empty(*s, dtype=dt).pin_memory())
         self._io(out_mean, "out_mean", on_dev, shape=(T, d, batch))
@@ -197,14 +222,15 @@ class Context:
         self._check(fn(self.h, d, m, T, batch, *ptrs, _fp(y), mask_p, _fp(mean), _fp(cov), _fp(nle), st_p, flags))
         return dict(mean=mean, cov=cov if (want_cov or need_cov) else None, neg_log_evidence=nle, status=status)
 
-    def lgssm_predict(self, y, A, B, P, Q, m0, S0, *, horizon=0, u=None, mask=None, want_cov=True, want_pred_cov=True,
+    def lgssm_predict(self, y, A, B, P, Q, m0, S0, *, horizon=0, u=None, inputs=None, mask=None, want_cov=True, want_pred_cov=True,
                       want_forecast_states=True, want_evidence=False, want_status=False, per_chain_model=False,
                       force_per_chain_path=False, cov_shared_out=False, transition_first=False, asynchronous=False):
         """Smoother + predictive distributions of the observations (``rxg_lgssm_smooth_predict_f32``).
         y[T, m, batch] on this context's device; ``mask`` as for :meth:`lgssm` ([T, batch] per chain, or a [T] pattern
         shared by every chain).  Returns dict(mean, cov, neg_log_evidence, status) as :meth:`lgssm` plus
         pred_mean[T+H, m, batch], pred_cov[T+H, m, m, batch] (or [T+H, m, m] with ``cov_shared_out``), and the state
-        forecasts fc_mean[H, d, batch], fc_cov[H, d, d, batch] (or [H, d, d]); rows T.. of pred_* are the forecasts."""
+        forecasts fc_mean[H, d, batch], fc_cov[H, d, d, batch] (or [H, d, d]); rows T.. of pred_* are the forecasts.
+        ``inputs`` as for :meth:`lgssm` with T + H rows: forecast k = 1..H uses row T + k - 1."""
         if not y.is_cuda:
             raise ValueError("lgssm_predict: y must be a CUDA tensor (the prediction entry takes device pointers)")
         H = int(horizon)
@@ -212,7 +238,7 @@ class Context:
             raise ValueError(f"horizon must be >= 0, got {horizon}")
         T, m, batch, d, flags, ptrs, mask, mask_p, keep = self._sweep_args(
             y, A, B, P, Q, m0, S0, u, mask, True, per_chain_model, force_per_chain_path, cov_shared_out, transition_first,
-            asynchronous)
+            asynchronous, inputs, y.shape[0] + H)
         mk = lambda *s, dt=torch.float32: torch.empty(*s, dtype=dt, device=y.device)
         mean = mk(T, d, batch)
         need_cov = want_cov or per_chain_model or force_per_chain_path or mask is not None
@@ -230,10 +256,11 @@ class Context:
         return dict(mean=mean, cov=cov if want_cov else None, neg_log_evidence=nle, status=status, pred_mean=pred_mean,
                     pred_cov=pred_cov, fc_mean=fc_mean, fc_cov=fc_cov)
 
-    def lgssm_filter_chunk(self, y, A, B, P, Q, prev_mean, carry_cov, *, u=None, want_evidence=False,
+    def lgssm_filter_chunk(self, y, A, B, P, Q, prev_mean, carry_cov, *, u=None, inputs=None, want_evidence=False,
                            cov_shared_out=False, out_mean=None, out_cov=None):
         """One time-chunk of the streaming engine (``rxg_lgssm_filter_chunk_f32``).  ``prev_mean[d, batch]``
-        (CUDA) and ``carry_cov[d, d]`` (host fp32 numpy, updated IN PLACE) are the autoupdate carry."""
+        (CUDA) and ``carry_cov[d, d]`` (host fp32 numpy, updated IN PLACE) are the autoupdate carry.  ``inputs``: the
+        chunk's input rows ([Tc, d] host or [Tc, d, batch] CUDA, as for :meth:`lgssm`; row 0 enters x[t0])."""
         self._dev(y, prev_mean)
         T, m, batch = y.shape
         d = prev_mean.shape[0]
@@ -251,6 +278,11 @@ class Context:
         cov = out_cov if out_cov is not None else (self.empty(T, d, d) if cov_shared_out else self.empty(T, d, d, batch))
         nle = self.empty(batch) if want_evidence else None
         flags = L.PTR_DEVICE | (L.COV_SHARED_OUT if cov_shared_out else 0)
+        seq = self._inputs(inputs, u, T, d, batch)
+        if seq is not None:
+            flags |= seq[0]
+            ptrs[-1] = seq[1]
+            keep.append(seq[2])
         cc = carry_cov.ctypes.data_as(L.fp)
         self._check(self.lib.rxg_lgssm_filter_chunk_f32(self.h, d, m, T, batch, *ptrs, _fp(prev_mean), cc, _fp(y),
                                                         _fp(mean), _fp(cov), _fp(nle), flags))

@@ -111,6 +111,27 @@ int stage_shared_mask(rxg_ctx* ctx, int T, const uint8_t* host_mask, LgssmCall& 
     c.n_observed = nobs;
     return RXG_OK;
 }
+int stage_inputs(rxg_ctx* ctx, unsigned flags, const float* u, int rows, int d, LgssmCall& c) {
+    const unsigned f = flags & (RXG_U_SEQ_SHARED | RXG_U_SEQ_CHAIN);
+    c.u = u; c.useq = nullptr; c.useq_host = nullptr; c.useq_chain = false;
+    if (!f) return RXG_OK;
+    if (f == (RXG_U_SEQ_SHARED | RXG_U_SEQ_CHAIN))
+        return fail(ctx, RXG_ERR_BAD_ARG, "lgssm: RXG_U_SEQ_SHARED and RXG_U_SEQ_CHAIN are exclusive");
+    if (!u) return fail(ctx, RXG_ERR_BAD_ARG, "lgssm: an RXG_U_SEQ_* flag needs the input sequence u");
+    c.u = nullptr;
+    if (f == RXG_U_SEQ_CHAIN) {
+        if (!(flags & RXG_PTR_DEVICE))
+            return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm: a per-chain input sequence (RXG_U_SEQ_CHAIN) takes device pointers");
+        c.useq = u; c.useq_chain = true;
+        return RXG_OK;
+    }
+    const size_t bytes = (size_t)rows * d * 4;
+    if (!grow(ctx, &ctx->d_useq, &ctx->useq_bytes, bytes)) return RXG_ERR_CUDA;
+    // pageable host source: the runtime has read it before the call returns
+    RXG_CUDA(ctx, cudaMemcpyAsync(ctx->d_useq, u, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    c.useq = (const float*)ctx->d_useq; c.useq_host = u;
+    return RXG_OK;
+}
 void* workspace(rxg_ctx* ctx, size_t bytes) { return grow(ctx, &ctx->ws, &ctx->ws_bytes, bytes); }
 void* staging(rxg_ctx* ctx, size_t bytes) { return grow(ctx, &ctx->stage, &ctx->stage_bytes, bytes); }
 void* predict_scratch(rxg_ctx* ctx, size_t bytes) { return grow(ctx, &ctx->pred_buf, &ctx->pred_bytes, bytes); }
@@ -193,6 +214,7 @@ int rxg_destroy(rxg_ctx* ctx) {
     if (ctx->d_bad) cudaFree(ctx->d_bad);
     for (int i = 0; i < 4; ++i) if (ctx->aux_buf[i]) cudaFree(ctx->aux_buf[i]);
     if (ctx->d_tmask) cudaFree(ctx->d_tmask);
+    if (ctx->d_useq) cudaFree(ctx->d_useq);
     if (ctx->pred_buf) cudaFree(ctx->pred_buf);
     if (ctx->h_bad) cudaFreeHost(ctx->h_bad);
     for (int i = 0; i < 4; ++i) if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
@@ -347,6 +369,10 @@ static int lgssm_entry(rxg_ctx* ctx, bool smooth, int d, int m, int T, int64_t b
     c.d = d; c.m = m; c.T = T; c.batch = batch;
     c.A = A; c.B = B; c.P = P; c.Q = Q; c.m0 = m0; c.S0 = S0; c.u = u;
     c.flags = flags; c.smooth = smooth;
+    {
+        const int rci = stage_inputs(ctx, flags, u, T + (pred ? pred->H : 0), d, c);
+        if (rci != RXG_OK) return rci;
+    }
     if ((flags & RXG_MASK_SHARED) && ymask) {
         if (per_chain_model || (flags & RXG_PATH_PER_CHAIN))
             return fail(ctx, RXG_ERR_BAD_ARG, "lgssm: RXG_MASK_SHARED belongs to the shared-model gain-table path");
@@ -558,9 +584,12 @@ int rxg_lgssm_filter_chunk_f32(rxg_ctx* ctx, int d, int m, int T, int64_t batch,
         return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_filter_chunk: (d=%d, m=%d) is outside the compiled kernel families", d, m);
     RXG_CUDA(ctx, cudaSetDevice(ctx->device));
     std::vector<float> zero((size_t)d, 0.f);
+    int rc0 = RXG_OK;
     LgssmCall c;
     c.d = d; c.m = m; c.T = T; c.batch = batch;
-    c.A = A; c.B = B; c.P = P; c.Q = Q; c.m0 = zero.data(); c.S0 = carry_cov; c.u = u;
+    c.A = A; c.B = B; c.P = P; c.Q = Q; c.m0 = zero.data(); c.S0 = carry_cov;
+    rc0 = stage_inputs(ctx, flags, u, T, d, c);
+    if (rc0 != RXG_OK) return rc0;
     c.mean0_chain = prev_mean;
     c.y = y; c.ymask = nullptr; c.mean = filt_mean; c.cov = filt_cov; c.nle = neg_log_evidence; c.status = nullptr;
     c.flags = (flags | RXG_TRANSITION_FIRST) & ~(unsigned)RXG_ASYNC;

@@ -194,7 +194,10 @@ __device__ __forceinline__ BwdEl<D> bwd_combine(const BwdEl<D>& early, const Bwd
 template <int D, int M>
 __global__ void __cluster_dims__(GS_CTAS, 1, 1) __launch_bounds__(GS_THREADS, 1)
 gain_scan_kernel(const __grid_constant__ ModelF<D, M> mdl, GainWs ws, ScanWs sw, int T, int transition_first,
-                 float* __restrict__ cov_shared_out, int* __restrict__ bad_out, const uint8_t* __restrict__ tmask) {
+                 float* __restrict__ cov_shared_out, int* __restrict__ bad_out, const uint8_t* __restrict__ tmask,
+                 const float* __restrict__ useq) {
+    // useq[T][D] (or null for the constant mdl.u): a shared input sequence (RXG_U_SEQ_SHARED) -- the offset terms
+    // become gf_t = (I - K_t B) u_t and gb_t = -G_t u_{t+1}; nothing else depends on it.
     // tmask[T] (or null): 1 = the datum of step t exists for EVERY chain, 0 = missing for every chain (RXG_MASK_SHARED).
     // A missing step is a pure transition: scan element (A, P, 0), no gain, no evidence term -- the covariances stay
     // chain independent, so the whole batch stays on this path instead of the per-chain covariance recursion.
@@ -370,7 +373,7 @@ gain_scan_kernel(const __grid_constant__ ModelF<D, M> mdl, GainWs ws, ScanWs sw,
             rec[TB::C_OFF] = (float)cconst;
             Vec<double, D> uu, gf;
 #pragma unroll
-            for (int i = 0; i < D; ++i) uu(i) = (double)mdl.u[i];
+            for (int i = 0; i < D; ++i) uu(i) = (double)(useq ? useq[(size_t)t * D + i] : mdl.u[i]);
             gf = mulv(IKB, uu);
             if (!(t > 0 || transition_first)) {
 #pragma unroll
@@ -399,7 +402,7 @@ gain_scan_kernel(const __grid_constant__ ModelF<D, M> mdl, GainWs ws, ScanWs sw,
             store_f(brec + TB::G_OFF, be.E);
             Vec<double, D> uu;
 #pragma unroll
-            for (int i = 0; i < D; ++i) uu(i) = -(double)mdl.u[i];
+            for (int i = 0; i < D; ++i) uu(i) = -(double)(useq ? useq[(size_t)(t + 1) * D + i] : mdl.u[i]);
             gb = mulv(be.E, uu);
         } else {
 #pragma unroll

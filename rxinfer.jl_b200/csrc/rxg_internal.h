@@ -50,6 +50,8 @@ struct rxg_ctx {
     unsigned peer_epoch = 0;
     void* d_tmask = nullptr;     // device copy of a shared missing-data pattern (RXG_MASK_SHARED)
     size_t tmask_bytes = 0;
+    void* d_useq = nullptr;      // device copy of a shared input sequence (RXG_U_SEQ_SHARED)
+    size_t useq_bytes = 0;
     // grow-only scratch of the general-shape front end (padded operands, shifted observations)
     void* aux_buf[4] = {nullptr, nullptr, nullptr, nullptr};
     size_t aux_bytes[4] = {0, 0, 0, 0};
@@ -94,6 +96,11 @@ struct LgssmCall {
     // shared model: host pointers (row-major); per-chain model: device pointers [..][batch]
     const float *A, *B, *P, *Q, *m0, *S0;
     const float* u;          // transition offset (same pointer space as the model) or null
+    // per-step inputs (RXG_U_SEQ_*; then u is null): device sequence, row t at useq + t * d * ustride (ustride = batch
+    // for a per-chain sequence [rows][d][batch], 1 for a shared one [rows][d] read with batch stride 0)
+    const float* useq = nullptr;
+    const float* useq_host = nullptr; // the shared sequence's host copy [rows][d] (large-state trajectory, embedding)
+    bool useq_chain = false;
     const float* mean0_chain = nullptr;   // device [d][batch]: per-chain prior mean (streaming carry) or null
     const float* y;          // device
     const uint8_t* ymask;    // device or null
@@ -120,6 +127,8 @@ int launch_replicate_cov(rxg_ctx* ctx, cudaStream_t st, const float* src, int64_
                          int64_t b, int G, int skip);
 int ensure_aux_stream(rxg_ctx* ctx);
 int stage_shared_mask(rxg_ctx* ctx, int T, const uint8_t* host_mask, LgssmCall& c);    // rxg_api.cu
+// rxg_api.cu: validate the RXG_U_SEQ_* flags and set c.u / c.useq* (`rows` rows of the sequence are staged / read)
+int stage_inputs(rxg_ctx* ctx, unsigned flags, const float* u, int rows, int d, LgssmCall& c);
 // rxg_lgssm_general.cu: any (d, m) in 1..64 (native families, embedding, generic per-chain kernel)
 int lgssm_dispatch(rxg_ctx* ctx, LgssmCall& c);
 // rxg_lgssm.cu: the register-resident families (d <= 6 shapes)

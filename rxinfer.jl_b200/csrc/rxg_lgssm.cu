@@ -36,12 +36,15 @@ namespace rxg {
 // ============================================================================================
 // Family 1: one thread per chain, full (mu, Sigma) recursion
 // ============================================================================================
-template <int D, int M, bool PER_CHAIN, bool SMOOTH>
+// USEQ: per-step inputs, u[t] = useq[(t * D + i) * ustride + b * uchain] (a per-chain [rows][D][batch] sequence, or a
+// shared [rows][D] one with ustride = 1, uchain = 0) replaces the constant offset.
+template <int D, int M, bool PER_CHAIN, bool SMOOTH, bool USEQ = false>
 __global__ void __launch_bounds__(128)
 lgssm_chain_kernel(const __grid_constant__ ModelF<D, M> mdl, PerChainPtrs pc,
                    const float* __restrict__ y, const uint8_t* __restrict__ mask,
                    float* __restrict__ mean, float* __restrict__ cov, float* __restrict__ nle,
-                   int32_t* __restrict__ status, int T, int64_t batch, int transition_first) {
+                   int32_t* __restrict__ status, int T, int64_t batch, int transition_first,
+                   const float* __restrict__ useq = nullptr, int64_t ustride = 0, int uchain = 0) {
     const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= batch) return;
 
@@ -93,6 +96,9 @@ lgssm_chain_kernel(const __grid_constant__ ModelF<D, M> mdl, PerChainPtrs pc,
             // rule #1  *(:out): (A mu, A S A')   rule #2  MvNormalMeanCovariance(:out): + P
             //          (+ the `+` rule with a PointMass operand: pure mean shift by u)
             mu = mulv(A, mu);
+            if (USEQ)
+#pragma unroll
+                for (int i = 0; i < D; ++i) u(i) = __ldg(useq + ((int64_t)t * D + i) * ustride + b * uchain);
 #pragma unroll
             for (int i = 0; i < D; ++i) mu(i) += u(i);
             Mat<float, D, D> AS = mul(A, S);
@@ -181,6 +187,9 @@ lgssm_chain_kernel(const __grid_constant__ ModelF<D, M> mdl, PerChainPtrs pc,
             Mat<float, D, D> GS = mul(G, Ss);
             Ss = sym_mul_nt_add(GS, G, C);
             Vec<float, D> mup = mulv(A, muf);
+            if (USEQ)       // the transition into x[t+1]
+#pragma unroll
+                for (int i = 0; i < D; ++i) u(i) = __ldg(useq + ((int64_t)(t + 1) * D + i) * ustride + b * uchain);
 #pragma unroll
             for (int i = 0; i < D; ++i) mup(i) = mus(i) - (mup(i) + u(i));
             Vec<float, D> dm = mulv(G, mup);
@@ -237,7 +246,8 @@ __global__ void gain_riccati_seq(const __grid_constant__ ModelF<D, M> mdl, GainW
 // Phase 2 (parallel in t): gains, innovation factors, conditional covariances.
 template <int D, int M>
 __global__ void gain_tables(const __grid_constant__ ModelF<D, M> mdl, GainWs ws, int T,
-                            int transition_first, int* __restrict__ bad_out, const uint8_t* __restrict__ tmask) {
+                            int transition_first, int* __restrict__ bad_out, const uint8_t* __restrict__ tmask,
+                            const float* __restrict__ useq) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
     using TB = Tab<D, M>;
@@ -289,7 +299,7 @@ __global__ void gain_tables(const __grid_constant__ ModelF<D, M> mdl, GainWs ws,
         rec[TB::C_OFF] = (float)cconst;
         Vec<double, D> uu, gf;
 #pragma unroll
-        for (int i = 0; i < D; ++i) uu(i) = (double)mdl.u[i];
+        for (int i = 0; i < D; ++i) uu(i) = (double)(useq ? useq[(size_t)t * D + i] : mdl.u[i]);
         gf = mulv(IKB, uu);
         if (!(t > 0 || transition_first)) {
 #pragma unroll
@@ -318,7 +328,7 @@ __global__ void gain_tables(const __grid_constant__ ModelF<D, M> mdl, GainWs ws,
         {
             Vec<double, D> uu;
 #pragma unroll
-            for (int i = 0; i < D; ++i) uu(i) = -(double)mdl.u[i];
+            for (int i = 0; i < D; ++i) uu(i) = -(double)(useq ? useq[(size_t)(t + 1) * D + i] : mdl.u[i]);
             gb = mulv(G, uu);
         }
         store_d(ws.Cc + (size_t)t * D * D, C);
@@ -380,9 +390,17 @@ static int run_chain_family(rxg_ctx* ctx, LgssmCall& c) {
     const int threads = 64;
     const unsigned blocks = (unsigned)((c.batch + threads - 1) / threads);
     const int tf = (c.flags & RXG_TRANSITION_FIRST) ? 1 : 0;
+    const int64_t ustride = c.useq_chain ? c.batch : 1;
+    const int uchain = c.useq_chain ? 1 : 0;
 #define RXG_LAUNCH_CHAIN(PC, SM)                                                                   \
-    lgssm_chain_kernel<D, M, PC, SM><<<blocks, threads, 0, ctx->stream>>>(                         \
-        mdl, pc, c.y, c.ymask, c.mean, c.cov, c.nle, c.status, c.T, c.batch, tf)
+    do {                                                                                           \
+        if (c.useq)                                                                                \
+            lgssm_chain_kernel<D, M, PC, SM, true><<<blocks, threads, 0, ctx->stream>>>(           \
+                mdl, pc, c.y, c.ymask, c.mean, c.cov, c.nle, c.status, c.T, c.batch, tf, c.useq, ustride, uchain); \
+        else                                                                                       \
+            lgssm_chain_kernel<D, M, PC, SM><<<blocks, threads, 0, ctx->stream>>>(                 \
+                mdl, pc, c.y, c.ymask, c.mean, c.cov, c.nle, c.status, c.T, c.batch, tf);          \
+    } while (0)
     if (ctx->profile) { cudaEventRecord(ctx->ev[0], ctx->stream); cudaEventRecord(ctx->ev[1], ctx->stream); }
     if (per_chain) { if (c.smooth) RXG_LAUNCH_CHAIN(true, true); else RXG_LAUNCH_CHAIN(true, false); }
     else           { if (c.smooth) RXG_LAUNCH_CHAIN(false, true); else RXG_LAUNCH_CHAIN(false, false); }
@@ -401,14 +419,46 @@ static int launch_shared(rxg_ctx* ctx, LgssmCall& c, const ModelF<D, M>& mdl, co
     const unsigned blocks = (unsigned)((nthr + threads - 1) / threads);
     const int tf = (c.flags & RXG_TRANSITION_FIRST) ? 1 : 0;
     const bool evid = c.nle != nullptr;
-    bool has_u = false;
+    bool has_u = c.useq != nullptr && !c.useq_chain;       // a shared input sequence lives in the gain tables' offsets
     for (int i = 0; i < D; ++i) has_u |= (mdl.u[i] != 0.f);
     // checkpoint + recompute instead of the forward->backward stash (RXG_NO_CKPT=1: A/B switch)
     bool ckpt = c.smooth && (D * D <= 16) && (CPT == 2);   // with one chain per thread the stash path is faster
     if (ctx->opt[RXG_OPT_SWEEP_VARIANT] == 1) ckpt = false;                     // stash variant (A/B switch)
     // fused all-gather: only the headline variant (smoothing, no evidence, no offset) has a PEER instantiation;
     // everything else leaves fused_peer_stores false and the caller pushes the finished slab
-    const bool peer = c.smooth && !evid && !has_u && (c.po.n_mean > 0 || c.po.n_cov > 0);
+    const bool peer = c.smooth && !evid && !has_u && !c.useq && (c.po.n_mean > 0 || c.po.n_cov > 0);
+    if (c.useq_chain) {
+        // per-chain input sequence: its own instantiation, streamed beside y (no offset, no peer stores)
+#define RXG_LAUNCH_USEQ(SM, EV, CK)                                                                \
+        lgssm_shared_kernel<D, M, CPT, PF, SM, EV, false, CK, false, 1><<<blocks, threads, 0, ctx->stream>>>( \
+            mdl, ws.fwd, ws.bwd, ws.sf, c.y, c.mean, c.cov, c.nle, c.T, c.batch, tf, write_cov, c.mean0_chain, c.po, c.useq)
+        if (ctx->profile) cudaEventRecord(ctx->ev[1], ctx->stream);
+        if (c.smooth) {
+            if (ckpt) { if (evid) RXG_LAUNCH_USEQ(true, true, true); else RXG_LAUNCH_USEQ(true, false, true); }
+            else      { if (evid) RXG_LAUNCH_USEQ(true, true, false); else RXG_LAUNCH_USEQ(true, false, false); }
+        } else {
+            if (evid) RXG_LAUNCH_USEQ(false, true, false); else RXG_LAUNCH_USEQ(false, false, false);
+        }
+#undef RXG_LAUNCH_USEQ
+        if (ctx->profile) cudaEventRecord(ctx->ev[2], ctx->stream);
+        ctx->launches += 1;
+        c.fused_peer_stores = false;
+        return check_cuda(ctx, cudaGetLastError(), "lgssm_shared_kernel (input sequence) launch");
+    }
+    if (c.useq && evid) {
+        // shared input sequence with evidence: the tables carry the offsets, the evidence form reads u_t
+#define RXG_LAUNCH_USEQ2(SM, CK)                                                                   \
+        lgssm_shared_kernel<D, M, CPT, PF, SM, true, true, CK, false, 2><<<blocks, threads, 0, ctx->stream>>>( \
+            mdl, ws.fwd, ws.bwd, ws.sf, c.y, c.mean, c.cov, c.nle, c.T, c.batch, tf, write_cov, c.mean0_chain, c.po, c.useq)
+        if (ctx->profile) cudaEventRecord(ctx->ev[1], ctx->stream);
+        if (c.smooth) { if (ckpt) RXG_LAUNCH_USEQ2(true, true); else RXG_LAUNCH_USEQ2(true, false); }
+        else RXG_LAUNCH_USEQ2(false, false);
+#undef RXG_LAUNCH_USEQ2
+        if (ctx->profile) cudaEventRecord(ctx->ev[2], ctx->stream);
+        ctx->launches += 1;
+        c.fused_peer_stores = false;
+        return check_cuda(ctx, cudaGetLastError(), "lgssm_shared_kernel (shared input sequence, evidence) launch");
+    }
 #define RXG_LAUNCH_SHARED2(SM, EV, OF, CK)                                                         \
     do {                                                                                           \
         if (SM && !EV && !OF && peer)                                                              \
@@ -511,10 +561,12 @@ static int run_shared_family(rxg_ctx* ctx, LgssmCall& c) {
     c.cov_table = (c.want_cov_table && c.smooth) ? (float*)(base + o_ctab) : nullptr;
     if (ctx->profile) cudaEventRecord(ctx->ev[0], ctx->stream);
     float* cov_once = (cov_shared && c.cov && c.smooth) ? c.cov : (c.smooth ? c.cov_table : nullptr);
+    // a shared input sequence goes into the tables' offset terms; a per-chain one into the sweep (tables without inputs)
+    const float* useq_tab = c.useq_chain ? nullptr : c.useq;
     if (ctx->opt[RXG_OPT_GAIN_SEQ] != 0) {
         // sequential Riccati recursion (cross-check of the scan; ~70x slower at T = 1000)
         gain_riccati_seq<D, M><<<1, 32, 0, ctx->stream>>>(mdl, ws, c.T, tf, bad_flag(ctx), c.tmask);
-        gain_tables<D, M><<<(c.T + 63) / 64, 64, 0, ctx->stream>>>(mdl, ws, c.T, tf, bad_flag(ctx), c.tmask);
+        gain_tables<D, M><<<(c.T + 63) / 64, 64, 0, ctx->stream>>>(mdl, ws, c.T, tf, bad_flag(ctx), c.tmask, useq_tab);
         ctx->launches += 2;
         if (c.smooth) {
             gain_smooth_seq<D, M><<<1, 32, 0, ctx->stream>>>(ws, c.T, cov_once);
@@ -522,7 +574,8 @@ static int run_shared_family(rxg_ctx* ctx, LgssmCall& c) {
         }
     } else {
         // time-parallel associative scans in one 8-CTA cluster
-        gain_scan_kernel<D, M><<<GS_CTAS, GS_THREADS, 0, ctx->stream>>>(mdl, ws, sw, c.T, tf, cov_once, bad_flag(ctx), c.tmask);
+        gain_scan_kernel<D, M><<<GS_CTAS, GS_THREADS, 0, ctx->stream>>>(mdl, ws, sw, c.T, tf, cov_once, bad_flag(ctx), c.tmask,
+                                                                          useq_tab);
         ctx->launches += 1;
     }
     if (!c.smooth && cov_shared && c.cov) {
@@ -537,12 +590,13 @@ static int run_shared_family(rxg_ctx* ctx, LgssmCall& c) {
     const int write_cov = (c.cov != nullptr && !cov_shared) ? 1 : 0;
     // sweep variant (RXG_OPT_SWEEP_VARIANT): 3 / 4 = time-segmented kernel with / without L2 eviction hints
     const long long variant = ctx->opt[RXG_OPT_SWEEP_VARIANT];
-    if (variant == 3 && seg_sweep_eligible<D, M>(c)) {
+    if (variant == 3 && !c.useq && seg_sweep_eligible<D, M>(c)) {      // inputs: the lock-step kernel
         SegWs sgw;
         sgw.rec = (float*)(base + o_srec_t); sgw.nrec = (float*)(base + o_snrec); sgw.srec = (float*)(base + o_ssrec);
         return launch_seg<D, M>(ctx, c, mdl, ws, sgw, write_cov, variant == 3);
     }
-    const bool al16 = (((uintptr_t)c.y | (uintptr_t)c.mean | (uintptr_t)c.cov | (uintptr_t)c.nle | (uintptr_t)c.mean0_chain) & 15) == 0;
+    const bool al16 = (((uintptr_t)c.y | (uintptr_t)c.mean | (uintptr_t)c.cov | (uintptr_t)c.nle | (uintptr_t)c.mean0_chain |
+                        (uintptr_t)(c.useq_chain ? c.useq : nullptr)) & 15) == 0;
     // chains per thread: keep >= ~2 resident warps per SM sub-partition
     // Wider per-thread vectors cut the number of (128-byte-per-warp) store instructions per byte.
     int cpt = (c.batch >= (int64_t)ctx->sm_count * 64 * 2) ? 2 : 1;

@@ -11,9 +11,11 @@
 // Block-diagonal structure is preserved exactly by every message of the schedule (zeros stay zeros in floating
 // point), so the posteriors of the real coordinates are those of the original model; each dummy observation adds
 // exactly 1/2 log 2 pi per step to the evidence (innovation 0, innovation variance 1), which is subtracted.
-// Offset by linearity: x_t = z_t + xi_t with the deterministic trajectory z_t = A z_{t-1} + u (z = 0 at the prior);
-// xi follows the offset-free model observed through y_t - B z_t, covariances and evidence are unchanged, and
-// E[x_t | y] = z_t + E[xi_t | y].
+// Offset by linearity: x_t = z_t + xi_t with the deterministic trajectory z_t = A z_{t-1} + u_t (z = 0 at the prior;
+// u_t = u for a constant offset, row t of the input sequence with RXG_U_SEQ_*); xi follows the offset-free model
+// observed through y_t - B z_t, covariances and evidence are unchanged (the shift has a Jacobian of 1), and
+// E[x_t | y] = z_t + E[xi_t | y].  A shared offset / sequence gives one host trajectory (fp64); a per-chain sequence
+// gives one trajectory per chain (input_traj_kernel).
 // [ref: the reference handles any d, m and the `+` node generically: test/models/statespace/mlgssm_test.jl:8-17,
 //  ulgssm_tests.jl:7-16.]
 #include <math.h>
@@ -103,16 +105,96 @@ bool embedding_shape(int d, int m, int* D, int* M) {
     return false;
 }
 
-// offset on the large-state family, removed by linearity (shared model)
+// z_t = A z_{t-1} + u_t per chain (u[T][d][batch]; z = 0 at the prior and at t = 0 without a transition), written to
+// z[T][d][batch], and ys = y - B z_t.  Block = 32 chains x NY row threads; A and B in shared memory (broadcast reads),
+// z_{t-1} / z_t of the 32 chains double buffered in shared memory: one barrier per step.
+__global__ void __launch_bounds__(1024) input_traj_kernel(const float* __restrict__ A, const float* __restrict__ B,
+                                                          const float* __restrict__ u, const float* __restrict__ y,
+                                                          float* __restrict__ ys, float* __restrict__ z, int d, int m, int T,
+                                                          int64_t batch, int tf) {
+    extern __shared__ float sh[];
+    float* sA = sh;                    // d x d
+    float* sB = sA + d * d;            // m x d
+    float* sz = sB + m * d;            // [2][d][32]
+    const int lane = threadIdx.x, ny = blockDim.y;
+    const int tid = threadIdx.y * 32 + lane, nt = 32 * ny;
+    for (int e = tid; e < d * d; e += nt) sA[e] = A[e];
+    for (int e = tid; e < m * d; e += nt) sB[e] = B[e];
+    const int64_t b = (int64_t)blockIdx.x * 32 + lane;
+    const bool on = b < batch;
+    __syncthreads();
+    for (int t = 0; t < T; ++t) {
+        const float* zp = sz + ((t + 1) & 1) * d * 32;
+        float* zc = sz + (t & 1) * d * 32;
+        const bool pred = t > 0 || tf;
+        for (int i = threadIdx.y; i < d; i += ny) {
+            float s = 0.f;
+            if (pred && on) {
+                s = __ldg(u + ((int64_t)t * d + i) * batch + b);
+                if (t > 0)
+                    for (int j = 0; j < d; ++j) s = __fmaf_rn(sA[i * d + j], zp[j * 32 + lane], s);
+            }
+            zc[i * 32 + lane] = s;
+            if (on) z[((int64_t)t * d + i) * batch + b] = s;
+        }
+        __syncthreads();
+        if (on)
+            for (int k = threadIdx.y; k < m; k += ny) {
+                float s = __ldg(y + ((int64_t)t * m + k) * batch + b);
+                for (int j = 0; j < d; ++j) s = __fmaf_rn(-sB[k * d + j], zc[j * 32 + lane], s);
+                ys[((int64_t)t * m + k) * batch + b] = s;
+            }
+    }
+}
+__global__ void add_kernel(float* __restrict__ v, const float* __restrict__ w, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) v[i] += __ldg(w + i);
+}
+
+// offset / input sequence on the large-state family, removed by linearity (shared model)
 int large_with_offset(rxg_ctx* ctx, LgssmCall& c) {
+    if (c.useq_chain) {
+        const int d = c.d, m = c.m, T = c.T;
+        const int64_t batch = c.batch;
+        const size_t nz = (size_t)T * d * batch, ny = (size_t)T * m * batch;
+        size_t off = 0;
+        auto carve = [&](size_t n) { size_t o = off; off += (n * 4 + 255) / 256 * 256; return o; };
+        const size_t o_AB = carve((size_t)d * d + (size_t)m * d), o_ys = carve(c.tables_only ? 0 : ny);
+        char* base = (char*)aux(ctx, 3, off);
+        float* zb = (float*)aux(ctx, 2, nz * 4);
+        if (!base || !zb) return RXG_ERR_CUDA;
+        float *dAB = (float*)(base + o_AB), *ys = (float*)(base + o_ys);
+        LgssmCall c2 = c;
+        c2.useq = nullptr; c2.useq_chain = false;
+        if (!c.tables_only) {
+            RXG_CUDA(ctx, cudaMemcpyAsync(dAB, c.A, (size_t)d * d * 4, cudaMemcpyHostToDevice, ctx->stream));
+            RXG_CUDA(ctx, cudaMemcpyAsync(dAB + (size_t)d * d, c.B, (size_t)m * d * 4, cudaMemcpyHostToDevice, ctx->stream));
+            const int rows = d > m ? d : m, nyt = rows < 32 ? rows : 32;
+            const size_t smem = ((size_t)d * d + (size_t)m * d + 2 * (size_t)d * 32) * 4;
+            RXG_CUDA(ctx, cudaFuncSetAttribute(input_traj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            input_traj_kernel<<<(unsigned)((batch + 31) / 32), dim3(32, nyt), smem, ctx->stream>>>(
+                dAB, dAB + (size_t)d * d, c.useq, c.y, ys, zb, d, m, T, batch, (c.flags & RXG_TRANSITION_FIRST) ? 1 : 0);
+            ctx->launches += 1;
+            RXG_CUDA(ctx, cudaGetLastError());
+            c2.y = ys;
+        }
+        int rc = lgssm_large_dispatch(ctx, c2);
+        if (rc != RXG_OK) return rc;
+        if (!c.tables_only && c.mean) {
+            add_kernel<<<grid_for(ctx, (int64_t)nz), 256, 0, ctx->stream>>>(c.mean, zb, (int64_t)nz);
+            ctx->launches += 1;
+        }
+        c.fused_peer_stores = false;
+        return check_cuda(ctx, cudaGetLastError(), "input trajectory kernels");
+    }
     const int d = c.d, m = c.m, T = c.T;
     std::vector<double> z((size_t)d, 0.0), zn((size_t)d);
     std::vector<float> traj((size_t)T * d), btraj((size_t)T * m);
     const bool tf = (c.flags & RXG_TRANSITION_FIRST) != 0;
     for (int t = 0; t < T; ++t) {
         if (t > 0 || tf) {
+            const float* ut = c.useq_host ? c.useq_host + (size_t)t * d : c.u;
             for (int i = 0; i < d; ++i) {
-                double s = (double)c.u[i];
+                double s = (double)ut[i];
                 for (int j = 0; j < d; ++j) s += (double)c.A[i * d + j] * z[j];
                 zn[i] = s;
             }
@@ -135,7 +217,7 @@ int large_with_offset(rxg_ctx* ctx, LgssmCall& c) {
     RXG_CUDA(ctx, cudaMemcpyAsync(btr, btraj.data(), btraj.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
     RXG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     LgssmCall c2 = c;
-    c2.u = nullptr;
+    c2.u = nullptr; c2.useq = nullptr; c2.useq_host = nullptr;
     if (!c.tables_only) {
         shift_rows_kernel<<<grid_for(ctx, (int64_t)ny), 256, 0, ctx->stream>>>(c.y, ys, btr, (int64_t)T * m, c.batch, -1.f);
         c2.y = ys;
@@ -174,6 +256,10 @@ int embedded(rxg_ctx* ctx, LgssmCall& c, int D, int M) {
     auto carve = [&](size_t n) { size_t o = off; off += (n * 4 + 255) / 256 * 256; return o; };
     const size_t o_y = carve(c.tables_only ? 0 : n_y), o_mean = carve(c.tables_only ? 0 : n_mean);
     const size_t o_tab = carve(want_cov ? n_tab : 0), o_m0 = carve(c.mean0_chain ? n_m0 : 0);
+    const size_t o_u = carve(c.useq ? (size_t)T * D * (c.useq_chain ? batch : 1) : 0);
+    std::vector<float> useq_pad(c.useq_host ? (size_t)T * D : 0, 0.f);     // shared input sequence, padded on the host
+    for (size_t t = 0; c.useq_host && t < (size_t)T; ++t)
+        for (int i = 0; i < d; ++i) useq_pad[t * D + i] = c.useq_host[t * d + i];
     char* base = (char*)aux(ctx, 0, off);
     if (!base) return RXG_ERR_CUDA;
     float *yp = (float*)(base + o_y), *meanp = (float*)(base + o_mean), *tab = (float*)(base + o_tab), *m0p = (float*)(base + o_m0);
@@ -181,6 +267,18 @@ int embedded(rxg_ctx* ctx, LgssmCall& c, int D, int M) {
     c2.d = D; c2.m = M;
     c2.A = A.data(); c2.B = B.data(); c2.P = P.data(); c2.Q = Q.data(); c2.m0 = m0.data(); c2.S0 = S0.data();
     c2.u = c.u ? u.data() : nullptr;
+    if (c.useq) {
+        float* up = (float*)(base + o_u);
+        if (c.useq_chain) {
+            pad_rows_kernel<<<grid_for(ctx, (int64_t)T * D * batch), 256, 0, ctx->stream>>>(c.useq, up, T, d, D, batch);
+            ctx->launches += 1;
+        } else {
+            // pageable host source: the runtime has read it before the call returns
+            RXG_CUDA(ctx, cudaMemcpyAsync(up, useq_pad.data(), useq_pad.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+            c2.useq_host = useq_pad.data();
+        }
+        c2.useq = up;
+    }
     c2.po = PeerOut{};                       // the embedded sweep writes padded rows: no in-kernel peer stores
     c2.want_cov_table = false; c2.cov_table = nullptr; c2.ev_tables = nullptr;
     if (!c.tables_only) {
@@ -254,6 +352,7 @@ int lgssm_dispatch(rxg_ctx* ctx, LgssmCall& c) {
         return lgssm_generic_chain(ctx, c);
     }
     if (lgssm_large_supported(c.d, c.m)) {
+        if (c.useq) return large_with_offset(ctx, c);
         if (c.u) {
             bool nz = false;
             for (int i = 0; i < c.d; ++i) nz |= (c.u[i] != 0.f);

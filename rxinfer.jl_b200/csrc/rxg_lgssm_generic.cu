@@ -27,6 +27,9 @@ struct GenArgs {
     int per_chain;                       // model arrays carry a trailing [batch] axis
     const float *A, *B, *P, *Q, *m0, *S0, *u;     // device pointers (shared: row-major; per chain: [..][batch])
     const float* mean0_chain;            // [d][batch] or null
+    const float* useq;                   // per-step inputs (replace u): row t at useq + t * d * ustride (+ b if uchain)
+    int64_t ustride;
+    int uchain;
     const float* y;
     const uint8_t* mask;
     float *mean, *cov, *nle;
@@ -183,6 +186,10 @@ __global__ void __launch_bounds__(256) lgssm_generic_chain_kernel(GenArgs g) {
         // ---------------------------------------------------------------- forward
         for (int t = 0; t < g.T; ++t) {
             if (t > 0 || g.transition_first) {
+                if (g.useq) {
+                    for (int i = threadIdx.x; i < d; i += blockDim.x) v_u[i] = g.useq[((int64_t)t * d + i) * g.ustride + b * g.uchain];
+                    __syncthreads();
+                }
                 g_mulv(v_t, sA, v_mu, v_u, d, d, ld);                 // mu <- A mu + u
                 for (int i = threadIdx.x; i < d; i += blockDim.x) v_mu[i] = v_t[i];
                 g_mul_nn(sT, sA, sS, nullptr, d, d, d, ld);           // T = A S
@@ -235,6 +242,8 @@ __global__ void __launch_bounds__(256) lgssm_generic_chain_kernel(GenArgs g) {
                 for (int e = threadIdx.x; e < d * d; e += blockDim.x)
                     sS[(e / d) * ld + e % d] = g.cov[((int64_t)t * d * d + e) * g.batch + b];
                 for (int i = threadIdx.x; i < d; i += blockDim.x) v_mu[i] = g.mean[((int64_t)t * d + i) * g.batch + b];
+                if (g.useq)       // the transition into x[t+1]
+                    for (int i = threadIdx.x; i < d; i += blockDim.x) v_u[i] = g.useq[((int64_t)(t + 1) * d + i) * g.ustride + b * g.uchain];
                 __syncthreads();
                 g_mul_nn(sT, sA, sS, nullptr, d, d, d, ld);           // T = A Sf
                 g_sym_nt(sL, sT, sA, sP, d, d, ld);                   // L = A Sf A' + P = Sp(t+1)
@@ -311,6 +320,7 @@ int lgssm_generic_chain(rxg_ctx* ctx, const LgssmCall& c) {
         g.A = dA; g.B = dB; g.P = dP; g.Q = dQ; g.S0 = dS0; g.m0 = dm0; g.u = c.u ? du : nullptr;
     }
     g.mean0_chain = c.mean0_chain;
+    g.useq = c.useq; g.ustride = c.useq_chain ? c.batch : 1; g.uchain = c.useq_chain ? 1 : 0;
     g.y = c.y; g.mask = c.ymask; g.mean = c.mean; g.cov = c.cov; g.nle = c.nle; g.status = c.status;
     g.smooth = c.smooth ? 1 : 0;
     g.transition_first = (c.flags & RXG_TRANSITION_FIRST) ? 1 : 0;

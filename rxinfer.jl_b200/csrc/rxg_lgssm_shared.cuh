@@ -120,16 +120,92 @@ __device__ __forceinline__ void peer_store(const PeerOut& po, int write_cov, int
     }
 }
 
+// u[t] of one step for this thread's CPT chains: per-chain input sequence useq[rows][D][batch]
+template <int D, int CPT>
+__device__ __forceinline__ void load_input(const float* __restrict__ useq, int t, int64_t batch, int64_t b, float (&u)[D][CPT]) {
+#pragma unroll
+    for (int i = 0; i < D; ++i) Pack<CPT>::ld(useq + ((int64_t)t * D + i) * batch + b, u[i]);
+}
+
+// USEQ forward step: nm = F mu + K (y_t - B u_t) + u_t
+template <int D, int M, int CPT>
+__device__ __forceinline__ void input_step(const float* Ft, const float* Kt, const float* Bm, const float (&mu)[D][CPT],
+                                           const float (&yt)[M][CPT], const float (&ut)[D][CPT], float (&nm)[D][CPT]) {
+    float ye[M][CPT];
+#pragma unroll
+    for (int k = 0; k < M; ++k)
+#pragma unroll
+        for (int c = 0; c < CPT; ++c) {
+            float a = yt[k][c];
+#pragma unroll
+            for (int j = 0; j < D; ++j) a = __fmaf_rn(-Bm[k * D + j], ut[j][c], a);
+            ye[k][c] = a;
+        }
+#pragma unroll
+    for (int i = 0; i < D; ++i)
+#pragma unroll
+        for (int c = 0; c < CPT; ++c) {
+            float a = __fmaf_rn(Ft[i * D], mu[0][c], ut[i][c]);
+#pragma unroll
+            for (int j = 1; j < D; ++j) a = __fmaf_rn(Ft[i * D + j], mu[j][c], a);
+#pragma unroll
+            for (int k = 0; k < M; ++k) a = __fmaf_rn(Kt[i * M + k], ye[k][c], a);
+            nm[i][c] = a;
+        }
+}
+// USEQ backward step: nm = E mu_f[t] + G (mu_s[t+1] - u_{t+1})   (record T-1 has G = 0: no row T is read)
+template <int D, int CPT>
+__device__ __forceinline__ void input_back(const float* Et, const float* Gt, const float (&fm)[D][CPT], const float (&ms)[D][CPT],
+                                           const float* __restrict__ useq, int t, int T, int64_t batch, int64_t b,
+                                           float (&nm)[D][CPT]) {
+    float gv[D][CPT];
+#pragma unroll
+    for (int i = 0; i < D; ++i)
+#pragma unroll
+        for (int c = 0; c < CPT; ++c) gv[i][c] = ms[i][c];
+    if (t + 1 < T) {
+        float un[D][CPT];
+        load_input<D, CPT>(useq, t + 1, batch, b, un);
+#pragma unroll
+        for (int i = 0; i < D; ++i)
+#pragma unroll
+            for (int c = 0; c < CPT; ++c) gv[i][c] -= un[i][c];
+    }
+#pragma unroll
+    for (int i = 0; i < D; ++i)
+#pragma unroll
+        for (int c = 0; c < CPT; ++c) {
+            float a = Et[i * D] * fm[0][c];
+#pragma unroll
+            for (int j = 1; j < D; ++j) a = __fmaf_rn(Et[i * D + j], fm[j][c], a);
+#pragma unroll
+            for (int j = 0; j < D; ++j) a = __fmaf_rn(Gt[i * D + j], gv[j][c], a);
+            nm[i][c] = a;
+        }
+}
+
 // PEER: the final posteriors are also stored to the peer ranks' gathered buffers (fused all-gather, rxg_peer.cu).
 // A separate instantiation, because the kernel is instruction-cache sensitive: the loops over peers inside the
 // unrolled step bodies took the single-GPU kernel from 3.4 K to 11 K instructions.
-template <int D, int M, int CPT, int PF, bool SMOOTH, bool EVID, bool OFFSET, bool CKPT, bool PEER = false>
-__global__ void __launch_bounds__(32, 16 / CPT)   // CPT=1: <= 128 regs so ~14 warps/SM stay resident; wider CPT trades warps for ILP
+// USEQ = 1: per-chain input sequence (RXG_U_SEQ_CHAIN, useq[rows][D][batch]), streamed beside y; the gain tables are
+// those without inputs (OFFSET = false) and the inputs enter the mean recursions directly:
+//     forward   mu_f[t] = F_t mu_f[t-1] + K_t (y_t - B u_t) + u_t     (EVID: innovation y_t - B (A mu_f[t-1] + u_t))
+//     backward  mu_s[t] = E_t mu_f[t] + G_t (mu_s[t+1] - u_{t+1})
+// USEQ = 2: shared input sequence (RXG_U_SEQ_SHARED, useq[rows][D]) with evidence: the tables carry the offsets
+// gf_t, gb_t (OFFSET = true) and only the explicit evidence form reads u_t (uniform over the warp) where the constant
+// offset reads mdl.u.
+// Separate instantiations: every other one compiles to the code it had without them.
+// (USEQ at d * m > 16 with one chain per thread: <= 168 registers, 128 would spill)
+template <int D, int M, int CPT, int PF, bool SMOOTH, bool EVID, bool OFFSET, bool CKPT, bool PEER = false, int USEQ = 0>
+__global__ void __launch_bounds__(32, (USEQ != 0 && D * M > 16 && CPT == 1) ? 12 : 16 / CPT)   // CPT=1: <= 128 regs so ~14 warps/SM stay resident; wider CPT trades warps for ILP
 lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __restrict__ fwd_tab,
                     const float* __restrict__ bwd_tab, const float* __restrict__ sf_tab,
                     const float* __restrict__ y, float* __restrict__ mean, float* __restrict__ cov,
                     float* __restrict__ nle, int T, int64_t batch, int transition_first,
-                    int write_cov, const float* __restrict__ mu0c, const __grid_constant__ PeerOut po) {
+                    int write_cov, const float* __restrict__ mu0c, const __grid_constant__ PeerOut po,
+                    const float* __restrict__ useq = nullptr) {
+    static_assert(USEQ == 0 || (!PEER && OFFSET == (USEQ == 2) && (USEQ == 1 || EVID)),
+                  "input sequences: per chain without table offsets, shared with them (evidence form only); no peer stores");
     using TB = Tab<D, M>;
     // CKPT (smoothing only): the forward pass keeps one filtered mean per TC-step chunk; the backward
     // pass re-reads y and recomputes the chunk's filtered means into s_f (lane-contiguous, private
@@ -194,11 +270,32 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
                 float Kt[pad4(D * M)];
                 load_smem<pad4(D * M)>(rec + TB::K_OFF, Kt);
                 float nm[D][CPT];
+                float ut[D][CPT];                   // u_t (USEQ; zero at a step without a transition)
+                if constexpr (USEQ == 2) {
+#pragma unroll
+                    for (int i = 0; i < D; ++i) {
+                        const float v = (t > 0 || transition_first) ? __ldg(useq + (size_t)t * D + i) : 0.f;
+#pragma unroll
+                        for (int c = 0; c < CPT; ++c) ut[i][c] = v;
+                    }
+                }
+                if constexpr (USEQ == 1) {
+                    if (t > 0 || transition_first) load_input<D, CPT>(useq, t, batch, b, ut);
+                    else
+#pragma unroll
+                        for (int i = 0; i < D; ++i)
+#pragma unroll
+                            for (int c = 0; c < CPT; ++c) ut[i][c] = 0.f;
+                }
                 if (!EVID) {
                     // mu_f[t] = F_t mu_f[t-1] + K_t y_t,  F_t = (I - K_t B) A   (rules #1-#4 + product)
                     float Ft[pad4(D * D)], gf[pad4(D)];
                     load_smem<pad4(D * D)>(rec + TB::F_OFF, Ft);
                     if (OFFSET) load_smem<pad4(D)>(rec + TB::GF_OFF, gf);        // (I - K B) u: the fused `+` rule
+                    if constexpr (USEQ == 1) {
+                        // mu_f[t] = F_t mu_f[t-1] + K_t (y_t - B u_t) + u_t
+                        input_step<D, M, CPT>(Ft, Kt, mdl.B, mu, ycur[s], ut, nm);
+                    } else {
 #pragma unroll
                     for (int i = 0; i < D; ++i)
 #pragma unroll
@@ -210,6 +307,7 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
                             for (int k = 0; k < M; ++k) a = __fmaf_rn(Kt[i * M + k], ycur[s][k][c], a);
                             nm[i][c] = a;
                         }
+                    }
                 } else {
                     // explicit form so that the innovation is available for the evidence
                     float Li[pad4(M * M)], cc[4];
@@ -222,7 +320,9 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
 #pragma unroll
                         for (int i = 0; i < D; ++i) {
                             if (pred) {
-                                float a = OFFSET ? __fmaf_rn(mdl.A[i * D], mu[0][c], mdl.u[i]) : mdl.A[i * D] * mu[0][c];
+                                float a;
+                                if constexpr (USEQ != 0) a = __fmaf_rn(mdl.A[i * D], mu[0][c], ut[i][c]);
+                                else a = OFFSET ? __fmaf_rn(mdl.A[i * D], mu[0][c], mdl.u[i]) : mdl.A[i * D] * mu[0][c];
 #pragma unroll
                                 for (int j = 1; j < D; ++j) a = __fmaf_rn(mdl.A[i * D + j], mu[j][c], a);
                                 mp[i] = a;
@@ -396,6 +496,17 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
                         if (OFFSET) load_smem<pad4(D)>(rec + TB::GF_OFF, gf);
                         float nm[D][CPT];
                         const bool first_no_pred = (t == 0) && !transition_first && EVID;
+                        if constexpr (USEQ == 1) {
+                            // the recompute re-reads u_t beside y_t
+                            float ut[D][CPT];
+                            if (t > 0 || transition_first) load_input<D, CPT>(useq, t, batch, b, ut);
+                            else
+#pragma unroll
+                                for (int i = 0; i < D; ++i)
+#pragma unroll
+                                    for (int c = 0; c < CPT; ++c) ut[i][c] = 0.f;
+                            input_step<D, M, CPT>(Ft, Kt, mdl.B, mu, ycur[s], ut, nm);
+                        } else {
 #pragma unroll
                         for (int i = 0; i < D; ++i)
 #pragma unroll
@@ -407,6 +518,7 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
                                 for (int kk = 0; kk < M; ++kk) a = __fmaf_rn(Kt[i * M + kk], ycur[s][kk][c], a);
                                 nm[i][c] = a;
                             }
+                        }
                         (void)first_no_pred;
 #pragma unroll
                         for (int i = 0; i < D; ++i)
@@ -439,6 +551,9 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
                     for (int i = 0; i < D; ++i)
 #pragma unroll
                         for (int c = 0; c < CPT; ++c) fm[i][c] = s_f[((slot * D + i) * CPT + c) * 32 + lane];
+                    if constexpr (USEQ == 1) {
+                        input_back<D, CPT>(Et, Gt, fm, ms, useq, t, T, batch, b, nm);
+                    } else {
 #pragma unroll
                     for (int i = 0; i < D; ++i)
 #pragma unroll
@@ -450,6 +565,7 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
                             for (int jj = 0; jj < D; ++jj) a = __fmaf_rn(Gt[i * D + jj], ms[jj][c], a);
                             nm[i][c] = a;
                         }
+                    }
 #pragma unroll
                     for (int i = 0; i < D; ++i) {
 #pragma unroll
@@ -518,6 +634,9 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
                 load_smem<pad4(D * D)>(rec + TB::G_OFF, Gt);
                 if (OFFSET) load_smem<pad4(D)>(rec + TB::GB_OFF, gb);            // -G u
                 float nm[D][CPT];
+                if constexpr (USEQ == 1) {
+                    input_back<D, CPT>(Et, Gt, fcur[s], ms, useq, t, T, batch, b, nm);
+                } else {
 #pragma unroll
                 for (int i = 0; i < D; ++i)
 #pragma unroll
@@ -529,6 +648,7 @@ lgssm_shared_kernel(const __grid_constant__ ModelF<D, M> mdl, const float* __res
                         for (int j = 0; j < D; ++j) a = __fmaf_rn(Gt[i * D + j], ms[j][c], a);
                         nm[i][c] = a;
                     }
+                }
 #pragma unroll
                 for (int i = 0; i < D; ++i) {
 #pragma unroll

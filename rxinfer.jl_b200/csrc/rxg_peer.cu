@@ -276,6 +276,8 @@ int rxg_lgssm_smooth_gather_f32(rxg_ctx* ctx, int d, int m, int T, int64_t batch
                                 const float* y, const uint8_t* ymask, float* const* gathered_mean,
                                 float* const* gathered_cov, float* neg_log_evidence, int32_t* status, unsigned flags) {
     if (!ctx) return RXG_ERR_BAD_ARG;
+    if (flags & (RXG_U_SEQ_SHARED | RXG_U_SEQ_CHAIN))
+        return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_smooth_gather: per-step input sequences (RXG_U_SEQ_*) are not supported here");
     if (!(flags & RXG_PTR_DEVICE)) return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_smooth_gather takes device pointers");
     if (ctx->peer_n < 1) return fail(ctx, RXG_ERR_BAD_ARG, "lgssm_smooth_gather: rxg_peer_group has not been called");
     if (d < 1 || m < 1 || T < 1 || batch_local < 1) return fail(ctx, RXG_ERR_BAD_ARG, "lgssm_smooth_gather: d, m, T, batch must be >= 1");

@@ -253,10 +253,13 @@ __global__ void __launch_bounds__(32) k_forecast_cov(int d, int H, const float* 
 }
 
 // Forecast means x_k = A x_{k-1} + u from mu_s[T-1], one thread per chain; the state vectors live in shared memory
-// ([d][FM_THREADS] per buffer: consecutive chains in consecutive banks).
+// ([d][FM_THREADS] per buffer: consecutive chains in consecutive banks).  With an input sequence (useq: row r at
+// useq + r * d * ustride, + b if uchain) forecast k = 1..H adds row T + k - 1 instead of u.
 __global__ void __launch_bounds__(FM_THREADS) k_forecast_mean(int d, int H, int64_t batch, const float* __restrict__ A,
                                                               const float* __restrict__ u, int64_t ms, int64_t mb,
-                                                              const float* __restrict__ last_mean, float* __restrict__ out) {
+                                                              const float* __restrict__ last_mean, float* __restrict__ out,
+                                                              const float* __restrict__ useq, int64_t ustride, int uchain,
+                                                              int T) {
     extern __shared__ float xs[];
     const int tid = threadIdx.x;
     const int64_t b = (int64_t)blockIdx.x * FM_THREADS + tid;
@@ -266,7 +269,8 @@ __global__ void __launch_bounds__(FM_THREADS) k_forecast_mean(int d, int H, int6
     for (int i = 0; i < d; ++i) x0[i * FM_THREADS + tid] = __ldg(last_mean + (int64_t)i * batch + b);
     for (int k = 0; k < H; ++k) {
         for (int i = 0; i < d; ++i) {
-            float s = u ? __ldg(u + (int64_t)i * ms + b * mb) : 0.f;
+            float s = useq ? __ldg(useq + ((int64_t)(T + k) * d + i) * ustride + b * uchain)
+                           : (u ? __ldg(u + (int64_t)i * ms + b * mb) : 0.f);
             for (int j = 0; j < d; ++j) s = __fmaf_rn(__ldg(A + (int64_t)(i * d + j) * ms + b * mb), x0[j * FM_THREADS + tid], s);
             x1[i * FM_THREADS + tid] = s;
             out[((int64_t)k * d + i) * batch + b] = s;
@@ -409,7 +413,8 @@ int lgssm_predict_post(rxg_ctx* ctx, const LgssmCall& c, const PredictArgs& p) {
         k_forecast_cov<<<(unsigned)nch, 32, smem, ctx->stream>>>(d, H, A, P, ms, mb, sig + (int64_t)(T - 1) * d * d * sig_s, sig_s,
                                                                  sig_b, fsig, route_b ? batch : 1, sig_b);
         k_forecast_mean<<<(unsigned)((batch + FM_THREADS - 1) / FM_THREADS), FM_THREADS, (size_t)2 * d * FM_THREADS * 4,
-                          ctx->stream>>>(d, H, batch, A, u, ms, mb, c.mean + (int64_t)(T - 1) * d * batch, fmean);
+                          ctx->stream>>>(d, H, batch, A, u, ms, mb, c.mean + (int64_t)(T - 1) * d * batch, fmean,
+                                         c.useq, c.useq_chain ? batch : 1, c.useq_chain ? 1 : 0, T);
         ctx->launches += 2;
         RXG_CUDA(ctx, cudaGetLastError());
     }

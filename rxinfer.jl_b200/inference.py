@@ -157,11 +157,14 @@ def _predict_keys(predictvars, model, data):
         raise NotImplementedError("predictvars / horizon: predictions of the streaming engine (datastream) are outside the "
                                   "batched hot path; pass `data`")
     if isinstance(predictvars, KeepLast):
-        predictvars = {k: KeepLast() for k in data if k != "ymask"}
+        predictvars = {k: KeepLast() for k in data if k not in ("ymask", "u")}     # known inputs are not predicted
     if not isinstance(predictvars, dict):
         raise NotImplementedError(f"predictvars={predictvars!r}: expected KeepLast() or a dict of KeepLast() values; "
                                   "run this call through stock ReactiveMP")
     for k, v in predictvars.items():
+        if k == "u":
+            raise NotImplementedError("predictvars: 'u' holds known inputs, which have no predictive distribution on the "
+                                      "batched path")
         if k not in ("y", "o"):
             raise NotImplementedError(f"predictvars: {k!r} is not a data variable of the LGSSM (y, o)")
         if not isinstance(v, KeepLast):
@@ -215,13 +218,24 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
                                  datastream=datastream, autostart=autostart, cov_shared_out=cov_shared_out)
     if "y" not in data:
         raise KeyError("data must contain the observations under key 'y'")   # reference: missing data key error
-    ctx = context or default_context()
     y = data["y"]
+    # known per-step inputs x[t] ~ A x[t-1] + u[t]: data["u"] is a host [T(+H), d] sequence shared by every chain or a
+    # CUDA [T(+H), d, batch] tensor (one sequence per chain)
+    inputs = data.get("u")
+    if inputs is not None and getattr(model, "u", None) is not None:
+        raise ValueError("the model has a constant offset u and data carries an input sequence 'u': fold the constant "
+                         "into the sequence")
+    if inputs is not None and not isinstance(model, (linear_gaussian_ssm_smoothing, linear_gaussian_ssm_filtering)):
+        raise NotImplementedError(f"data['u']: input sequences belong to the LGSSM, not {type(model).__name__}")
+    if inputs is not None and horizon > 0 and inputs.shape[0] != y.shape[0] + horizon:
+        raise ValueError(f"data['u'] needs T + horizon = {y.shape[0] + horizon} rows (the forecasts use the inputs of "
+                         f"the forecast steps), got {inputs.shape[0]}")
+    ctx = context or default_context()
     mask = data.get("ymask")
     try:
         if isinstance(model, linear_gaussian_ssm_filtering):
-            r = ctx.lgssm(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], u=model.u, smooth=False, mask=mask,
-                          want_evidence=free_energy, per_chain_model=model.per_chain, transition_first=True,
+            r = ctx.lgssm(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], u=model.u, inputs=inputs,
+                          smooth=False, mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain, transition_first=True,
                           cov_shared_out=cov_shared_out)
             q = MvNormalMeanCovariance(r["mean"], r["cov"])
             return InferenceResult(posteriors={}, history={"x_t": q}, free_energy=r["neg_log_evidence"], model=model)
@@ -231,7 +245,7 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
                                           "KeepEach() results are outside the hot path")
             if predict is not None:
                 r = ctx.lgssm_predict(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], horizon=horizon,
-                                      u=model.u, mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain,
+                                      u=model.u, inputs=inputs, mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain,
                                       cov_shared_out=cov_shared_out, transition_first=model.prior_on_previous_state,
                                       want_status=True)
                 bad = r["status"] != 0
@@ -252,8 +266,8 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
                     preds["o"] = MvNormalMeanCovariance(r["pred_mean"][T:], r["pred_cov"][T:])
                 return InferenceResult(posteriors={"x": MvNormalMeanCovariance(mean, cov)}, predictions=preds,
                                        free_energy=r["neg_log_evidence"], model=model)
-            r = ctx.lgssm(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], u=model.u, smooth=True, mask=mask,
-                          want_evidence=free_energy, per_chain_model=model.per_chain, cov_shared_out=cov_shared_out,
+            r = ctx.lgssm(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], u=model.u, inputs=inputs, smooth=True,
+                          mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain, cov_shared_out=cov_shared_out,
                           transition_first=model.prior_on_previous_state)
             return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"])},
                                    free_energy=r["neg_log_evidence"], model=model)

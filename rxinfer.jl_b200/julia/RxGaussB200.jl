@@ -44,6 +44,8 @@ const RXG_PATH_PER_CHAIN   = UInt32(1) << 4
 const RXG_TRANSITION_FIRST = UInt32(1) << 5
 const RXG_COV_REPLICATE    = UInt32(1) << 6
 const RXG_MASK_SHARED      = UInt32(1) << 7
+const RXG_U_SEQ_SHARED     = UInt32(1) << 8     # u is one input sequence for every chain: host [T][d]
+const RXG_U_SEQ_CHAIN      = UInt32(1) << 9     # u is one input sequence per chain: device [T][d][batch]
 
 const RXG_OPT_GAIN_SEQ, RXG_OPT_LARGE_SEQ, RXG_OPT_NO_UMMA, RXG_OPT_SWEEP_VARIANT, RXG_OPT_FORCE_CPT = 0, 1, 2, 3, 4
 const RXG_OPT_HOST_THREADS, RXG_OPT_HOST_COV_D2H, RXG_OPT_HOST_BCAST_MIN_MB, RXG_OPT_HOST_SLICES, RXG_OPT_GATHER_MODE = 5, 6, 7, 8, 9
@@ -486,7 +488,9 @@ struct LGSSMPattern
     u::Union{Nothing, Vector{Float64}}
     transition_first::Bool            # the prior sits on the state BEFORE the first datum (mlgssm_test.jl:8-17)
     smoothing::Bool
+    u_data::Bool                      # x[t] ~ A * x[t-1] + u[t] with `u` a data variable: known per-step inputs
 end
+LGSSMPattern(A, B, P, Q, m0, S0, u, transition_first, smoothing) = LGSSMPattern(A, B, P, Q, m0, S0, u, transition_first, smoothing, false)
 struct HGFPattern
     kappa::Float64
     omega::Float64
@@ -536,9 +540,10 @@ One fused forward(+backward) sum-product sweep over `batch` series through `rxg_
 Returns `(mean[batch, d, T], cov[batch, d, d, T], neg_log_evidence[batch] or nothing, status or nothing)`.
 """
 function sweep(ctx::Context, p::LGSSMPattern, y::Array{Float32, 3}; mask::Union{Nothing, Matrix{UInt8}} = nothing,
-               free_energy::Bool = false, status::Bool = false)
+               free_energy::Bool = false, status::Bool = false, inputs = nothing)
     batch, m, T = size(y)
     d = size(p.A, 1)
+    inputs isa Array{Float32, 3} && return sweep_chain_inputs(ctx, p, y, inputs; mask, free_energy)
     mean = Array{Float32}(undef, batch, d, T)
     cov = Array{Float32}(undef, batch, d, d, T)
     nle = free_energy ? Vector{Float32}(undef, batch) : Float32[]
@@ -547,13 +552,42 @@ function sweep(ctx::Context, p::LGSSMPattern, y::Array{Float32, 3}; mask::Union{
     m0r = rowmajor32(p.m0)
     ur = p.u === nothing ? Float32[] : rowmajor32(p.u)
     flags = p.transition_first ? RXG_TRANSITION_FIRST : UInt32(0)
+    if inputs !== nothing                 # one sequence for every series: host u[d, T] (column t = u[t]) = row-major [T][d]
+        ur = inputs::Matrix{Float32}
+        flags |= RXG_U_SEQ_SHARED
+    end
     f = p.smoothing ? Lib.lgssm_smooth : Lib.lgssm_filter
     GC.@preserve y mask mean cov nle st Ar Br Pr Qr S0r m0r ur begin
         f(ctx, d, m, T, batch, pointer(Ar), pointer(Br), pointer(Pr), pointer(Qr), pointer(m0r), pointer(S0r),
-          p.u === nothing ? NULLF : pointer(ur), pointer(y), mask === nothing ? Ptr{UInt8}(C_NULL) : pointer(mask),
+          (p.u === nothing && inputs === nothing) ? NULLF : pointer(ur), pointer(y), mask === nothing ? Ptr{UInt8}(C_NULL) : pointer(mask),
           pointer(mean), pointer(cov), free_energy ? pointer(nle) : NULLF, status ? pointer(st) : Ptr{Int32}(C_NULL), flags)
     end
     return mean, cov, free_energy ? nle : nothing, status ? st : nothing
+end
+
+# One input sequence per series (inputs[batch, d, T] = row-major [T][d][batch]): RXG_U_SEQ_CHAIN takes device pointers.
+function sweep_chain_inputs(ctx::Context, p::LGSSMPattern, y::Array{Float32, 3}, inputs::Array{Float32, 3};
+                            mask::Union{Nothing, Matrix{UInt8}} = nothing, free_energy::Bool = false)
+    batch, m, T = size(y)
+    d = size(p.A, 1)
+    dy, du = upload(ctx, y), upload(ctx, inputs)
+    dmask = mask === nothing ? C_NULL : Lib.device_alloc(ctx, sizeof(mask))
+    mask === nothing || GC.@preserve mask Lib.memcpy_h2d(ctx, dmask, Ptr{Cvoid}(pointer(mask)), sizeof(mask))
+    mean, cov = DeviceArray(ctx, batch, d, T), DeviceArray(ctx, batch, d, d, T)
+    nle = free_energy ? DeviceArray(ctx, batch) : nothing
+    Ar, Br, Pr, Qr, S0r = rowmajor32(p.A), rowmajor32(p.B), rowmajor32(p.P), rowmajor32(p.Q), rowmajor32(p.S0)
+    m0r = rowmajor32(p.m0)
+    flags = RXG_PTR_DEVICE | RXG_U_SEQ_CHAIN | (p.transition_first ? RXG_TRANSITION_FIRST : UInt32(0))
+    f = p.smoothing ? Lib.lgssm_smooth : Lib.lgssm_filter
+    try
+        GC.@preserve Ar Br Pr Qr S0r m0r begin
+            f(ctx, d, m, T, batch, pointer(Ar), pointer(Br), pointer(Pr), pointer(Qr), pointer(m0r), pointer(S0r), du.ptr, dy.ptr,
+              Ptr{UInt8}(dmask), mean.ptr, cov.ptr, nle === nothing ? NULLF : nle.ptr, Ptr{Int32}(C_NULL), flags)
+        end
+    finally
+        mask === nothing || Lib.device_free(ctx, dmask)
+    end
+    return download(mean), download(cov), nle === nothing ? nothing : download(nle), nothing
 end
 
 """
@@ -671,6 +705,14 @@ function constant_on(model, nodeprops, name::Symbol)
     end
     return nothing
 end
+# a data variable (known input) among the operands of a node other than `out`, or `nothing`
+function data_operand(model, nodeprops)
+    for (label, edge, data) in GraphPPL.neighbors(nodeprops)
+        GraphPPL.getname(edge) === :out && continue
+        GraphPPL.is_data(GraphPPL.getproperties(data)) && return label
+    end
+    return nothing
+end
 variable_on(nodeprops, name::Symbol) = begin
     for (label, edge, data) in GraphPPL.neighbors(nodeprops)
         GraphPPL.getname(edge) === name && return label
@@ -679,7 +721,7 @@ variable_on(nodeprops, name::Symbol) = begin
 end
 
 """
-    recognise(generator, one_series) -> LGSSMPattern | nothing
+    recognise(generator, one_series; inputs = nothing) -> LGSSMPattern | nothing
 
 Instantiates the GraphPPL graph of `generator` conditioned on ONE series (as `infer` does: `RxInfer.create_model(generator |
 data)`, src/model/model.jl:146-178) and pattern-matches it against the linear-Gaussian state-space chain
@@ -688,11 +730,12 @@ data)`, src/model/model.jl:146-178) and pattern-matches it against the linear-Ga
     x[t] ~ MvNormal(mean = A * x[t-1] (+ u), cov = P),   y[t] ~ MvNormal(mean = B * x[t], cov = Q)
 
 with constant A, B, P, Q shared by all steps (benchmarks/...Benchmark.ipynb:95-105; test/models/statespace/mlgssm_test.jl:8-17;
-ulgssm_tests.jl:7-16).  Anything else -- other node types, random-variable parameters, non-constant matrices, form
+ulgssm_tests.jl:7-16).  With `inputs` (one series of the data variable `u`), `x[t] ~ MvNormal(mean = A * x[t-1] + u[t], ...)` with
+`u` passed as data is recognised too: known per-step inputs, reported as `u_data = true`.  Anything else -- other node types, random-variable parameters, non-constant matrices, form
 constraints -- returns `nothing` and the caller falls back to stock ReactiveMP.
 """
-function recognise(generator, one_series)
-    model = RxInfer.getmodel(RxInfer.create_model(generator | (y = one_series,)))
+function recognise(generator, one_series; inputs = nothing)
+    model = RxInfer.getmodel(RxInfer.create_model(generator | (inputs === nothing ? (y = one_series,) : (y = one_series, u = inputs))))
     mvn = Any[]      # (label, props) of MvNormalMeanCovariance nodes
     muls = Any[]
     adds = Any[]
@@ -755,16 +798,23 @@ function recognise(generator, one_series)
         transition_first = count(==(A), As) == T
     end
     us = Any[]
+    ndata = 0                                 # `+` nodes whose operand is the data variable u[t] (known inputs)
     for props in adds
         c = constant_on(model, props, :in)
-        c === nothing && return nothing
+        if c === nothing
+            inputs !== nothing && data_operand(model, props) !== nothing || return nothing
+            ndata += 1
+            continue
+        end
         push!(us, c)
     end
     (isempty(us) || allsame(us)) || return nothing
+    ndata > 0 && !isempty(us) && return nothing          # a constant and an input on the same chain: not this pattern
+    inputs !== nothing && ndata == 0 && return nothing   # `u` is data but no transition uses it
     P = isempty(Ps) ? zeros(d, d) : first(Ps)
     return LGSSMPattern(Matrix{Float64}(A), Matrix{Float64}(B), Matrix{Float64}(P), Matrix{Float64}(first(Qs)),
                         Vector{Float64}(priors[1][1]), Matrix{Float64}(priors[1][2]),
-                        isempty(us) ? nothing : Vector{Float64}(first(us)), transition_first, true)
+                        isempty(us) ? nothing : Vector{Float64}(first(us)), transition_first, true, ndata > 0)
 end
 
 """
@@ -780,8 +830,12 @@ take.  When the model is recognised as a linear-Gaussian state-space chain with 
 function infer_batched(; model, data, iterations = nothing, free_energy = false, context::Context = default_context(),
                        constraints = nothing, initialization = nothing, returnvars = nothing, materialize::Bool = true, kwargs...)
     ys = data.y
-    stock() = map(b -> RxInfer.infer(; model, data = (y = ys[b],), iterations, free_energy, constraints, initialization, returnvars, kwargs...),
+    # every data key is forwarded per series (y, known inputs u, ...)
+    series(b) = NamedTuple{keys(data)}(map(v -> v[b], values(data)))
+    stock() = map(b -> RxInfer.infer(; model, data = series(b), iterations, free_energy, constraints, initialization, returnvars, kwargs...),
                   collect(eachindex(ys)))
+    keys(data) ⊆ (:y, :u) || return stock()
+    us = haskey(data, :u) ? data.u : nothing
     # `predictvars = (y = KeepLast(),)` is the one prediction request of the fused path; any other form (forecast nodes, KeepEach,
     # other variables) stays in the fallback list
     pv = get(kwargs, :predictvars, nothing)
@@ -790,8 +844,21 @@ function infer_batched(; model, data, iterations = nothing, free_energy = false,
     (constraints === nothing && initialization === nothing) || return stock()      # BP on a tree needs neither
     (iterations === nothing || iterations == 1) || return stock()                  # KeepEach on BP is per-iteration output
     has_missing = any(s -> any(ismissing, s), ys)
-    pattern = recognise(model, has_missing ? collect(skipmissing(first(ys))) : first(ys))
+    pattern = recognise(model, has_missing ? collect(skipmissing(first(ys))) : first(ys);
+                        inputs = us === nothing ? nothing : first(us))
     pattern === nothing && return stock()
+    # known inputs: one host sequence when every series carries the same one, else one per series (device)
+    inputs = nothing
+    if us !== nothing
+        (has_missing || predict_y) && return stock()         # predictions with inputs: stock RxInfer
+        T, d = length(first(ys)), length(pattern.m0)
+        all(s -> length(s) == T, us) || return stock()
+        inputs = if all(s -> s == first(us), us)
+            Float32[first(us)[t][i] for i in 1:d, t in 1:T]
+        else
+            Float32[us[b][t][i] for b in eachindex(us), i in 1:d, t in 1:T]
+        end
+    end
     RxInfer.ReactiveMP.is_predefined_node(MvNormalMeanCovariance)                 # touches the node registry: fails early if RxInfer is broken
     y, mask = has_missing ? pack_missing(ys) : (pack(ys), nothing)
     # the reference predicts every data variable with missing entries (batch.jl:222-227) and what predictvars asks for
@@ -802,7 +869,7 @@ function infer_batched(; model, data, iterations = nothing, free_energy = false,
             [MvNormalMeanCovariance(Float64.(ŷ[b, :, t]), Float64.(Ŝ[b, :, :, t])) for t in 1:size(ŷ, 3), b in 1:size(ŷ, 1)] :
             (mean = ŷ, cov = Ŝ)
     else
-        μ, Σ, F, _ = sweep(context, pattern, y; mask, free_energy = free_energy !== false)
+        μ, Σ, F, _ = sweep(context, pattern, y; mask, free_energy = free_energy !== false, inputs)
     end
     batch, d, T = size(μ)
     posteriors = if materialize

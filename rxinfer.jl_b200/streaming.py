@@ -21,7 +21,7 @@ class RxInferenceEngine:
     """Created by ``infer(model=..., datastream=..., autoupdates=..., keephistory=...)``.
 
     ``datastream``: an iterable of chunks (CUDA fp32 tensors ``[Tc, m, batch]``, or ``[Tc, batch]`` for the
-    HGF), or ``None`` for a push-driven engine (``engine.push(chunk)``; the reference's
+    HGF; an LGSSM chunk may also be ``{"y": ..., "u": ...}`` with the chunk's known inputs), or ``None`` for a push-driven engine (``engine.push(chunk)``; the reference's
     ``Subject``-style datastream).  ``autostart=True`` consumes an iterable datastream immediately."""
 
     def __init__(self, ctx, model, *, batch, iterations=1, keephistory=None, historyvars=None, free_energy=False,
@@ -92,10 +92,16 @@ class RxInferenceEngine:
     # -------------------------------------------------------------- one tick = one chunk (streaming.jl:344-430)
     def push(self, chunk):
         """Consume one chunk; returns the chunk's marginals (dict name -> batched distribution)."""
+        inputs = None
+        if isinstance(chunk, dict):      # {"y": [Tc, m, batch], "u": the chunk's known inputs ([Tc, d] or [Tc, d, batch])}
+            if self._kind != "lgssm" and "u" in chunk:
+                raise NotImplementedError("input sequences belong to the LGSSM streaming engine")
+            chunk, inputs = chunk["y"], chunk.get("u")
         if self._kind == "lgssm":
             mo = self.model
             r = self.ctx.lgssm_filter_chunk(chunk, mo.A, mo.B, mo.P, mo.Q, self._prev_mean, self._carry_cov, u=mo.u,
-                                            want_evidence=self.free_energy_enabled, cov_shared_out=self.cov_shared_out)
+                                            inputs=inputs, want_evidence=self.free_energy_enabled,
+                                            cov_shared_out=self.cov_shared_out)
             self._prev_mean = r["mean"][-1]              # view into this chunk's output; stays alive through the history or here
             out = {"x_t": MvNormalMeanCovariance(r["mean"], r["cov"])}
             if self.free_energy_enabled:
