@@ -5,6 +5,7 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
   python bench_extra.py [--which per_chain,filter,hgf,rules,vmp,scaling_T]
   python bench_extra.py --which predict      (opt-in: observation predictions / forecasts after the smoother)
   python bench_extra.py --which inputs       (opt-in: known per-step inputs u[t], shared and per-chain sequences)
+  python bench_extra.py --which vmp_wishart  (opt-in: Wishart-precision VMP around the smoother vs the composed path)
 """
 from __future__ import annotations
 
@@ -138,6 +139,82 @@ def bench_inputs(ctx, peak):
         torch.cuda.empty_cache()
 
 
+def vmp_wishart_counts(d, m, masked):
+    """Algorithmic bytes and FLOPs per (chain, step, iteration) of one non-final iteration of the fused Wishart VMP kernel
+    (lgssm_vmp_wishart_kernel), and the bytes of the same iteration on the composed path (per-chain smoother + a reduction
+    over T).  Bytes: y is read in both directions; the filtered mean and the lower triangle of the filtered covariance are
+    written (stash) and read back; a per-chain mask adds one byte per direction.  FLOPs: 2 x the FMAs of the step helpers
+    (predict, update, RTS step) and of the R_b accumulation, dense counts of rxg_linalg.cuh."""
+    tri = lambda n: n * (n + 1) // 2
+    stash = 4 * (d + tri(d))
+    fused = 2 * 4 * m + 2 * stash + (2 if masked else 0)
+    composed = (4 * m + 2 * stash + 4 * (d + d * d) + (1 if masked else 0)) + (4 * m + 4 * d + 4 * d * d + (1 if masked else 0))
+    predict = d * d + d ** 3 + tri(d) * d
+    update = m * d * d + tri(m) * d + m ** 3 // 6 + d * m * m // 2 + m * d + m * m // 2 + d * m + tri(d) * m
+    rts = d ** 3 + tri(d) * d + d ** 3 // 6 + d ** 3 // 2 + d ** 3 // 2 + tri(d) * d + d ** 3 + tri(d) * d + 2 * d * d
+    acc = m * d + m * m + m * d * d + tri(m) * d
+    return fused, composed, 2 * (predict + update + rts + acc)
+
+
+def _composed_wishart(ctx, y, mod, its, nu0, Psi0, W0, mask):
+    """The path users compose without the fused entry: per-chain Context.lgssm with Q_b = inv(E[w_b]), a torch
+    reduction over T and the Wishart update in torch (fp64)."""
+    T, m, nb = y.shape
+    dev = lambda M: torch.as_tensor(np.ascontiguousarray(np.broadcast_to(np.asarray(M, np.float32)[..., None],
+                                                                          np.shape(M) + (nb,))), device="cuda")
+    A, B, P, m0, S0 = (dev(mod[k]) for k in ("A", "B", "P", "m0", "S0"))
+    Bd = torch.as_tensor(mod["B"], dtype=torch.float64, device="cuda")
+    W = torch.as_tensor(W0, dtype=torch.float64, device="cuda").unsqueeze(0).repeat(nb, 1, 1)
+    obs = torch.ones(T, nb, dtype=torch.float64, device="cuda") if mask is None else mask.double()
+    for _ in range(its):
+        Q = torch.linalg.inv(W).permute(1, 2, 0).float().contiguous()
+        r = ctx.lgssm(y, A, B, P, Q, m0, S0, mask=mask, per_chain_model=True)
+        e = y.double() - torch.einsum("kd,tdb->tkb", Bd, r["mean"].double())
+        R = torch.einsum("tb,tkb,tlb->bkl", obs, e, e) + torch.einsum("tb,kd,tdeb,le->bkl", obs, Bd, r["cov"].double(), Bd)
+        W = (nu0 + obs.sum(0))[:, None, None] * torch.linalg.inv(torch.as_tensor(Psi0, device="cuda") + R)
+    return W
+
+
+def bench_vmp_wishart(ctx, peak):
+    """Fused Wishart-precision VMP (rxg_lgssm_vmp_wishart_f32) vs the composed path on the same inputs, alternated in one
+    run; kernel time from CUDA events around the launch (rxg_set_profiling)."""
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(13)
+    T, nb, its = 1000, 65536, 10
+    for d, masked in ((4, False), (4, True), (2, False)):
+        m = d
+        mod = notebook_model_f32() if d == 4 else notebook_model_d2_f32()
+        y = torch.randn(T, m, nb, device="cuda", generator=g) * 3.3
+        mask = (torch.rand(T, nb, device="cuda", generator=g) >= 0.1).to(torch.uint8) if masked else None
+        nu0, Psi0, W0 = m + 2.0, 10.0 * np.eye(m), 0.1 * np.eye(m)
+        fused = lambda: ctx.lgssm_vmp_wishart(y, mod["A"], mod["B"], mod["P"], mod["m0"], mod["S0"], iterations=its,
+                                              w_prior=(nu0, Psi0), init_E_W=W0, mask=mask)
+        composed = lambda: _composed_wishart(ctx, y, mod, its, nu0, Psi0, W0, mask)
+        call_ms, comp_ms, kern_ms = [], [], []
+        for _ in range(3):
+            call_ms.append(timed(fused, warm=2, reps=3))
+            comp_ms.append(timed(composed, warm=1, reps=2))
+            ctx.set_profiling(True)
+            fused()
+            kern_ms.append(ctx.profile_last_ms()[0])
+            ctx.set_profiling(False)
+        kms, cms, pms = float(np.median(kern_ms)), float(np.median(call_ms)), float(np.median(comp_ms))
+        bf, bc, fl = vmp_wishart_counts(d, m, masked)
+        n = T * nb * its
+        t_hbm, t_fp32 = bf * n / (peak * 1e9), fl * n / 67e12
+        print(json.dumps({"what": "Wishart-precision VMP around the smoother (lgssm_vmp_wishart_kernel)", "d": d, "m": m,
+                          "T": T, "batch": nb, "iterations": its, "mask_10pct": masked, "kernel_ms": kms, "call_ms": cms,
+                          "ms_per_iteration": kms / its, "composed_path_ms": pms, "speedup_vs_composed": pms / cms,
+                          "bytes_per_chain_step_iteration": bf, "composed_bytes_per_chain_step_iteration": bc,
+                          "flops_per_chain_step_iteration": fl, "achieved_GBs": bf * n / kms / 1e6,
+                          "achieved_TFLOPs": fl * n / kms / 1e9,
+                          "bound": "hbm" if t_hbm >= t_fp32 else "fp32",
+                          "kernel_frac_of_bound": max(t_hbm, t_fp32) * 1e3 / kms,
+                          "peak_hbm_gbs": peak, "peak_fp32_tflops": 67, "gpu": gname, "power_limit": plim}), flush=True)
+        del y, mask
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -149,6 +226,8 @@ def main():
         bench_predict(ctx, peak)
     if "inputs" in which:
         bench_inputs(ctx, peak)
+    if "vmp_wishart" in which:
+        bench_vmp_wishart(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

@@ -357,6 +357,26 @@ int rxg_lgssm_vmp_gamma_fe_f32(rxg_ctx*, int T, int64_t batch, int iterations, f
                                float m0, float v0, float a0, float b0, float init_E_tau, const float* y,
                                float* post_mean, float* post_var, float* shape, float* rate,
                                float* free_energy, unsigned flags);
+/* VMP around the multivariate smoother with an unknown observation precision MATRIX w, one per chain
+ * [ref: docs/src/manuals/model-specification.md:265-271, run with constraints = q(x, w) = q(x)q(w) and `iterations`]:
+ *   w ~ Wishart(nu0, inv(inv_scale0)); x[1] ~ N(m0, S0) (RXG_TRANSITION_FIRST: one transition earlier);
+ *   x[t] ~ N(A x[t-1] + u, P); y[t] ~ N(B x[t], inv(w)); q(x) q(w), q(x) structured over the chain.
+ * A, B, P, m0, S0, u (constant, [d] or NULL), inv_scale0 and init_E_W (= E[w] of the initial q(w)) are HOST arrays shared
+ * by all chains; the data and outputs are device arrays (RXG_PTR_DEVICE is required).  y[T][m][batch]; ymask NULL,
+ * [T][batch] (device) or, with RXG_MASK_SHARED, one host pattern [T].  Outputs: q(x) of the LAST iteration (KeepLast)
+ * in post_mean[T][d][batch] / post_cov[T][d][d][batch]; q(w) = Wishart(df, inv(inv_scale)) after EVERY iteration
+ * (KeepEach) in df[iterations][batch] / inv_scale[iterations][m][m][batch]; the Bethe free energy after every iteration
+ * in fp64, free_energy[iterations][batch] or NULL; status[batch] or NULL (RXG_ERR_NOT_SPD when a pivot of the chain's
+ * recursion or Wishart update was not positive).  Each iteration runs the Kalman filter + RTS smoother with
+ * Q = inv(E[w]), then q(w) = (nu0 + N_b, inv_scale0 + sum_observed (y - B mu)(y - B mu)' + B Sigma B').
+ * d, m in 1..6.  Flags: RXG_PTR_DEVICE, RXG_TRANSITION_FIRST, RXG_MASK_SHARED, RXG_ASYNC; others are refused with
+ * RXG_ERR_UNSUPPORTED (the covariances depend on the chain through w).  iterations >= 1, nu0 > m - 1, and SPD
+ * inv_scale0 / init_E_W, else RXG_ERR_BAD_ARG.                                                                  */
+int rxg_lgssm_vmp_wishart_f32(rxg_ctx*, int d, int m, int T, int64_t batch, int iterations, const float* A,
+                              const float* B, const float* P, const float* m0, const float* S0, const float* u,
+                              float nu0, const float* inv_scale0, const float* init_E_W, const float* y,
+                              const uint8_t* ymask, float* post_mean, float* post_cov, float* df, float* inv_scale,
+                              double* free_energy, int32_t* status, unsigned flags);
 /* Hierarchical Gaussian Filter, streaming, `iters` VMP iterations per datum
  * [ref: test/models/statespace/hgf_tests.jl:10-69; loop src/inference/streaming.jl:349-407].
  * y[T][batch]; init = (m_z, v_z, m_x, v_x); out[T][4][batch] = (m_x, v_x, m_z, v_z).            */

@@ -9,7 +9,7 @@ loudly if it is missing or no GPU is present -- there is no CPU fallback.
 from . import _lib
 from ._lib import RxGaussError
 from .distributions import (GammaShapeRate, MvNormalMeanCovariance, MvNormalWeightedMeanPrecision,
-                            NormalMeanVariance, PointMass, vague)
+                            NormalMeanVariance, PointMass, Wishart, WishartFast, vague)
 
 
 def __getattr__(name):   # lazy: these import torch
@@ -17,7 +17,8 @@ def __getattr__(name):   # lazy: these import torch
         from . import context
         return getattr(context, name)
     if name in ("infer", "InferenceResult", "linear_gaussian_ssm_smoothing", "linear_gaussian_ssm_filtering",
-                "hgf", "univariate_lgssm_gamma_precision", "kalman_gamma_streaming", "latent_autoregressive", "default_context",
+                "hgf", "univariate_lgssm_gamma_precision", "kalman_gamma_streaming", "latent_autoregressive",
+                "linear_gaussian_ssm_wishart_precision", "default_context",
                 "KeepLast", "KeepEach"):
         from . import inference
         return getattr(inference, name)

@@ -13,13 +13,16 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "librxgauss.so")
 LGSSM_SHAPES = [(1, 1), (2, 1), (2, 2), (3, 3), (4, 1), (4, 2), (4, 4), (6, 6)]
 # (source, object stem, extra flags): rxg_lgssm.cu is compiled once per (d, m) shape (explicit instantiation) + once for the dispatch
+# rxg_lgssm_vmp.cu likewise once per Wishart dimension m (d = 1..6 each) + once for the C entry
 UNITS = ([("rxg_lgssm.cu", f"rxg_lgssm_d{d}m{m}", (f"-DRXG_INST_D={d}", f"-DRXG_INST_M={m}")) for d, m in reversed(LGSSM_SHAPES)] +
+         [("rxg_lgssm_vmp.cu", f"rxg_lgssm_vmp_m{m}", (f"-DRXG_VMP_M={m}",)) for m in range(6, 0, -1)] +
          [(s, s.replace(".cu", ""), ()) for s in
           ("rxg_lgssm_large.cu", "rxg_lgssm.cu", "rxg_umma_sweep.cu", "rxg_api.cu", "rxg_peer.cu", "rxg_rules.cu", "rxg_hgf.cu",
-           "rxg_lgssm_general.cu", "rxg_lgssm_generic.cu", "rxg_lar.cu", "rxg_rules_large.cu", "rxg_predict.cu")] +
+           "rxg_lgssm_general.cu", "rxg_lgssm_generic.cu", "rxg_lar.cu", "rxg_rules_large.cu", "rxg_predict.cu",
+           "rxg_lgssm_vmp.cu")] +
          [("rxg_hostfill.cpp", "rxg_hostfill", ())])        # plain C++ (g++): host-side covariance broadcast
 SOURCES = sorted({u[0] for u in UNITS})
-HEADERS = ["rxg_internal.h", "rxg_linalg.cuh", "rxg_gain.cuh", "rxg_lgssm_common.cuh", "rxg_lgssm_shared.cuh", "rxg_lgssm_seg.cuh", "rxg_umma.cuh", "rxg_lar.cuh", os.path.join("..", "..", "include", "rxgauss.h")]
+HEADERS = ["rxg_internal.h", "rxg_linalg.cuh", "rxg_gain.cuh", "rxg_lgssm_common.cuh", "rxg_chain_step.cuh", "rxg_lgssm_shared.cuh", "rxg_lgssm_seg.cuh", "rxg_umma.cuh", "rxg_lar.cuh", os.path.join("..", "..", "include", "rxgauss.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-mavx2", "-Xcompiler", "-pthread", "--expt-relaxed-constexpr", "-Xptxas", "-v",

@@ -331,6 +331,64 @@ class Context:
                                                         _fp(pv), _fp(sh), _fp(rt), _fp(fe), L.PTR_DEVICE))
         return dict(mean=pm, var=pv, shape=sh, rate=rt, free_energy=fe)
 
+    def lgssm_vmp_wishart(self, y, A, B, P, m0, S0, iterations=10, w_prior=None, init_E_W=None, u=None, mask=None,
+                          transition_first=False, want_free_energy=False, asynchronous=False):
+        """VMP around the smoother with an unknown observation precision matrix per chain (``rxg_lgssm_vmp_wishart_f32``):
+        w ~ Wishart(nu0, inv(inv_scale0)), x[t] ~ N(A x[t-1] + u, P), y[t] ~ N(B x[t], inv(w)), q(x) q(w).
+        y[T, m, batch] on this context's device; ``mask`` as for :meth:`lgssm` ([T, batch] per chain or a [T] pattern
+        shared by every chain).  ``w_prior = (nu0, inv_scale0)`` (default (m + 1, I)); ``init_E_W`` = E[w] of the
+        initial q(w) (default: the mean of ``vague(Wishart, m)``, m * 1e12 I).  Returns dict(mean[T, d, batch],
+        cov[T, d, d, batch] of the last iteration, df[iterations, batch], inv_scale[iterations, m, m, batch] after every
+        iteration, free_energy[iterations, batch] fp64 or None, status[batch])."""
+        if y.dim() != 3:
+            raise ValueError(f"y: expected [T, m, batch], got shape {tuple(y.shape)}")
+        T, m, batch = y.shape
+        d = np.asarray(A).shape[-1]
+        iterations = int(iterations)
+        if iterations < 1:
+            raise ValueError(f"iterations must be >= 1, got {iterations}")
+        nu0, inv_scale0 = (m + 1.0, np.eye(m)) if w_prior is None else w_prior
+        if init_E_W is None:
+            init_E_W = m * 1e12 * np.eye(m)                     # mean of vague(Wishart, m): df = m, scale 1e12 I
+        shapes = dict(A=(d, d), B=(m, d), P=(d, d), m0=(d,), S0=(d, d), inv_scale0=(m, m), init_E_W=(m, m))
+        mats = dict(A=A, B=B, P=P, m0=m0, S0=S0, inv_scale0=inv_scale0, init_E_W=init_E_W)
+        if u is not None:
+            shapes["u"], mats["u"] = (d,), u
+        keep = {}
+        for k, v in mats.items():
+            a, p = _model32(v)
+            if a.shape != shapes[k]:
+                raise ValueError(f"{k}: expected shape {shapes[k]}, got {a.shape}")
+            keep[k] = (a, p)
+        self._io(y, "y", True)
+        flags = L.PTR_DEVICE
+        mask_p = ctypes.cast(c_void_p(None), L.u8p)
+        if mask is not None and getattr(mask, "ndim", 2) == 1:
+            sm = np.ascontiguousarray(np.asarray(mask.cpu() if isinstance(mask, torch.Tensor) else mask, dtype=np.uint8))
+            if sm.shape != (T,):
+                raise ValueError(f"shared mask: expected shape ({T},), got {sm.shape}")
+            keep["mask"] = sm
+            mask_p = sm.ctypes.data_as(L.u8p)
+            flags |= L.MASK_SHARED
+        elif mask is not None:
+            self._io(mask, "mask", True, dtype=torch.uint8, shape=(T, batch))
+            mask_p = ctypes.cast(c_void_p(mask.data_ptr()), L.u8p)
+        if transition_first:
+            flags |= L.TRANSITION_FIRST
+        if asynchronous:
+            flags |= L.ASYNC
+        mean, cov = self.empty(T, d, batch), self.empty(T, d, d, batch)
+        df, iS = self.empty(iterations, batch), self.empty(iterations, m, m, batch)
+        fe = self.empty(iterations, batch, dtype=torch.float64) if want_free_energy else None
+        st = self.empty(batch, dtype=torch.int32)
+        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
+        up = keep["u"][1] if "u" in keep else L.as_fp(0)
+        self._check(self.lib.rxg_lgssm_vmp_wishart_f32(
+            self.h, d, m, T, batch, iterations, keep["A"][1], keep["B"][1], keep["P"][1], keep["m0"][1], keep["S0"][1], up,
+            float(nu0), keep["inv_scale0"][1], keep["init_E_W"][1], _fp(y), mask_p, _fp(mean), _fp(cov), _fp(df), _fp(iS),
+            fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
+        return dict(mean=mean, cov=cov, df=df, inv_scale=iS, free_energy=fe, status=st)
+
     # ------------------------------------------------------------------ per-rule kernels
     def _mat(self, M):
         """PointMass matrix operand: host array => shared; CUDA tensor [r,c,n] => per message."""

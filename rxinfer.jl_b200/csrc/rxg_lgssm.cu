@@ -24,6 +24,7 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include "rxg_chain_step.cuh"
 #include "rxg_gain.cuh"
 #include "rxg_internal.h"
 #include "rxg_linalg.cuh"
@@ -93,40 +94,15 @@ lgssm_chain_kernel(const __grid_constant__ ModelF<D, M> mdl, PerChainPtrs pc,
             if (mask) onext = mask[(int64_t)(t + 1) * batch + b];
         }
         if (t > 0 || transition_first) {
-            // rule #1  *(:out): (A mu, A S A')   rule #2  MvNormalMeanCovariance(:out): + P
-            //          (+ the `+` rule with a PointMass operand: pure mean shift by u)
-            mu = mulv(A, mu);
-            if (USEQ)
+            if constexpr (USEQ)
+                chain_predict(A, P, u, [&](Vec<float, D>& uu) {
 #pragma unroll
-                for (int i = 0; i < D; ++i) u(i) = __ldg(useq + ((int64_t)t * D + i) * ustride + b * uchain);
-#pragma unroll
-            for (int i = 0; i < D; ++i) mu(i) += u(i);
-            Mat<float, D, D> AS = mul(A, S);
-            S = sym_mul_nt_add(AS, A, P);
+                    for (int i = 0; i < D; ++i) uu(i) = __ldg(useq + ((int64_t)t * D + i) * ustride + b * uchain);
+                }, mu, S);
+            else
+                chain_predict(A, P, u, NoInput{}, mu, S);
         }
-        if (observed) {
-            // rules #3,#4 (observation message) folded with the product at x_t, gain form:
-            //   Sinn = B S B' + Q = L L',  V = S B' L^-T,  mu += V L^-1 (y - B mu),  S -= V V'
-            Mat<float, M, D> BS = mul(B, S);
-            Mat<float, M, M> Sinn = sym_mul_nt_add(BS, B, Q);
-            Chol<float, M> ch = want_nle ? cholesky<float, M, true>(Sinn, bad)
-                                         : cholesky<float, M, false>(Sinn, bad);
-            Mat<float, D, M> V = solve_right_Lt(transpose(BS), ch.L);
-            Vec<float, M> e = mulv(B, mu);
-#pragma unroll
-            for (int k = 0; k < M; ++k) e(k) = yt(k) - e(k);
-            Vec<float, M> z = solve_L(ch.L, e);
-            Vec<float, D> dm = mulv(V, z);
-#pragma unroll
-            for (int i = 0; i < D; ++i) mu(i) += dm(i);
-            S = sym_downdate(S, V);
-            if (want_nle) {
-                float q = 0.f;
-#pragma unroll
-                for (int k = 0; k < M; ++k) q = __fmaf_rn(z(k), z(k), q);
-                acc_nle += (double)(0.5f * q - ch.neg_half_logdet) + M * RXG_HALF_LOG_2PI;
-            }
-        }
+        if (observed) chain_update(B, Q, yt, want_nle, mu, S, bad, acc_nle);
         // filtered (mu, Sigma): the filter's output, the smoother's stash (lower triangle only)
 #pragma unroll
         for (int i = 0; i < D; ++i) mean[((int64_t)t * D + i) * batch + b] = mu(i);
@@ -177,24 +153,13 @@ lgssm_chain_kernel(const __grid_constant__ ModelF<D, M> mdl, PerChainPtrs pc,
 #pragma unroll
                     for (int j = 0; j <= i; ++j) pS[q++] = cov[(((int64_t)tp * D + i) * D + j) * batch + b];
             }
-            // Sp = A Sf A' + P (the forward message into x_{t+1}); RTS gain G = Sf A' Sp^-1
-            Mat<float, D, D> AS = mul(A, Sf);
-            Mat<float, D, D> Sp = sym_mul_nt_add(AS, A, P);
-            Chol<float, D> ch = cholesky<float, D, false>(Sp, bad);
-            Mat<float, D, D> U = solve_right_Lt(transpose(AS), ch.L);   // Sf A' L^-T
-            Mat<float, D, D> G = solve_right_L(U, ch.L);
-            Mat<float, D, D> C = sym_downdate(Sf, U);                   // cov(x_t | x_{t+1})
-            Mat<float, D, D> GS = mul(G, Ss);
-            Ss = sym_mul_nt_add(GS, G, C);
-            Vec<float, D> mup = mulv(A, muf);
-            if (USEQ)       // the transition into x[t+1]
+            if constexpr (USEQ)
+                chain_rts(A, P, u, [&](Vec<float, D>& uu) {      // the transition into x[t+1]
 #pragma unroll
-                for (int i = 0; i < D; ++i) u(i) = __ldg(useq + ((int64_t)(t + 1) * D + i) * ustride + b * uchain);
-#pragma unroll
-            for (int i = 0; i < D; ++i) mup(i) = mus(i) - (mup(i) + u(i));
-            Vec<float, D> dm = mulv(G, mup);
-#pragma unroll
-            for (int i = 0; i < D; ++i) mus(i) = muf(i) + dm(i);
+                    for (int i = 0; i < D; ++i) uu(i) = __ldg(useq + ((int64_t)(t + 1) * D + i) * ustride + b * uchain);
+                }, muf, Sf, mus, Ss, bad);
+            else
+                chain_rts(A, P, u, NoInput{}, muf, Sf, mus, Ss, bad);
 #pragma unroll
             for (int i = 0; i < D; ++i) mean[((int64_t)t * D + i) * batch + b] = mus(i);
 #pragma unroll

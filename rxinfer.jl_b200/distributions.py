@@ -85,6 +85,19 @@ class WishartFast:
     invS: torch.Tensor
 
 
+@dataclass
+class Wishart:
+    """``Wishart(df, scale)`` as a model is written (a prior or an initial marginal): host ``scale[m, m]``."""
+    df: float
+    scale: object
+
+    def inv_scale(self):
+        return np.linalg.inv(np.asarray(self.scale, dtype=np.float64))
+
+    def mean(self):
+        return float(self.df) * np.asarray(self.scale, dtype=np.float64)
+
+
 def vague(kind, like: torch.Tensor):
     """``vague(NormalMeanVariance)`` = N(0, 1e12); ``vague(GammaShapeRate)`` = Gamma(1, 1e-12)
     (TinyHugeNumbers, upstream)."""

@@ -18,7 +18,7 @@ import torch
 
 from . import _lib as L
 from .context import Context
-from .distributions import GammaShapeRate, MvNormalMeanCovariance, NormalMeanVariance
+from .distributions import GammaShapeRate, MvNormalMeanCovariance, NormalMeanVariance, Wishart, WishartFast
 
 
 # --------------------------------------------------------------------------- recognised models
@@ -89,6 +89,23 @@ class latent_autoregressive:
     x0_prior_precision: float = 1.0
     init_gamma: tuple = (1.0, 1.0)          # q(gamma) of the @initialization
     init_theta_precision: float = 1.0       # q(theta) = N(0, I / init_theta_precision)
+
+
+@dataclass
+class linear_gaussian_ssm_wishart_precision:
+    """LGSSM observed with an unknown precision MATRIX per series
+    (/root/reference/docs/src/manuals/model-specification.md:265-271):
+    ``w ~ w_prior; x[1] ~ x0; x[t] ~ N(A x[t-1] + u, P); y[t] ~ N(B x[t], precision = w)``, run with
+    ``constraints = q(x, w) = q(x)q(w)``, ``initialization = q(w) = w_init`` and ``iterations``.  ``w_prior`` and
+    ``w_init`` are ``Wishart(df, scale)`` as the model writes them; ``x0 = (mean, cov)``."""
+    A: np.ndarray
+    B: np.ndarray
+    P: np.ndarray
+    x0: tuple
+    w_prior: Wishart
+    w_init: Wishart
+    u: object = None
+    prior_on_previous_state: bool = False
 
 
 class KeepLast:
@@ -201,6 +218,16 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             raise NotImplementedError(f"options {sorted(bad)} are outside the batched hot path")
     if data is not None and datastream is not None:
         raise ValueError("`data` and `datastream` are mutually exclusive")    # reference: inference.jl argument check
+    if isinstance(model, linear_gaussian_ssm_wishart_precision):
+        if predictvars is not None:
+            raise NotImplementedError("predictvars: predictions of the Wishart-precision LGSSM are outside the batched hot path")
+        if data is not None and "u" in data:
+            raise NotImplementedError("data['u']: input sequences on the Wishart-precision LGSSM are outside the batched hot "
+                                      "path (a constant offset is model.u)")
+        if isinstance(returnvars, dict) and isinstance(returnvars.get("x"), KeepEach):
+            raise NotImplementedError("returnvars: q(x) is kept for the last iteration only (KeepLast) on the batched path")
+        if data is None:
+            raise ValueError("the Wishart-precision LGSSM needs `data` (it has no streaming form)")
     horizon = getattr(model, "horizon", 0) if isinstance(model, linear_gaussian_ssm_smoothing) else 0
     if isinstance(model, linear_gaussian_ssm_filtering) and horizon:
         raise NotImplementedError("horizon > 0 belongs to the smoothing LGSSM")
@@ -295,6 +322,20 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             return InferenceResult(posteriors={"x": NormalMeanVariance(r["mean"], r["var"]),
                                                "τ": GammaShapeRate(r["shape"], r["rate"])}, model=model,
                                    free_energy=r["free_energy"])
+        if isinstance(model, linear_gaussian_ssm_wishart_precision):
+            r = ctx.lgssm_vmp_wishart(y, model.A, model.B, model.P, model.x0[0], model.x0[1], iterations=iterations or 1,
+                                      w_prior=(model.w_prior.df, model.w_prior.inv_scale()), init_E_W=model.w_init.mean(),
+                                      u=model.u, mask=mask, transition_first=model.prior_on_previous_state,
+                                      want_free_energy=bool(free_energy))
+            bad = r["status"] != 0
+            if bool(bad.any()):
+                codes = sorted({L.STATUS_NAMES.get(int(c), str(int(c))) for c in r["status"][bad].unique().tolist()})
+                raise L.RxGaussError(L.RXG_ERR_NOT_SPD if "NOT_SPD" in codes else int(r["status"][bad][0]),
+                                     f"{int(bad.sum())} of {bad.numel()} chains flagged {codes}")
+            # returnvars of the reference's call under `iterations`: x = KeepLast() here, w = KeepEach() (iteration axis)
+            return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]),
+                                               "w": WishartFast(r["df"], r["inv_scale"])},
+                                   model=model, free_energy=r["free_energy"])
         if isinstance(model, latent_autoregressive):
             yy = y[:, 0] if y.dim() == 3 else y
             r = ctx.lar_vmp(yy.contiguous(), model.order, model.tau, iterations=iterations or 1, gamma_prior=model.gamma_prior,

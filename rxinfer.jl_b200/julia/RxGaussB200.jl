@@ -206,6 +206,11 @@ hgf_filter_fe(ctx, T, batch, its, kappa, omega, zvar, yvar, init, prev, y, out, 
 stream_vmp_gamma(ctx, T, batch, its, w, init, prev, y, out, fe, fl) =
     check(ctx, ccall((:rxg_stream_vmp_gamma_f32, LIB), Cint,
         (Ptr{Cvoid}, Cint, Int64, Cint, Cfloat, F32P, F32P, F32P, F32P, F32P, Cuint), ctx.handle, T, batch, its, w, init, prev, y, out, fe, fl))
+lgssm_vmp_wishart(ctx, d, m, T, batch, its, A, B, P, m0, S0, u, nu0, iS0, EW0, y, mask, mean, cov, df, iS, fe, st, fl) =
+    check(ctx, ccall((:rxg_lgssm_vmp_wishart_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, Cfloat, F32P, F32P, F32P, Ptr{UInt8},
+         F32P, F32P, F32P, F32P, Ptr{Float64}, Ptr{Int32}, Cuint),
+        ctx.handle, d, m, T, batch, its, A, B, P, m0, S0, u, nu0, iS0, EW0, y, mask, mean, cov, df, iS, fe, st, fl))
 mv_iid_wishart_vmp(ctx, d, N, batch, its, mu0, L0, nu0, iS0, EP0, y, mm, mc, df, iS, st, fl) =
     check(ctx, ccall((:rxg_mv_iid_wishart_vmp_f32, LIB), Cint,
         (Ptr{Cvoid}, Cint, Cint, Int64, Cint, F32P, F32P, Cfloat, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Int32}, Cuint),
@@ -666,6 +671,35 @@ function mv_iid_wishart(ctx::Context, y::Array{Float32, 3}; iterations = 10)
     GC.@preserve mu0 L0 iS0 EP0 Lib.mv_iid_wishart_vmp(ctx, d, N, batch, iterations, pointer(mu0), pointer(L0), Float32(d + 1), pointer(iS0),
                                                        pointer(EP0), dy.ptr, mm.ptr, mc.ptr, df.ptr, iS.ptr, Ptr{Int32}(C_NULL), RXG_PTR_DEVICE)
     return download(mm), download(mc), download(df), download(iS)
+end
+
+"""VMP around the multivariate smoother with an unknown observation precision matrix per series
+(`rxg_lgssm_vmp_wishart_f32`; model-specification.md:265-271 with `constraints = q(x, w) = q(x)q(w)`); host data
+`y[batch, m, T]`.  `w_prior = (df, inverse scale)` of the Wishart prior (default `(m + 1, I)`); `init_E_W` = E[w] of the
+initial q(w) (default: the mean of `vague(Wishart, m)`).  Returns q(x) of the last iteration (mean `[batch, d, T]`, cov
+`[batch, d, d, T]`), q(w) after every iteration (df `[batch, iterations]`, inverse scale `[batch, m, m, iterations]`), the
+Bethe free energy `[batch, iterations]` (Float64) and the per-series status."""
+function lgssm_wishart(ctx::Context, y::Array{Float32, 3}; A::Matrix, B::Matrix, P::Matrix, x0 = nothing, u = nothing,
+                       iterations = 10, w_prior = nothing, init_E_W = nothing, transition_first = false)
+    batch, m, T = size(y)
+    d = size(A, 1)
+    m0, S0 = x0 === nothing ? (zeros(Float32, d), Matrix{Float32}(100I, d, d)) : (Float32.(x0[1]), Float32.(x0[2]))
+    nu0, iS0 = w_prior === nothing ? (Float32(m + 1), Matrix{Float32}(I, m, m)) : (Float32(w_prior[1]), Float32.(w_prior[2]))
+    EW0 = init_E_W === nothing ? Matrix{Float32}(m * 1f12 * I, m, m) : Float32.(init_E_W)
+    # row-major host matrices for the C side
+    At, Bt, Pt, S0t, iS0t, EW0t = (Matrix{Float32}(permutedims(M)) for M in (A, B, P, S0, iS0, EW0))
+    uv = u === nothing ? nothing : Float32.(u)
+    dy = upload(ctx, y)
+    mean, cov = DeviceArray(ctx, batch, d, T), DeviceArray(ctx, batch, d, d, T)
+    df, iS = DeviceArray(ctx, batch, iterations), DeviceArray(ctx, batch, m, m, iterations)
+    dfe = DeviceArray(ctx, 2 * batch * iterations)                  # fp64 output: two Float32 slots per value
+    st = DeviceArray(ctx, batch)
+    fl = RXG_PTR_DEVICE | (transition_first ? RXG_TRANSITION_FIRST : UInt32(0))
+    GC.@preserve At Bt Pt m0 S0t uv iS0t EW0t Lib.lgssm_vmp_wishart(ctx, d, m, T, batch, iterations, pointer(At), pointer(Bt),
+        pointer(Pt), pointer(m0), pointer(S0t), uv === nothing ? NULLF : pointer(uv), nu0, pointer(iS0t), pointer(EW0t), dy.ptr,
+        Ptr{UInt8}(C_NULL), mean.ptr, cov.ptr, df.ptr, iS.ptr, Ptr{Float64}(dfe.ptr), Ptr{Int32}(st.ptr), fl)
+    fe = reshape(reinterpret(Float64, vec(download(dfe))), batch, iterations)
+    return download(mean), download(cov), download(df), download(iS), fe, reinterpret(Int32, download(st))
 end
 
 """Fused structured VMP of the latent autoregressive model (lar_tests.jl:52-122); `y[batch, T]`.  Returns the reference's
