@@ -24,6 +24,8 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include <utility>
+
 #include "rxg_chain_step.cuh"
 #include "rxg_gain.cuh"
 #include "rxg_internal.h"
@@ -31,6 +33,7 @@
 #include "rxg_lgssm_common.cuh"
 #include "rxg_lgssm_shared.cuh"
 #include "rxg_lgssm_seg.cuh"
+#include "rxg_sweep_select.h"
 
 namespace rxg {
 
@@ -345,6 +348,20 @@ static void fill_model(ModelF<D, M>& mdl, const LgssmCall& c) {
     for (int i = 0; i < D; ++i) { mdl.m0[i] = c.m0[i]; mdl.u[i] = c.u ? c.u[i] : 0.f; }
 }
 
+template <int D, int M, bool PER_CHAIN, bool SMOOTH>
+static void launch_chain(rxg_ctx* ctx, const LgssmCall& c, const ModelF<D, M>& mdl, const PerChainPtrs& pc) {
+    const int threads = 64;
+    const unsigned blocks = (unsigned)((c.batch + threads - 1) / threads);
+    const int tf = (c.flags & RXG_TRANSITION_FIRST) ? 1 : 0;
+    if (c.useq)
+        lgssm_chain_kernel<D, M, PER_CHAIN, SMOOTH, true><<<blocks, threads, 0, ctx->stream>>>(
+            mdl, pc, c.y, c.ymask, c.mean, c.cov, c.nle, c.status, c.T, c.batch, tf, c.useq, c.useq_chain ? c.batch : 1,
+            c.useq_chain ? 1 : 0);
+    else
+        lgssm_chain_kernel<D, M, PER_CHAIN, SMOOTH><<<blocks, threads, 0, ctx->stream>>>(
+            mdl, pc, c.y, c.ymask, c.mean, c.cov, c.nle, c.status, c.T, c.batch, tf);
+}
+
 template <int D, int M>
 static int run_chain_family(rxg_ctx* ctx, LgssmCall& c) {
     ModelF<D, M> mdl = {};
@@ -352,100 +369,50 @@ static int run_chain_family(rxg_ctx* ctx, LgssmCall& c) {
     const bool per_chain = (c.flags & RXG_MODEL_PER_CHAIN) != 0;
     if (per_chain) pc = PerChainPtrs{c.A, c.B, c.P, c.Q, c.m0, c.S0, c.u};
     else fill_model<D, M>(mdl, c);
-    const int threads = 64;
-    const unsigned blocks = (unsigned)((c.batch + threads - 1) / threads);
-    const int tf = (c.flags & RXG_TRANSITION_FIRST) ? 1 : 0;
-    const int64_t ustride = c.useq_chain ? c.batch : 1;
-    const int uchain = c.useq_chain ? 1 : 0;
-#define RXG_LAUNCH_CHAIN(PC, SM)                                                                   \
-    do {                                                                                           \
-        if (c.useq)                                                                                \
-            lgssm_chain_kernel<D, M, PC, SM, true><<<blocks, threads, 0, ctx->stream>>>(           \
-                mdl, pc, c.y, c.ymask, c.mean, c.cov, c.nle, c.status, c.T, c.batch, tf, c.useq, ustride, uchain); \
-        else                                                                                       \
-            lgssm_chain_kernel<D, M, PC, SM><<<blocks, threads, 0, ctx->stream>>>(                 \
-                mdl, pc, c.y, c.ymask, c.mean, c.cov, c.nle, c.status, c.T, c.batch, tf);          \
-    } while (0)
     if (ctx->profile) { cudaEventRecord(ctx->ev[0], ctx->stream); cudaEventRecord(ctx->ev[1], ctx->stream); }
-    if (per_chain) { if (c.smooth) RXG_LAUNCH_CHAIN(true, true); else RXG_LAUNCH_CHAIN(true, false); }
-    else           { if (c.smooth) RXG_LAUNCH_CHAIN(false, true); else RXG_LAUNCH_CHAIN(false, false); }
-#undef RXG_LAUNCH_CHAIN
+    if (per_chain) (c.smooth ? launch_chain<D, M, true, true> : launch_chain<D, M, true, false>)(ctx, c, mdl, pc);
+    else           (c.smooth ? launch_chain<D, M, false, true> : launch_chain<D, M, false, false>)(ctx, c, mdl, pc);
     if (ctx->profile) cudaEventRecord(ctx->ev[2], ctx->stream);
     ctx->launches += 1;
     return check_cuda(ctx, cudaGetLastError(), "lgssm_chain_kernel launch");
 }
 
-template <int D, int M, int CPT>
-static int launch_shared(rxg_ctx* ctx, LgssmCall& c, const ModelF<D, M>& mdl, const GainWs& ws,
-                         int write_cov) {
-    constexpr int PF = 4;
-    const int threads = 32;                     // one warp per CTA (see rxg_lgssm_shared.cuh)
-    const int64_t nthr = c.batch / CPT;
-    const unsigned blocks = (unsigned)((nthr + threads - 1) / threads);
-    const int tf = (c.flags & RXG_TRANSITION_FIRST) ? 1 : 0;
-    const bool evid = c.nle != nullptr;
-    bool has_u = c.useq != nullptr && !c.useq_chain;       // a shared input sequence lives in the gain tables' offsets
-    for (int i = 0; i < D; ++i) has_u |= (mdl.u[i] != 0.f);
-    // checkpoint + recompute instead of the forward->backward stash (RXG_NO_CKPT=1: A/B switch)
-    bool ckpt = c.smooth && (D * D <= 16) && (CPT == 2);   // with one chain per thread the stash path is faster
-    if (ctx->opt[RXG_OPT_SWEEP_VARIANT] == 1) ckpt = false;                     // stash variant (A/B switch)
-    // fused all-gather: only the headline variant (smoothing, no evidence, no offset) has a PEER instantiation;
-    // everything else leaves fused_peer_stores false and the caller pushes the finished slab
-    const bool peer = c.smooth && !evid && !has_u && !c.useq && (c.po.n_mean > 0 || c.po.n_cov > 0);
-    if (c.useq_chain) {
-        // per-chain input sequence: its own instantiation, streamed beside y (no offset, no peer stores)
-#define RXG_LAUNCH_USEQ(SM, EV, CK)                                                                \
-        lgssm_shared_kernel<D, M, CPT, PF, SM, EV, false, CK, false, 1><<<blocks, threads, 0, ctx->stream>>>( \
-            mdl, ws.fwd, ws.bwd, ws.sf, c.y, c.mean, c.cov, c.nle, c.T, c.batch, tf, write_cov, c.mean0_chain, c.po, c.useq)
-        if (ctx->profile) cudaEventRecord(ctx->ev[1], ctx->stream);
-        if (c.smooth) {
-            if (ckpt) { if (evid) RXG_LAUNCH_USEQ(true, true, true); else RXG_LAUNCH_USEQ(true, false, true); }
-            else      { if (evid) RXG_LAUNCH_USEQ(true, true, false); else RXG_LAUNCH_USEQ(true, false, false); }
-        } else {
-            if (evid) RXG_LAUNCH_USEQ(false, true, false); else RXG_LAUNCH_USEQ(false, false, false);
+// Launches lgssm_shared_kernel if pick index I is the call's pick.  Only the picks select_shared_sweep can return
+// (sweep_pick_reachable) are instantiated.
+template <int D, int M, int I>
+static bool launch_sweep_if(int pick, rxg_ctx* ctx, const LgssmCall& c, const ModelF<D, M>& mdl, const GainWs& ws,
+                            int write_cov) {
+    constexpr SweepPick p = sweep_pick_at(I);
+    if constexpr (sweep_pick_reachable(D, M, p)) {
+        if (pick == I) {
+            const int threads = 32;                     // one warp per CTA (see rxg_lgssm_shared.cuh)
+            const unsigned blocks = (unsigned)((c.batch / p.cpt + threads - 1) / threads);
+            const int tf = (c.flags & RXG_TRANSITION_FIRST) ? 1 : 0;
+            lgssm_shared_kernel<D, M, p.cpt, 4, p.smooth, p.evid, p.offset, p.ckpt, p.peer, p.useq>
+                <<<blocks, threads, 0, ctx->stream>>>(mdl, ws.fwd, ws.bwd, ws.sf, c.y, c.mean, c.cov, c.nle, c.T, c.batch,
+                                                      tf, write_cov, c.mean0_chain, c.po, p.useq ? c.useq : nullptr);
+            return true;
         }
-#undef RXG_LAUNCH_USEQ
-        if (ctx->profile) cudaEventRecord(ctx->ev[2], ctx->stream);
-        ctx->launches += 1;
-        c.fused_peer_stores = false;
-        return check_cuda(ctx, cudaGetLastError(), "lgssm_shared_kernel (input sequence) launch");
     }
-    if (c.useq && evid) {
-        // shared input sequence with evidence: the tables carry the offsets, the evidence form reads u_t
-#define RXG_LAUNCH_USEQ2(SM, CK)                                                                   \
-        lgssm_shared_kernel<D, M, CPT, PF, SM, true, true, CK, false, 2><<<blocks, threads, 0, ctx->stream>>>( \
-            mdl, ws.fwd, ws.bwd, ws.sf, c.y, c.mean, c.cov, c.nle, c.T, c.batch, tf, write_cov, c.mean0_chain, c.po, c.useq)
-        if (ctx->profile) cudaEventRecord(ctx->ev[1], ctx->stream);
-        if (c.smooth) { if (ckpt) RXG_LAUNCH_USEQ2(true, true); else RXG_LAUNCH_USEQ2(true, false); }
-        else RXG_LAUNCH_USEQ2(false, false);
-#undef RXG_LAUNCH_USEQ2
-        if (ctx->profile) cudaEventRecord(ctx->ev[2], ctx->stream);
-        ctx->launches += 1;
-        c.fused_peer_stores = false;
-        return check_cuda(ctx, cudaGetLastError(), "lgssm_shared_kernel (shared input sequence, evidence) launch");
-    }
-#define RXG_LAUNCH_SHARED2(SM, EV, OF, CK)                                                         \
-    do {                                                                                           \
-        if (SM && !EV && !OF && peer)                                                              \
-            lgssm_shared_kernel<D, M, CPT, PF, SM, false, false, CK, true><<<blocks, threads, 0, ctx->stream>>>( \
-                mdl, ws.fwd, ws.bwd, ws.sf, c.y, c.mean, c.cov, c.nle, c.T, c.batch, tf, write_cov, c.mean0_chain, c.po); \
-        else                                                                                       \
-            lgssm_shared_kernel<D, M, CPT, PF, SM, EV, OF, CK><<<blocks, threads, 0, ctx->stream>>>( \
-                mdl, ws.fwd, ws.bwd, ws.sf, c.y, c.mean, c.cov, c.nle, c.T, c.batch, tf, write_cov, c.mean0_chain, c.po); \
-    } while (0)
-#define RXG_LAUNCH_SHARED(SM, EV)                                                                  \
-    do {                                                                                           \
-        if (SM && ckpt) { if (has_u) RXG_LAUNCH_SHARED2(SM, EV, true, true); else RXG_LAUNCH_SHARED2(SM, EV, false, true); } \
-        else            { if (has_u) RXG_LAUNCH_SHARED2(SM, EV, true, false); else RXG_LAUNCH_SHARED2(SM, EV, false, false); } \
-    } while (0)
+    return false;
+}
+template <int D, int M, int... I>
+static bool launch_sweep(int pick, rxg_ctx* ctx, const LgssmCall& c, const ModelF<D, M>& mdl, const GainWs& ws,
+                         int write_cov, std::integer_sequence<int, I...>) {
+    return (launch_sweep_if<D, M, I>(pick, ctx, c, mdl, ws, write_cov) || ...);
+}
+
+template <int D, int M>
+static int launch_shared(rxg_ctx* ctx, LgssmCall& c, const ModelF<D, M>& mdl, const GainWs& ws, int write_cov,
+                         const SweepPick& p) {
+    const int pick = sweep_pick_index(p);
     if (ctx->profile) cudaEventRecord(ctx->ev[1], ctx->stream);
-    if (c.smooth) { if (evid) RXG_LAUNCH_SHARED(true, true); else RXG_LAUNCH_SHARED(true, false); }
-    else          { if (evid) RXG_LAUNCH_SHARED(false, true); else RXG_LAUNCH_SHARED(false, false); }
-#undef RXG_LAUNCH_SHARED
-#undef RXG_LAUNCH_SHARED2
+    if (!launch_sweep<D, M>(pick, ctx, c, mdl, ws, write_cov, std::make_integer_sequence<int, SWEEP_PICK_COUNT>{}))
+        return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm: no lgssm_shared_kernel instantiation for sweep pick %d", pick);
     if (ctx->profile) cudaEventRecord(ctx->ev[2], ctx->stream);
     ctx->launches += 1;
-    c.fused_peer_stores = peer;          // the PEER instantiation stored the final posteriors to c.po itself
+    // the PEER instantiation stores the final posteriors to c.po itself; otherwise the caller pushes the finished slab
+    c.fused_peer_stores = p.peer;
     return check_cuda(ctx, cudaGetLastError(), "lgssm_shared_kernel launch");
 }
 
@@ -560,15 +527,21 @@ static int run_shared_family(rxg_ctx* ctx, LgssmCall& c) {
         sgw.rec = (float*)(base + o_srec_t); sgw.nrec = (float*)(base + o_snrec); sgw.srec = (float*)(base + o_ssrec);
         return launch_seg<D, M>(ctx, c, mdl, ws, sgw, write_cov, variant == 3);
     }
-    const bool al16 = (((uintptr_t)c.y | (uintptr_t)c.mean | (uintptr_t)c.cov | (uintptr_t)c.nle | (uintptr_t)c.mean0_chain |
-                        (uintptr_t)(c.useq_chain ? c.useq : nullptr)) & 15) == 0;
-    // chains per thread: keep >= ~2 resident warps per SM sub-partition
-    // Wider per-thread vectors cut the number of (128-byte-per-warp) store instructions per byte.
-    int cpt = (c.batch >= (int64_t)ctx->sm_count * 64 * 2) ? 2 : 1;
-    if (ctx->opt[RXG_OPT_FORCE_CPT] > 0) cpt = (int)ctx->opt[RXG_OPT_FORCE_CPT];      // test / tuning override
-    if (D * M > 16 && cpt > 2) cpt = 2;                              // register budget for d = 6
-    if (cpt >= 2 && al16 && c.batch % 2 == 0) return launch_shared<D, M, 2>(ctx, c, mdl, ws, write_cov);
-    return launch_shared<D, M, 1>(ctx, c, mdl, ws, write_cov);
+    SweepQuery q = {};
+    q.d = D;
+    q.m = M;
+    q.batch = c.batch;
+    q.sm_count = ctx->sm_count;
+    q.force_cpt = ctx->opt[RXG_OPT_FORCE_CPT];
+    q.aligned16 = (((uintptr_t)c.y | (uintptr_t)c.mean | (uintptr_t)c.cov | (uintptr_t)c.nle | (uintptr_t)c.mean0_chain |
+                    (uintptr_t)(c.useq_chain ? c.useq : nullptr)) & 15) == 0;
+    q.smooth = c.smooth;
+    q.evid = c.nle != nullptr;
+    for (int i = 0; i < D; ++i) q.offset |= (mdl.u[i] != 0.f);
+    q.input = !c.useq ? InputSeq::none : (c.useq_chain ? InputSeq::per_chain : InputSeq::shared);
+    q.peer_out = c.po.n_mean > 0 || c.po.n_cov > 0;
+    q.sweep_variant = variant;
+    return launch_shared<D, M>(ctx, c, mdl, ws, write_cov, select_shared_sweep(q));
 }
 
 template <int D, int M>
@@ -581,7 +554,7 @@ int run_dm(rxg_ctx* ctx, LgssmCall& c) {
 }
 
 // This translation unit is compiled once per (d, m) shape with -DRXG_INST_D / -DRXG_INST_M (explicit instantiation
-// of run_dm: the ~30 kernel variants of one shape), in parallel, and once without them for the dispatch below.
+// of run_dm: the kernel variants of one shape), in parallel, and once without them for the dispatch below.
 #ifdef RXG_INST_D
 template int run_dm<RXG_INST_D, RXG_INST_M>(rxg_ctx*, LgssmCall&);
 #else
