@@ -30,6 +30,7 @@
 #include "rxg_gain.cuh"
 #include "rxg_internal.h"
 #include "rxg_linalg.cuh"
+#include "rxg_lgssm_cluster.cuh"
 #include "rxg_lgssm_common.cuh"
 #include "rxg_lgssm_shared.cuh"
 #include "rxg_lgssm_seg.cuh"
@@ -453,6 +454,60 @@ static int launch_seg(rxg_ctx* ctx, LgssmCall& c, const ModelF<D, M>& mdl, const
     return check_cuda(ctx, cudaGetLastError(), "lgssm_seg_kernel launch");
 }
 
+// cluster sweep (rxg_lgssm_cluster.cuh): plain smoothing (no evidence, offset, inputs or per-chain prior mean -- the
+// streaming chunk, the only caller with one, filters) at d * d <= 16, m >= d, whole 32-chain tiles of 16-byte aligned
+// buffers, the default dispatch options, T within the shared-memory budget, and a cluster shape the device can hold
+// resident.  Every other call keeps lgssm_shared_kernel / lgssm_seg_kernel.  A fused gather takes the PEER instantiation:
+// the gathered buffers must hold the bits of the plain sweep.
+template <int D, int M>
+static int launch_cluster_if_eligible(rxg_ctx* ctx, LgssmCall& c, const ModelF<D, M>& mdl, const GainWs& ws, float* cl_tab,
+                                      int write_cov, bool& launched) {
+    launched = false;
+    if constexpr (D * D <= 16 && M >= D) {
+        using CT = ClusterTab<D, M>;
+        bool offset = false;
+        for (int i = 0; i < D; ++i) offset |= (mdl.u[i] != 0.f);
+        const bool aligned = (((uintptr_t)c.y | (uintptr_t)c.mean | (uintptr_t)c.cov) & 15) == 0;
+        if (!c.smooth || c.nle || c.useq || offset || c.mean0_chain || c.batch % 32 != 0 || !aligned ||
+            ctx->opt[RXG_OPT_SWEEP_VARIANT] != 0 || ctx->opt[RXG_OPT_FORCE_CPT] != 0)
+            return RXG_OK;
+        const size_t smem = CT::smem_bytes(c.T);
+        int smem_max = 0;
+        RXG_CUDA(ctx, cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+        if (smem > (size_t)smem_max) return RXG_OK;
+        const bool peer = c.po.n_mean > 0 || c.po.n_cov > 0;
+        auto kern = peer ? lgssm_cluster_sweep_kernel<D, M, true> : lgssm_cluster_sweep_kernel<D, M, false>;
+        RXG_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        cudaLaunchConfig_t cfg = {};
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = CL_CTAS;
+        attr[0].val.clusterDim.y = 1;
+        attr[0].val.clusterDim.z = 1;
+        cfg.gridDim = dim3((unsigned)(c.batch / 32 * CL_CTAS));
+        cfg.blockDim = dim3(32 * CL_WARPS);
+        cfg.dynamicSmemBytes = smem;
+        cfg.stream = ctx->stream;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        int nclusters = 0;
+        RXG_CUDA(ctx, cudaOccupancyMaxActiveClusters(&nclusters, kern, &cfg));
+        if (nclusters < 1) return RXG_OK;
+
+        const int spc = CT::spc(c.T);
+        cluster_tables_kernel<D, M><<<1, 256, 0, ctx->stream>>>(ws, cl_tab, c.T, spc);
+        if (ctx->profile) cudaEventRecord(ctx->ev[1], ctx->stream);
+        RXG_CUDA(ctx, cudaLaunchKernelEx(&cfg, kern, (const float*)ws.fwd, (const float*)ws.bwd, (const float*)cl_tab, c.y,
+                                         c.mean, c.cov, c.T, c.batch, write_cov, mdl, c.po));
+        if (ctx->profile) cudaEventRecord(ctx->ev[2], ctx->stream);
+        ctx->launches += 2;
+        c.fused_peer_stores = peer;
+        launched = true;
+        return check_cuda(ctx, cudaGetLastError(), "lgssm_cluster_sweep_kernel launch");
+    }
+    return RXG_OK;
+}
+
 template <int D, int M>
 static int run_shared_family(rxg_ctx* ctx, LgssmCall& c) {
     using TB = Tab<D, M>;
@@ -478,6 +533,7 @@ static int run_shared_family(rxg_ctx* ctx, LgssmCall& c) {
     const size_t o_srec_t = carve(T * ST::REC * sizeof(float)), o_snrec = carve(T * ST::NREC * sizeof(float));
     const size_t o_ssrec = carve(nseg * ST::SREC * sizeof(float));
     const size_t o_ctab = carve(c.want_cov_table ? T * D * D * sizeof(float) : 0);
+    const size_t o_cl = carve(ClusterTab<D, M>::table_floats(c.T) * sizeof(float));
     char* base = (char*)workspace(ctx, off);
     if (!base) return RXG_ERR_CUDA;
     GainWs ws;
@@ -520,6 +576,9 @@ static int run_shared_family(rxg_ctx* ctx, LgssmCall& c) {
     if (c.ev_tables) RXG_CUDA(ctx, cudaEventRecord(c.ev_tables, ctx->stream));
     if (c.tables_only) return RXG_OK;
     const int write_cov = (c.cov != nullptr && !cov_shared) ? 1 : 0;
+    bool launched = false;
+    rc = launch_cluster_if_eligible<D, M>(ctx, c, mdl, ws, (float*)(base + o_cl), write_cov, launched);
+    if (rc != RXG_OK || launched) return rc;
     // sweep variant (RXG_OPT_SWEEP_VARIANT): 3 / 4 = time-segmented kernel with / without L2 eviction hints
     const long long variant = ctx->opt[RXG_OPT_SWEEP_VARIANT];
     if (variant == 3 && !c.useq && seg_sweep_eligible<D, M>(c)) {      // inputs: the lock-step kernel
