@@ -6,6 +6,7 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
   python bench_extra.py --which predict      (opt-in: observation predictions / forecasts after the smoother)
   python bench_extra.py --which inputs       (opt-in: known per-step inputs u[t], shared and per-chain sequences)
   python bench_extra.py --which vmp_wishart  (opt-in: Wishart-precision VMP around the smoother vs the composed path)
+  python bench_extra.py --which vmp_noise    (opt-in: learned process precision, alone and with the observation precision)
 """
 from __future__ import annotations
 
@@ -139,21 +140,25 @@ def bench_inputs(ctx, peak):
         torch.cuda.empty_cache()
 
 
-def vmp_wishart_counts(d, m, masked):
+def vmp_wishart_counts(d, m, masked, learn="Q"):
     """Algorithmic bytes and FLOPs per (chain, step, iteration) of one non-final iteration of the fused Wishart VMP kernel
     (lgssm_vmp_wishart_kernel), and the bytes of the same iteration on the composed path (per-chain smoother + a reduction
-    over T).  Bytes: y is read in both directions; the filtered mean and the lower triangle of the filtered covariance are
-    written (stash) and read back; a per-chain mask adds one byte per direction.  FLOPs: 2 x the FMAs of the step helpers
-    (predict, update, RTS step) and of the R_b accumulation, dense counts of rxg_linalg.cuh."""
+    over T).  Bytes: y is read in both directions (forward only when Q is known: the backward pass reads y for R_q); the
+    filtered mean and the lower triangle of the filtered covariance are written (stash) and read back; a per-chain mask
+    adds one byte per direction.  FLOPs: 2 x the FMAs of the step helpers (predict, update, RTS step), of the R_q
+    accumulation (learned Q) and of the pair term of R_p (learned P: (I - A G) Ss (I - A G)' + A C A' + e e'), dense counts
+    of rxg_linalg.cuh."""
     tri = lambda n: n * (n + 1) // 2
     stash = 4 * (d + tri(d))
-    fused = 2 * 4 * m + 2 * stash + (2 if masked else 0)
+    lq, lp = "Q" in learn, "P" in learn
+    fused = (2 if lq else 1) * 4 * m + 2 * stash + ((2 if lq else 1) if masked else 0)
     composed = (4 * m + 2 * stash + 4 * (d + d * d) + (1 if masked else 0)) + (4 * m + 4 * d + 4 * d * d + (1 if masked else 0))
     predict = d * d + d ** 3 + tri(d) * d
     update = m * d * d + tri(m) * d + m ** 3 // 6 + d * m * m // 2 + m * d + m * m // 2 + d * m + tri(d) * m
     rts = d ** 3 + tri(d) * d + d ** 3 // 6 + d ** 3 // 2 + d ** 3 // 2 + tri(d) * d + d ** 3 + tri(d) * d + 2 * d * d
-    acc = m * d + m * m + m * d * d + tri(m) * d
-    return fused, composed, 2 * (predict + update + rts + acc)
+    acc = (m * d + m * m + m * d * d + tri(m) * d) if lq else 0
+    pair = (3 * d ** 3 + 2 * tri(d) * d + d * d + tri(d)) if lp else 0
+    return fused, composed, 2 * (predict + update + rts + acc + pair)
 
 
 def _composed_wishart(ctx, y, mod, its, nu0, Psi0, W0, mask):
@@ -215,6 +220,52 @@ def bench_vmp_wishart(ctx, peak):
         torch.cuda.empty_cache()
 
 
+def bench_vmp_noise(ctx, peak):
+    """Learned process precision (rxg_lgssm_vmp_noise_f32: learn P, learn P and Q) against the learned observation
+    precision alone (rxg_lgssm_vmp_wishart_f32), alternated in one run on the same data; kernel time from CUDA events
+    around the launch (rxg_set_profiling)."""
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(14)
+    T, nb, its = 1000, 65536, 10
+    for d in (4, 2):
+        m = d
+        mod = notebook_model_f32() if d == 4 else notebook_model_d2_f32()
+        y = torch.randn(T, m, nb, device="cuda", generator=g) * 3.3
+        q_prior, q_init = (m + 2.0, 10.0 * np.eye(m)), 0.1 * np.eye(m)
+        p_prior, p_init = (d + 2.0, 0.1 * np.eye(d)), np.linalg.inv(np.asarray(mod["P"], np.float64))
+        calls = {"Q": lambda: ctx.lgssm_vmp_wishart(y, mod["A"], mod["B"], mod["P"], mod["m0"], mod["S0"], iterations=its,
+                                                    w_prior=q_prior, init_E_W=q_init),
+                 "P": lambda: ctx.lgssm_vmp_noise(y, mod["A"], mod["B"], mod["m0"], mod["S0"], Q=mod["Q"], p_prior=p_prior,
+                                                  p_init=p_init, iterations=its),
+                 "PQ": lambda: ctx.lgssm_vmp_noise(y, mod["A"], mod["B"], mod["m0"], mod["S0"], p_prior=p_prior,
+                                                   p_init=p_init, q_prior=q_prior, q_init=q_init, iterations=its)}
+        kern = {k: [] for k in calls}
+        call = {k: [] for k in calls}
+        for _ in range(3):
+            for k, fn in calls.items():
+                call[k].append(timed(fn, warm=2, reps=3))
+                ctx.set_profiling(True)
+                fn()
+                kern[k].append(ctx.profile_last_ms()[0])
+                ctx.set_profiling(False)
+        for k in calls:
+            kms, cms = float(np.median(kern[k])), float(np.median(call[k]))
+            bf, _, fl = vmp_wishart_counts(d, m, False, learn=k)
+            n = T * nb * its
+            t_hbm, t_fp32 = bf * n / (peak * 1e9), fl * n / 67e12
+            print(json.dumps({"what": f"noise-precision VMP around the smoother, learn {k} (lgssm_vmp_wishart_kernel)",
+                              "learn": k, "d": d, "m": m, "T": T, "batch": nb, "iterations": its, "kernel_ms": kms,
+                              "kernel_ms_runs": kern[k], "call_ms": cms, "ms_per_iteration": kms / its,
+                              "bytes_per_chain_step_iteration": bf, "flops_per_chain_step_iteration": fl,
+                              "achieved_GBs": bf * n / kms / 1e6, "achieved_TFLOPs": fl * n / kms / 1e9,
+                              "bound": "hbm" if t_hbm >= t_fp32 else "fp32",
+                              "kernel_frac_of_hbm_bound": t_hbm * 1e3 / kms,
+                              "kernel_frac_of_bound": max(t_hbm, t_fp32) * 1e3 / kms,
+                              "peak_hbm_gbs": peak, "peak_fp32_tflops": 67, "gpu": gname, "power_limit": plim}), flush=True)
+        del y
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -228,6 +279,8 @@ def main():
         bench_inputs(ctx, peak)
     if "vmp_wishart" in which:
         bench_vmp_wishart(ctx, peak)
+    if "vmp_noise" in which:
+        bench_vmp_noise(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

@@ -377,6 +377,27 @@ int rxg_lgssm_vmp_wishart_f32(rxg_ctx*, int d, int m, int T, int64_t batch, int 
                               float nu0, const float* inv_scale0, const float* init_E_W, const float* y,
                               const uint8_t* ymask, float* post_mean, float* post_cov, float* df, float* inv_scale,
                               double* free_energy, int32_t* status, unsigned flags);
+/* The same VMP with an unknown PROCESS precision matrix w_p, alone or together with the observation precision w_q:
+ *   w_p ~ Wishart(nu_p0, inv(inv_scale_p0)) (else P known); w_q ~ Wishart(nu_q0, inv(inv_scale_q0)) (else Q known);
+ *   x[1] ~ N(m0, S0) (RXG_TRANSITION_FIRST: one transition earlier); x[t] ~ N(A x[t-1] + u, inv(w_p));
+ *   y[t] ~ N(B x[t], inv(w_q)); q(x) q(w_p) q(w_q), q(x) structured over the chain.
+ * For each noise pass exactly one of the known matrix (P / Q) and the pair (inv_scale_0, init_E_W = E[w] of the initial
+ * q(w)); at least one noise is learned (both known is the plain smoother: RXG_ERR_BAD_ARG).  A learned noise needs its
+ * outputs df_*[iterations][batch] / inv_scale_*[iterations][k][k][batch] (k = d for p, m for q, after EVERY iteration);
+ * a known noise's outputs must be NULL.  Each iteration runs the Kalman filter + RTS smoother with P = inv(E[w_p]) and
+ * Q = inv(E[w_q]), then q(w_p) = (nu_p0 + T - 1 + tf, inv_scale_p0 + R_p) with R_p the sum over the transitions of
+ * E[(x[t+1] - A x[t] - u)(x[t+1] - A x[t] - u)'] under the pairwise smoothed marginal (masks do not change the count),
+ * and q(w_q) as rxg_lgssm_vmp_wishart_f32 updates it.  free_energy[iterations][batch] (fp64) or NULL: the Bethe free
+ * energy with one Wishart block per learned noise.  Host model arrays, device data, masks, status, flags, d, m in 1..6
+ * and the refusals as rxg_lgssm_vmp_wishart_f32; nu_p0 > d - 1, nu_q0 > m - 1 and SPD inverse scales / initial E[w]
+ * of the learned noises, else RXG_ERR_BAD_ARG.  Called with Q learned and P known it computes exactly what
+ * rxg_lgssm_vmp_wishart_f32 computes.                                                                          */
+int rxg_lgssm_vmp_noise_f32(rxg_ctx*, int d, int m, int T, int64_t batch, int iterations, const float* A, const float* B,
+                            const float* m0, const float* S0, const float* u, const float* P, float nu_p0,
+                            const float* inv_scale_p0, const float* init_E_Wp, const float* Q, float nu_q0,
+                            const float* inv_scale_q0, const float* init_E_Wq, const float* y, const uint8_t* ymask,
+                            float* post_mean, float* post_cov, float* df_p, float* inv_scale_p, float* df_q,
+                            float* inv_scale_q, double* free_energy, int32_t* status, unsigned flags);
 /* Hierarchical Gaussian Filter, streaming, `iters` VMP iterations per datum
  * [ref: test/models/statespace/hgf_tests.jl:10-69; loop src/inference/streaming.jl:349-407].
  * y[T][batch]; init = (m_z, v_z, m_x, v_x); out[T][4][batch] = (m_x, v_x, m_z, v_z).            */

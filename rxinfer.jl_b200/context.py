@@ -361,6 +361,22 @@ class Context:
                 raise ValueError(f"{k}: expected shape {shapes[k]}, got {a.shape}")
             keep[k] = (a, p)
         self._io(y, "y", True)
+        mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
+        mean, cov = self.empty(T, d, batch), self.empty(T, d, d, batch)
+        df, iS = self.empty(iterations, batch), self.empty(iterations, m, m, batch)
+        fe = self.empty(iterations, batch, dtype=torch.float64) if want_free_energy else None
+        st = self.empty(batch, dtype=torch.int32)
+        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
+        up = keep["u"][1] if "u" in keep else L.as_fp(0)
+        self._check(self.lib.rxg_lgssm_vmp_wishart_f32(
+            self.h, d, m, T, batch, iterations, keep["A"][1], keep["B"][1], keep["P"][1], keep["m0"][1], keep["S0"][1], up,
+            float(nu0), keep["inv_scale0"][1], keep["init_E_W"][1], _fp(y), mask_p, _fp(mean), _fp(cov), _fp(df), _fp(iS),
+            fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
+        return dict(mean=mean, cov=cov, df=df, inv_scale=iS, free_energy=fe, status=st)
+
+    def _vmp_mask_flags(self, mask, T, batch, keep, transition_first, asynchronous):
+        """Mask pointer and flags of the Wishart VMP entries: a [T, batch] device mask per chain or a [T] pattern shared by
+        every chain (staged from the host; kept alive in ``keep``)."""
         flags = L.PTR_DEVICE
         mask_p = ctypes.cast(c_void_p(None), L.u8p)
         if mask is not None and getattr(mask, "ndim", 2) == 1:
@@ -377,17 +393,71 @@ class Context:
             flags |= L.TRANSITION_FIRST
         if asynchronous:
             flags |= L.ASYNC
+        return mask_p, flags
+
+    def lgssm_vmp_noise(self, y, A, B, m0, S0, *, P=None, Q=None, p_prior=None, p_init=None, q_prior=None, q_init=None,
+                        u=None, mask=None, transition_first=False, iterations=10, want_free_energy=False,
+                        asynchronous=False):
+        """VMP around the smoother with an unknown process precision matrix w_p, alone or together with an unknown
+        observation precision w_q, one of each per chain (``rxg_lgssm_vmp_noise_f32``):
+        w_p ~ Wishart(nu_p0, inv(inv_scale_p0)), w_q ~ Wishart(nu_q0, inv(inv_scale_q0)), x[t] ~ N(A x[t-1] + u, inv(w_p)),
+        y[t] ~ N(B x[t], inv(w_q)), q(x) q(w_p) q(w_q).  For each noise pass either the known matrix (``P`` / ``Q``) or the
+        prior ``(nu0, inv_scale0)`` together with ``*_init`` = E[w] of the initial q(w); a learned noise has no default
+        initial q(w) (a vague one makes the first fp32 sweep ill-conditioned).  y[T, m, batch] on this context's device;
+        ``mask`` as for :meth:`lgssm_vmp_wishart`.  Returns dict(mean[T, d, batch], cov[T, d, d, batch] of the last
+        iteration, df_p[iterations, batch] / inv_scale_p[iterations, d, d, batch] and df_q / inv_scale_q ([.., m, m, ..])
+        after every iteration (None for a known noise), free_energy[iterations, batch] fp64 or None, status[batch])."""
+        if y.dim() != 3:
+            raise ValueError(f"y: expected [T, m, batch], got shape {tuple(y.shape)}")
+        T, m, batch = y.shape
+        d = np.asarray(A).shape[-1]
+        iterations = int(iterations)
+        if iterations < 1:
+            raise ValueError(f"iterations must be >= 1, got {iterations}")
+        shapes = dict(A=(d, d), B=(m, d), m0=(d,), S0=(d, d))
+        mats = dict(A=A, B=B, m0=m0, S0=S0)
+        nus = {}
+        for name, k, known, prior, init in (("p", d, P, p_prior, p_init), ("q", m, Q, q_prior, q_init)):
+            if known is not None:
+                if prior is not None or init is not None:
+                    raise ValueError(f"{name.upper()} is known: pass either {name.upper()} or {name}_prior / {name}_init")
+                shapes[name.upper()], mats[name.upper()] = (k, k), known
+                continue
+            if prior is None or init is None:
+                raise ValueError(f"{name.upper()} is learned: pass {name}_prior = (nu0, inv_scale0) and {name}_init = E[w] "
+                                 f"of the initial q(w_{name}) (there is no default initial q(w))")
+            nus[name] = float(prior[0])
+            shapes[f"inv_scale_{name}0"], mats[f"inv_scale_{name}0"] = (k, k), prior[1]
+            shapes[f"init_E_W{name}"], mats[f"init_E_W{name}"] = (k, k), init
+        if not nus:
+            raise ValueError("P and Q are both known: that is the plain smoother (Context.lgssm)")
+        if u is not None:
+            shapes["u"], mats["u"] = (d,), u
+        keep = {}
+        for k, v in mats.items():
+            a, p = _model32(v)
+            if a.shape != shapes[k]:
+                raise ValueError(f"{k}: expected shape {shapes[k]}, got {a.shape}")
+            keep[k] = (a, p)
+        self._io(y, "y", True)
+        mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
         mean, cov = self.empty(T, d, batch), self.empty(T, d, d, batch)
-        df, iS = self.empty(iterations, batch), self.empty(iterations, m, m, batch)
+        out = {}
+        for name, k in (("p", d), ("q", m)):
+            learned = name in nus
+            out[f"df_{name}"] = self.empty(iterations, batch) if learned else None
+            out[f"inv_scale_{name}"] = self.empty(iterations, k, k, batch) if learned else None
         fe = self.empty(iterations, batch, dtype=torch.float64) if want_free_energy else None
         st = self.empty(batch, dtype=torch.int32)
         fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
-        up = keep["u"][1] if "u" in keep else L.as_fp(0)
-        self._check(self.lib.rxg_lgssm_vmp_wishart_f32(
-            self.h, d, m, T, batch, iterations, keep["A"][1], keep["B"][1], keep["P"][1], keep["m0"][1], keep["S0"][1], up,
-            float(nu0), keep["inv_scale0"][1], keep["init_E_W"][1], _fp(y), mask_p, _fp(mean), _fp(cov), _fp(df), _fp(iS),
-            fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
-        return dict(mean=mean, cov=cov, df=df, inv_scale=iS, free_energy=fe, status=st)
+        hp = lambda k: keep[k][1] if k in keep else L.as_fp(0)
+        self._check(self.lib.rxg_lgssm_vmp_noise_f32(
+            self.h, d, m, T, batch, iterations, hp("A"), hp("B"), hp("m0"), hp("S0"), hp("u"),
+            hp("P"), nus.get("p", 0.0), hp("inv_scale_p0"), hp("init_E_Wp"),
+            hp("Q"), nus.get("q", 0.0), hp("inv_scale_q0"), hp("init_E_Wq"),
+            _fp(y), mask_p, _fp(mean), _fp(cov), _fp(out["df_p"]), _fp(out["inv_scale_p"]), _fp(out["df_q"]),
+            _fp(out["inv_scale_q"]), fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
+        return dict(mean=mean, cov=cov, **out, free_energy=fe, status=st)
 
     # ------------------------------------------------------------------ per-rule kernels
     def _mat(self, M):

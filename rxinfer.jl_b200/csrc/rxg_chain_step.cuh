@@ -53,19 +53,28 @@ __device__ __forceinline__ void chain_update(const Mat<float, M, D>& B, const Ma
     }
 }
 
+// pair hook of an RTS step without lag-one statistics
+struct NoPair {
+    template <int D>
+    __device__ __forceinline__ void operator()(const Mat<float, D, D>&, const Mat<float, D, D>&,
+                                               const Mat<float, D, D>&) const {}
+};
+
 // one RTS step: filtered (muf, Sf) at t and smoothed (mus, Ss) at t+1 -> smoothed at t (in place).
 // Sp = A Sf A' + P (the forward message into x_{t+1}); RTS gain G = Sf A' Sp^-1; load_u(u) refreshes the input of the
-// transition into x_{t+1}.
-template <int D, typename LoadU>
+// transition into x_{t+1}.  pair(G, C, Ss) sees the gain, C = cov(x_t | x_{t+1}, y_{1:t}) and the smoothed covariance at
+// t+1 before Ss is overwritten (the lag-one statistics of the pairwise marginal).
+template <int D, typename LoadU, typename Pair = NoPair>
 __device__ __forceinline__ void chain_rts(const Mat<float, D, D>& A, const Mat<float, D, D>& P, Vec<float, D>& u,
                                           LoadU load_u, const Vec<float, D>& muf, const Mat<float, D, D>& Sf,
-                                          Vec<float, D>& mus, Mat<float, D, D>& Ss, bool& bad) {
+                                          Vec<float, D>& mus, Mat<float, D, D>& Ss, bool& bad, Pair pair = Pair{}) {
     Mat<float, D, D> AS = mul(A, Sf);
     Mat<float, D, D> Sp = sym_mul_nt_add(AS, A, P);
     Chol<float, D> ch = cholesky<float, D, false>(Sp, bad);
     Mat<float, D, D> U = solve_right_Lt(transpose(AS), ch.L);   // Sf A' L^-T
     Mat<float, D, D> G = solve_right_L(U, ch.L);
     Mat<float, D, D> C = sym_downdate(Sf, U);                   // cov(x_t | x_{t+1})
+    pair(G, C, Ss);
     Mat<float, D, D> GS = mul(G, Ss);
     Ss = sym_mul_nt_add(GS, G, C);
     Vec<float, D> mup = mulv(A, muf);

@@ -1,34 +1,50 @@
-// Variational message passing around the per-chain smoother with an unknown observation precision MATRIX, one per
-// chain: the multivariate twin of vmp_gamma_kernel (rxg_hgf.cu).
+// Variational message passing around the per-chain smoother with unknown noise precision MATRICES, one per chain: the
+// multivariate twin of vmp_gamma_kernel (rxg_hgf.cu).
 //
-//   w ~ Wishart(nu0, inv(Psi0));  x[1] ~ N(m0, S0) (or one transition earlier, RXG_TRANSITION_FIRST);
-//   x[t] ~ N(A x[t-1] + u, P);    y[t] ~ N(B x[t], inv(w));    q(x) q(w)
-// [ref: docs/src/manuals/model-specification.md:265-271, constraints q(x, w) = q(x)q(w)].
+//   w_p ~ Wishart(nu_p0, inv(Psi_p0)) (else P known);  w_q ~ Wishart(nu_q0, inv(Psi_q0)) (else Q known);
+//   x[1] ~ N(m0, S0) (or one transition earlier, RXG_TRANSITION_FIRST);
+//   x[t] ~ N(A x[t-1] + u, inv(w_p));    y[t] ~ N(B x[t], inv(w_q));    q(x) q(w_p) q(w_q)
+// [ref: docs/src/manuals/model-specification.md:265-271, constraints q(x, w) = q(x)q(w)].  LEARN says which precisions
+// are learned: LEARN_Q (rxg_lgssm_vmp_wishart_f32), LEARN_P or both (rxg_lgssm_vmp_noise_f32).
 //
 // One iteration k, per chain:
-//   q(x)  exact Kalman filter + RTS smoother with Q = inv(Wbar), Wbar = E[w] under q_{k-1}(w) (init_E_W at k = 0): the
-//         average energy of the y node under q(w) is N(y | Bx, inv(E[w])) up to constants.
-//   q(w)  = prior x prod_t MvNormalMeanPrecision(:Lambda)(q_out = PointMass(y_t), q_mu = N(B mu_t, B Sigma_t B')), i.e.
-//         df = nu0 + N_b, Psi = Psi0 + R_b, R_b = sum_{observed t} (y_t - B mu_t)(y_t - B mu_t)' + B Sigma_t B'.
-//   F_k   = NLE(Wbar) + N_b/2 (log det Wbar - E log det w) + 1/2 tr((E w - Wbar) R_b) + KL(q_k(w) || prior)   (fp64)
-//         with q(x) the exact chain posterior under Wbar (its Gaussian part collapses to the filter's evidence).
+//   q(x)  exact Kalman filter + RTS smoother with P = inv(Wbar_p), Q = inv(Wbar_q), Wbar = E[w] under q_{k-1}(w) (init_E_W
+//         at k = 0; a known noise keeps its matrix): the average energy of a Gaussian node under q(w) is N(. | ., inv(E[w]))
+//         up to constants.
+//   q(w_q) = prior x prod_t MvNormalMeanPrecision(:Lambda)(q_out = PointMass(y_t), q_mu = N(B mu_t, B Sigma_t B')), i.e.
+//         df = nu_q0 + N_q, Psi = Psi_q0 + R_q, R_q = sum_{observed t} (y_t - B mu_t)(y_t - B mu_t)' + B Sigma_t B'.
+//   q(w_p) = prior x prod_t MvNormalMeanPrecision(:Lambda)(q(out, mu) = pairwise marginal of (x_{t+1}, A x_t + u)), i.e.
+//         df = nu_p0 + N_p (N_p = T - 1 + tf transitions, masks do not change it), Psi = Psi_p0 + R_p,
+//         R_p = sum_t e e' + cov(x_{t+1} - A x_t | y), e = mu_{t+1} - A mu_t - u.  With the RTS gain G_t and
+//         C_t = cov(x_t | x_{t+1}, y_{1:t}), x_t = G_t x_{t+1} + eps (cov C_t, independent of x_{t+1}) given all the data, so
+//         cov(x_{t+1} - A x_t | y) = (I - A G_t) Sigma_{t+1} (I - A G_t)' + A C_t A': two PSD terms, no cancellation in fp32.
+//   F_k   = NLE(Wbar_p, Wbar_q) + per learned noise [N/2 (log det Wbar - E log det w) + 1/2 tr((E w - Wbar) R)
+//         + KL(q_k(w) || prior)]   (fp64), q(x) the exact chain posterior under (Wbar_p, Wbar_q) (its Gaussian part
+//         collapses to the filter's evidence).
 // One thread = one chain, all iterations in one launch; every array is [..][batch] (coalesced).  post_mean / post_cov are
 // the forward->backward stash of every iteration; only the last iteration writes the smoothed q(x) over it.  The Kalman and
 // RTS step bodies are lgssm_chain_kernel's (rxg_chain_step.cuh).
 //
-// This translation unit is compiled once per Wishart dimension m (-DRXG_VMP_M=m: d = 1..6 of that m) and once without it
-// for the C entry below.  m is compiled exactly: padding y would add dummy coordinates to w and change the answer.
+// This translation unit is compiled once per observation dimension m (-DRXG_VMP_M=m: d = 1..6 of that m, three LEARN
+// each) and once without it for the C entries below.  m is compiled exactly: padding y would add dummy coordinates to w_q
+// and change the answer.
 #include <math.h>
+
+#include <type_traits>
 
 #include "rxg_chain_step.cuh"
 #include "rxg_internal.h"
 
 namespace rxg {
 
+enum : int { LEARN_Q = 1, LEARN_P = 2, LEARN_PQ = 3 };
+
 struct VmpWishHost {        // host-side model of one call (fp64 where the kernel works in fp64)
-    const float *A, *B, *P, *m0, *S0, *u;
-    double nu0, logdet_Psi0;
+    const float *A, *B, *P, *Q, *m0, *S0, *u;    // P / Q: the known matrix, or null when it is learned
+    double nu0, logdet_Psi0;                     // observation precision prior
     double Psi0[36], W0[36];   // [m][m], symmetrised
+    double nu_p0, logdet_Psi_p0;                 // process precision prior
+    double Psi_p0[36], Wp0[36];  // [d][d], symmetrised
 };
 struct VmpWishIO {
     const float* y;
@@ -40,12 +56,28 @@ struct VmpWishIO {
     int T, iterations, tf;
     int64_t batch;
 };
+struct VmpNoiseIO : VmpWishIO {
+    float *df_p, *inv_scale_p;
+};
+template <int LEARN>
+using VmpIO = std::conditional_t<LEARN == LEARN_Q, VmpWishIO, VmpNoiseIO>;
 
+template <int K>
+struct WishPrior {
+    double nu0, logdet_Psi0, Psi0[K * K], W0[K * K];
+};
 template <int D, int M>
 struct VmpWishModel {
     float A[D * D], B[M * D], P[D * D], m0[D], S0[D * D], u[D];
-    double nu0, logdet_Psi0, Psi0[M * M], W0[M * M];
+    WishPrior<M> q;
 };
+template <int D, int M>
+struct VmpNoiseModel : VmpWishModel<D, M> {
+    float Q[M * M];
+    WishPrior<D> p;
+};
+template <int D, int M, int LEARN>
+using VmpModel = std::conditional_t<LEARN == LEARN_Q, VmpWishModel<D, M>, VmpNoiseModel<D, M>>;
 
 __device__ __forceinline__ double digamma_d(double x) {      // psi(x), x > 0: recurrence up to x >= 10, asymptotic series
     double r = 0.0;
@@ -54,9 +86,110 @@ __device__ __forceinline__ double digamma_d(double x) {      // psi(x), x > 0: r
     return r + log(x) - 0.5 * i - i2 * (1.0 / 12 - i2 * (1.0 / 120 - i2 * (1.0 / 252 - i2 * (1.0 / 240 - i2 * (1.0 / 132)))));
 }
 
+// RTS pair hook: V = cov(x_{t+1} - A x_t | y) = (I - A G) Ss (I - A G)' + A C A', Ss the smoothed covariance at t+1
+template <int D>
+struct PairCov {
+    const Mat<float, D, D>& A;
+    Mat<float, D, D>& V;
+    __device__ __forceinline__ void operator()(const Mat<float, D, D>& G, const Mat<float, D, D>& C,
+                                               const Mat<float, D, D>& Ss) const {
+        Mat<float, D, D> F = mul(A, G);
+#pragma unroll
+        for (int i = 0; i < D; ++i)
+#pragma unroll
+            for (int j = 0; j < D; ++j) F(i, j) = (i == j ? 1.f : 0.f) - F(i, j);
+        Mat<float, D, D> AC = mul(A, C), Z = {};
+        Mat<float, D, D> FS = mul(F, Ss);
+        V = sym_mul_nt_add(FS, F, sym_mul_nt_add(AC, A, Z));
+    }
+};
+
+// R_p += e e' + V, e = mnext - A ms - u: one transition's term (fp32) folded into the fp64 lower triangle
+template <int D>
+__device__ __forceinline__ void accumulate_pair(double* Rp, const Mat<float, D, D>& A, const Vec<float, D>& u,
+                                                const Vec<float, D>& mnext, const Vec<float, D>& ms,
+                                                const Mat<float, D, D>& V) {
+    Vec<float, D> e = mulv(A, ms);
+#pragma unroll
+    for (int k = 0; k < D; ++k) e(k) = mnext(k) - (e(k) + u(k));
+    int q = 0;
+#pragma unroll
+    for (int k = 0; k < D; ++k)
+#pragma unroll
+        for (int l = 0; l <= k; ++l) Rp[q++] += (double)__fmaf_rn(e(k), e(l), V(k, l));
+}
+
+// the noise covariance of one q(x) sweep: inv(Wbar) when the precision is learned, else the known matrix; and log det Wbar
+template <bool LEARNED, int K>
+__device__ __forceinline__ Mat<float, K, K> noise_cov(const Mat<double, K, K>& Wbar, const float* known, bool& bad) {
+    if constexpr (LEARNED) return convert<float>(cholinv(Wbar, bad));
+    else return load_const<float, K, K>(known);
+}
+template <bool LEARNED, int K>
+__device__ __forceinline__ double noise_logdet(const Mat<double, K, K>& Wbar, bool& bad) {
+    if constexpr (LEARNED) return -2.0 * cholesky<double, K, true>(Wbar, bad).neg_half_logdet;
+    else return 0.0;
+}
 template <int D, int M>
+__device__ __forceinline__ const float* known_q(const VmpWishModel<D, M>&) { return nullptr; }
+template <int D, int M>
+__device__ __forceinline__ const float* known_q(const VmpNoiseModel<D, M>& mdl) { return mdl.Q; }
+
+// q(w) = Wishart(nu0 + N, inv(Psi0 + R)) from the lower triangle of R, written for iteration it; with want_fe, FE gains
+// N/2 (log det Wbar - E log det w) + 1/2 tr((E w - Wbar) R) + KL(q(w) || prior) and STORE writes it to io.fe.  WBAR
+// becomes E[w].  fp64 throughout.  A macro rather than a function: expanded in the kernel body, the learn-Q kernels
+// compile to the same code as before the process noise could be learned (a helper function is optimised before it is
+// inlined, which reorders the loop-carried registers).
+#define RXG_WISHART_UPDATE(K, PR, R, N, LOGDET_W, WBAR, DF_OUT, IS_OUT, FE, STORE)                                    \
+    {                                                                                                               \
+        const double df = (PR).nu0 + (double)(N);                                                                   \
+        Mat<double, K, K> Psi;                                                                                      \
+        {                                                                                                           \
+            int q = 0;                                                                                              \
+            _Pragma("unroll") for (int k = 0; k < K; ++k)                                                           \
+                _Pragma("unroll") for (int l = 0; l <= k; ++l) {                                                    \
+                    Psi(k, l) = (PR).Psi0[k * K + l] + R[q];                                                        \
+                    Psi(l, k) = Psi(k, l);                                                                          \
+                    ++q;                                                                                            \
+                }                                                                                                   \
+        }                                                                                                           \
+        const Mat<double, K, K> Pinv = cholinv(Psi, bad);                                                           \
+        DF_OUT[(int64_t)it * batch + b] = (float)df;                                                                \
+        _Pragma("unroll") for (int k = 0; k < K; ++k)                                                               \
+            _Pragma("unroll") for (int l = 0; l < K; ++l)                                                           \
+                IS_OUT[(((int64_t)it * K + k) * K + l) * batch + b] = (float)Psi(k, l);                             \
+        Mat<double, K, K> Wn;                                                                                       \
+        _Pragma("unroll") for (int i = 0; i < K * K; ++i) Wn.a[i] = df * Pinv.a[i];                                 \
+        if (want_fe) {                                                                                              \
+            const double logdet_Psi = -2.0 * cholesky<double, K, true>(Psi, bad).neg_half_logdet;                   \
+            double psi_m = 0.0, lg = 0.0; /* sum_i psi((df - i)/2), sum_i [lgamma((nu0 - i)/2) - lgamma((df - i)/2)] */ \
+            _Pragma("unroll") for (int i = 0; i < K; ++i) {                                                         \
+                psi_m += digamma_d(0.5 * (df - i));                                                                 \
+                lg += lgamma(0.5 * ((PR).nu0 - i)) - lgamma(0.5 * (df - i));                                        \
+            }                                                                                                       \
+            const double Elogdet = psi_m + K * 0.69314718055994530942 - logdet_Psi;                                 \
+            double trR = 0.0, trP = 0.0; /* tr((E w - Wbar) R), tr(Psi0 inv(Psi)) */                                \
+            {                                                                                                       \
+                int q = 0;                                                                                          \
+                _Pragma("unroll") for (int k = 0; k < K; ++k)                                                       \
+                    _Pragma("unroll") for (int l = 0; l <= k; ++l) {                                                \
+                        const double f = (k == l) ? 1.0 : 2.0;                                                      \
+                        trR += f * (Wn(k, l) - WBAR(k, l)) * R[q++];                                                \
+                        trP += f * (PR).Psi0[k * K + l] * Pinv(k, l);                                               \
+                    }                                                                                               \
+            }                                                                                                       \
+            const double kl = -0.5 * (PR).nu0 * ((PR).logdet_Psi0 - logdet_Psi) + 0.5 * df * (trP - K) + lg +       \
+                              0.5 * (df - (PR).nu0) * psi_m;                                                        \
+            FE = FE + 0.5 * (N) * (LOGDET_W - Elogdet) + 0.5 * trR + kl;                                            \
+            if (STORE) io.fe[(int64_t)it * batch + b] = FE;                                                         \
+        }                                                                                                           \
+        WBAR = Wn;                                                                                                  \
+    }
+
+template <int D, int M, int LEARN>
 __global__ void __launch_bounds__(128)
-lgssm_vmp_wishart_kernel(const __grid_constant__ VmpWishModel<D, M> mdl, const VmpWishIO io) {
+lgssm_vmp_wishart_kernel(const __grid_constant__ VmpModel<D, M, LEARN> mdl, const VmpIO<LEARN> io) {
+    constexpr bool LQ = (LEARN & LEARN_Q) != 0, LP = (LEARN & LEARN_P) != 0;
     const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t batch = io.batch;
     if (b >= batch) return;
@@ -75,16 +208,25 @@ lgssm_vmp_wishart_kernel(const __grid_constant__ VmpWishModel<D, M> mdl, const V
     };
     Mat<double, M, M> Wbar;
 #pragma unroll
-    for (int i = 0; i < M * M; ++i) Wbar.a[i] = mdl.W0[i];
+    for (int i = 0; i < M * M; ++i) Wbar.a[i] = mdl.q.W0[i];
+    Mat<double, D, D> Wp;                  // E[w_p] under the previous q(w_p)
+    if constexpr (LP) {
+#pragma unroll
+        for (int i = 0; i < D * D; ++i) Wp.a[i] = mdl.p.W0[i];
+    }
     bool bad = false;
     const bool want_fe = io.fe != nullptr;
     Vec<float, D> mu;
 
     for (int it = 0; it < io.iterations; ++it) {
         const bool last = it == io.iterations - 1;
-        // ---- q(x) under Q = inv(Wbar)
-        const double logdet_W = -2.0 * cholesky<double, M, true>(Wbar, bad).neg_half_logdet;
-        const Mat<float, M, M> Q = convert<float>(cholinv(Wbar, bad));
+        // ---- q(x) under P = inv(Wp) and Q = inv(Wbar) (learned) or the known matrices
+        const double logdet_W = noise_logdet<LQ>(Wbar, bad);
+        const Mat<float, M, M> Q = noise_cov<LQ>(Wbar, known_q(mdl), bad);
+        const double logdet_Wp = noise_logdet<LP>(Wp, bad);
+        Mat<float, D, D> Pl;
+        if constexpr (LP) Pl = convert<float>(cholinv(Wp, bad));
+        const Mat<float, D, D>& Pb = LP ? Pl : P;
 #pragma unroll
         for (int i = 0; i < D; ++i) mu(i) = mdl.m0[i];
         Mat<float, D, D> S = S0;
@@ -105,7 +247,7 @@ lgssm_vmp_wishart_kernel(const __grid_constant__ VmpWishModel<D, M> mdl, const V
                 for (int k = 0; k < M; ++k) ynext[k] = __ldg(y + ((int64_t)(t + 1) * M + k) * batch + b);
                 onext = observed_at(t + 1);
             }
-            if (t > 0 || io.tf) chain_predict(A, P, u, NoInput{}, mu, S);
+            if (t > 0 || io.tf) chain_predict(A, Pb, u, NoInput{}, mu, S);
             if (obs) {
                 chain_update(B, Q, yt, want_fe, mu, S, bad, nle);
                 ++nobs;
@@ -122,7 +264,8 @@ lgssm_vmp_wishart_kernel(const __grid_constant__ VmpWishModel<D, M> mdl, const V
             }
         }
 
-        // ---- backward RTS pass and R_b = sum_{observed t} (y_t - B mu_t)(y_t - B mu_t)' + B Sigma_t B' (fp64)
+        // ---- backward RTS pass, R_q = sum_{observed t} (y_t - B mu_t)(y_t - B mu_t)' + B Sigma_t B' and
+        //      R_p = sum_t e e' + cov(x_{t+1} - A x_t | y), e = mu_{t+1} - A mu_t - u (fp64 sums of fp32 step terms)
         double R[M * (M + 1) / 2];
 #pragma unroll
         for (int q = 0; q < M * (M + 1) / 2; ++q) R[q] = 0.0;
@@ -143,7 +286,14 @@ lgssm_vmp_wishart_kernel(const __grid_constant__ VmpWishModel<D, M> mdl, const V
 #pragma unroll
                 for (int l = 0; l <= k; ++l) R[q++] += (double)Rt(k, l);
         };
-        if (obs) accumulate(mu, S, yt);
+        double Rp[D * (D + 1) / 2];
+        if constexpr (LP) {
+#pragma unroll
+            for (int q = 0; q < D * (D + 1) / 2; ++q) Rp[q] = 0.0;
+        }
+        if constexpr (LQ) {
+            if (obs) accumulate(mu, S, yt);
+        }
         Vec<float, D> mus = mu;          // smoothed at t+1
         Mat<float, D, D> Ss = S;
         float pm[D], pS[D * (D + 1) / 2], py[M];
@@ -178,7 +328,14 @@ lgssm_vmp_wishart_kernel(const __grid_constant__ VmpWishModel<D, M> mdl, const V
             for (int k = 0; k < M; ++k) yv(k) = py[k];
             const bool ob = po;
             if (t > 0) prefetch(t - 1);
-            chain_rts(A, P, u, NoInput{}, muf, Sf, mus, Ss, bad);
+            if constexpr (LP) {
+                const Vec<float, D> mnext = mus;
+                Mat<float, D, D> V;
+                chain_rts(A, Pb, u, NoInput{}, muf, Sf, mus, Ss, bad, PairCov<D>{A, V});
+                accumulate_pair(Rp, A, u, mnext, mus, V);
+            } else {
+                chain_rts(A, Pb, u, NoInput{}, muf, Sf, mus, Ss, bad);
+            }
             if (last) {
 #pragma unroll
                 for (int i = 0; i < D; ++i) mean[((int64_t)t * D + i) * batch + b] = mus(i);
@@ -187,59 +344,26 @@ lgssm_vmp_wishart_kernel(const __grid_constant__ VmpWishModel<D, M> mdl, const V
 #pragma unroll
                     for (int j = 0; j < D; ++j) cov[(((int64_t)t * D + i) * D + j) * batch + b] = Ss(i, j);
             }
-            if (ob) accumulate(mus, Ss, yv);
+            if constexpr (LQ) {
+                if (ob) accumulate(mus, Ss, yv);
+            }
+        }
+        if constexpr (LP) {
+            if (io.tf) {   // the transition from the prior state into x[1]: one more RTS step from (m0, S0), not written out
+                Vec<float, D> m0v, mx = mus;
+                Mat<float, D, D> Sx = Ss, V;
+#pragma unroll
+                for (int i = 0; i < D; ++i) m0v(i) = mdl.m0[i];
+                chain_rts(A, Pb, u, NoInput{}, m0v, S0, mx, Sx, bad, PairCov<D>{A, V});
+                accumulate_pair(Rp, A, u, mus, mx, V);
+            }
         }
         mu = mus;
 
-        // ---- q(w) = Wishart(df, inv(Psi)) and the free energy (fp64)
-        const double df = mdl.nu0 + (double)nobs;
-        Mat<double, M, M> Psi;
-        {
-            int q = 0;
-#pragma unroll
-            for (int k = 0; k < M; ++k)
-#pragma unroll
-                for (int l = 0; l <= k; ++l) {
-                    Psi(k, l) = mdl.Psi0[k * M + l] + R[q];
-                    Psi(l, k) = Psi(k, l);
-                    ++q;
-                }
-        }
-        const Mat<double, M, M> Pinv = cholinv(Psi, bad);
-        io.df[(int64_t)it * batch + b] = (float)df;
-#pragma unroll
-        for (int k = 0; k < M; ++k)
-#pragma unroll
-            for (int l = 0; l < M; ++l) io.inv_scale[(((int64_t)it * M + k) * M + l) * batch + b] = (float)Psi(k, l);
-        Mat<double, M, M> Wn;
-#pragma unroll
-        for (int i = 0; i < M * M; ++i) Wn.a[i] = df * Pinv.a[i];
-        if (want_fe) {
-            const double logdet_Psi = -2.0 * cholesky<double, M, true>(Psi, bad).neg_half_logdet;
-            double psi_m = 0.0, lg = 0.0;      // sum_i psi((df - i)/2), sum_i [lgamma((nu0 - i)/2) - lgamma((df - i)/2)]
-#pragma unroll
-            for (int i = 0; i < M; ++i) {
-                psi_m += digamma_d(0.5 * (df - i));
-                lg += lgamma(0.5 * (mdl.nu0 - i)) - lgamma(0.5 * (df - i));
-            }
-            const double Elogdet = psi_m + M * 0.69314718055994530942 - logdet_Psi;
-            double trR = 0.0, trP = 0.0;        // tr((E w - Wbar) R), tr(Psi0 inv(Psi))
-            {
-                int q = 0;
-#pragma unroll
-                for (int k = 0; k < M; ++k)
-#pragma unroll
-                    for (int l = 0; l <= k; ++l) {
-                        const double f = (k == l) ? 1.0 : 2.0;
-                        trR += f * (Wn(k, l) - Wbar(k, l)) * R[q++];
-                        trP += f * mdl.Psi0[k * M + l] * Pinv(k, l);
-                    }
-            }
-            const double kl = -0.5 * mdl.nu0 * (mdl.logdet_Psi0 - logdet_Psi) + 0.5 * df * (trP - M) + lg +
-                              0.5 * (df - mdl.nu0) * psi_m;
-            io.fe[(int64_t)it * batch + b] = nle + 0.5 * nobs * (logdet_W - Elogdet) + 0.5 * trR + kl;
-        }
-        Wbar = Wn;
+        // ---- q(w_p), q(w_q) = Wishart(df, inv(Psi)) and the free energy (fp64)
+        double fe = nle;
+        if constexpr (LP) RXG_WISHART_UPDATE(D, mdl.p, Rp, T - 1 + io.tf, logdet_Wp, Wp, io.df_p, io.inv_scale_p, fe, !LQ)
+        if constexpr (LQ) RXG_WISHART_UPDATE(M, mdl.q, R, nobs, logdet_W, Wbar, io.df, io.inv_scale, fe, true)
     }
     if (io.status) {
         bool nan = false;
@@ -249,32 +373,46 @@ lgssm_vmp_wishart_kernel(const __grid_constant__ VmpWishModel<D, M> mdl, const V
     }
 }
 
-template <int D, int M>
-int launch_vmp_wishart(rxg_ctx* ctx, const VmpWishHost& h, const VmpWishIO& io) {
-    VmpWishModel<D, M> mdl = {};
-    for (int i = 0; i < D * D; ++i) { mdl.A[i] = h.A[i]; mdl.P[i] = h.P[i]; mdl.S0[i] = h.S0[i]; }
+template <int D, int M, int LEARN>
+int launch_vmp_wishart(rxg_ctx* ctx, const VmpWishHost& h, const VmpNoiseIO& io) {
+    VmpModel<D, M, LEARN> mdl = {};
+    for (int i = 0; i < D * D; ++i) { mdl.A[i] = h.A[i]; mdl.P[i] = h.P ? h.P[i] : 0.f; mdl.S0[i] = h.S0[i]; }
     for (int i = 0; i < M * D; ++i) mdl.B[i] = h.B[i];
     for (int i = 0; i < D; ++i) { mdl.m0[i] = h.m0[i]; mdl.u[i] = h.u ? h.u[i] : 0.f; }
-    for (int i = 0; i < M * M; ++i) { mdl.Psi0[i] = h.Psi0[i]; mdl.W0[i] = h.W0[i]; }
-    mdl.nu0 = h.nu0;
-    mdl.logdet_Psi0 = h.logdet_Psi0;
+    for (int i = 0; i < M * M; ++i) { mdl.q.Psi0[i] = h.Psi0[i]; mdl.q.W0[i] = h.W0[i]; }
+    mdl.q.nu0 = h.nu0;
+    mdl.q.logdet_Psi0 = h.logdet_Psi0;
+    if constexpr (LEARN != LEARN_Q) {
+        for (int i = 0; i < M * M; ++i) mdl.Q[i] = h.Q ? h.Q[i] : 0.f;
+        for (int i = 0; i < D * D; ++i) { mdl.p.Psi0[i] = h.Psi_p0[i]; mdl.p.W0[i] = h.Wp0[i]; }
+        mdl.p.nu0 = h.nu_p0;
+        mdl.p.logdet_Psi0 = h.logdet_Psi_p0;
+    }
+    const VmpIO<LEARN>& kio = io;
     const int threads = 64;
     if (ctx->profile) { cudaEventRecord(ctx->ev[0], ctx->stream); cudaEventRecord(ctx->ev[1], ctx->stream); }
-    lgssm_vmp_wishart_kernel<D, M><<<(unsigned)((io.batch + threads - 1) / threads), threads, 0, ctx->stream>>>(mdl, io);
+    lgssm_vmp_wishart_kernel<D, M, LEARN><<<(unsigned)((io.batch + threads - 1) / threads), threads, 0, ctx->stream>>>(mdl, kio);
     if (ctx->profile) cudaEventRecord(ctx->ev[2], ctx->stream);
     ctx->launches += 1;
     return check_cuda(ctx, cudaGetLastError(), "lgssm_vmp_wishart_kernel launch");
 }
 
+#define RXG_VMP_DECL(PFX, DD, MM)                                                                           \
+    PFX template int launch_vmp_wishart<DD, MM, LEARN_Q>(rxg_ctx*, const VmpWishHost&, const VmpNoiseIO&);  \
+    PFX template int launch_vmp_wishart<DD, MM, LEARN_P>(rxg_ctx*, const VmpWishHost&, const VmpNoiseIO&);  \
+    PFX template int launch_vmp_wishart<DD, MM, LEARN_PQ>(rxg_ctx*, const VmpWishHost&, const VmpNoiseIO&);
+
 #ifdef RXG_VMP_M
-template int launch_vmp_wishart<1, RXG_VMP_M>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);
-template int launch_vmp_wishart<2, RXG_VMP_M>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);
-template int launch_vmp_wishart<3, RXG_VMP_M>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);
-template int launch_vmp_wishart<4, RXG_VMP_M>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);
-template int launch_vmp_wishart<5, RXG_VMP_M>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);
-template int launch_vmp_wishart<6, RXG_VMP_M>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);
+RXG_VMP_DECL(, 1, RXG_VMP_M) RXG_VMP_DECL(, 2, RXG_VMP_M) RXG_VMP_DECL(, 3, RXG_VMP_M)
+RXG_VMP_DECL(, 4, RXG_VMP_M) RXG_VMP_DECL(, 5, RXG_VMP_M) RXG_VMP_DECL(, 6, RXG_VMP_M)
 }  // namespace rxg
 #else
+
+#define RXG_VMP_EXTERN(DD)                                                                                  \
+    RXG_VMP_DECL(extern, DD, 1) RXG_VMP_DECL(extern, DD, 2) RXG_VMP_DECL(extern, DD, 3)                     \
+    RXG_VMP_DECL(extern, DD, 4) RXG_VMP_DECL(extern, DD, 5) RXG_VMP_DECL(extern, DD, 6)
+RXG_VMP_EXTERN(1) RXG_VMP_EXTERN(2) RXG_VMP_EXTERN(3) RXG_VMP_EXTERN(4) RXG_VMP_EXTERN(5) RXG_VMP_EXTERN(6)
+#undef RXG_VMP_EXTERN
 
 namespace {
 // fp64 Cholesky of the symmetrised (A + A')/2 on the host: false if it is not SPD; log det on success
@@ -299,28 +437,107 @@ bool host_spd(const float* a, int m, double* sym, double* logdet) {
     return true;
 }
 
-int dispatch(rxg_ctx* ctx, int d, int m, const VmpWishHost& h, const VmpWishIO& io) {
-#define RXG_VMP_CASE(DD, MM) case DD * 16 + MM: return launch_vmp_wishart<DD, MM>(ctx, h, io);
+template <int LEARN>
+int dispatch_shape(rxg_ctx* ctx, int d, int m, const VmpWishHost& h, const VmpNoiseIO& io) {
+#define RXG_VMP_CASE(DD, MM) case DD * 16 + MM: return launch_vmp_wishart<DD, MM, LEARN>(ctx, h, io);
 #define RXG_VMP_ROW(DD) RXG_VMP_CASE(DD, 1) RXG_VMP_CASE(DD, 2) RXG_VMP_CASE(DD, 3) RXG_VMP_CASE(DD, 4) \
                         RXG_VMP_CASE(DD, 5) RXG_VMP_CASE(DD, 6)
     switch (d * 16 + m) {
         RXG_VMP_ROW(1) RXG_VMP_ROW(2) RXG_VMP_ROW(3) RXG_VMP_ROW(4) RXG_VMP_ROW(5) RXG_VMP_ROW(6)
-        default: return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_vmp_wishart: d and m must be in 1..6 (got d=%d, m=%d)", d, m);
+        default: return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_vmp: d and m must be in 1..6 (got d=%d, m=%d)", d, m);
     }
 #undef RXG_VMP_ROW
 #undef RXG_VMP_CASE
 }
-}  // namespace
 
-#define RXG_VMP_EXTERN(DD)                                                                                  \
-    extern template int launch_vmp_wishart<DD, 1>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);          \
-    extern template int launch_vmp_wishart<DD, 2>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);          \
-    extern template int launch_vmp_wishart<DD, 3>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);          \
-    extern template int launch_vmp_wishart<DD, 4>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);          \
-    extern template int launch_vmp_wishart<DD, 5>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);          \
-    extern template int launch_vmp_wishart<DD, 6>(rxg_ctx*, const VmpWishHost&, const VmpWishIO&);
-RXG_VMP_EXTERN(1) RXG_VMP_EXTERN(2) RXG_VMP_EXTERN(3) RXG_VMP_EXTERN(4) RXG_VMP_EXTERN(5) RXG_VMP_EXTERN(6)
-#undef RXG_VMP_EXTERN
+// One noise of the call: the known matrix, or the Wishart prior and the initial E[w] when it is learned.
+struct NoiseArg {
+    char name;                 // 'p' or 'q'
+    int k;                     // its dimension (d or m)
+    const float *known, *inv_scale0, *init_E_W;
+    float nu0;
+    float *df, *inv_scale;     // outputs of a learned noise
+    bool learned() const { return inv_scale0 || init_E_W; }
+};
+
+// argument checks shared by both noises: exactly one of the known matrix and (inv_scale0, init_E_W); the outputs of a
+// learned noise and nothing else
+int check_noise(rxg_ctx* ctx, const char* who, const NoiseArg& a) {
+    if (!a.known == !a.learned())
+        return fail(ctx, RXG_ERR_BAD_ARG, "%s: pass exactly one of %c (known) and inv_scale_%c0 / init_E_W%c (learned)", who,
+                    a.name - 32, a.name, a.name);
+    if (a.learned() && !(a.inv_scale0 && a.init_E_W && a.df && a.inv_scale))
+        return fail(ctx, RXG_ERR_BAD_ARG, "%s: a learned %c needs inv_scale_%c0, init_E_W%c, df_%c and inv_scale_%c", who,
+                    a.name - 32, a.name, a.name, a.name, a.name);
+    if (!a.learned() && (a.df || a.inv_scale))
+        return fail(ctx, RXG_ERR_BAD_ARG, "%s: df_%c / inv_scale_%c must be NULL when %c is known", who, a.name, a.name,
+                    a.name - 32);
+    return RXG_OK;
+}
+
+int prior_of(rxg_ctx* ctx, const char* who, const NoiseArg& a, double* nu0, double* Psi0, double* logdet_Psi0, double* W0) {
+    if (!((double)a.nu0 > (double)(a.k - 1)) || !isfinite(a.nu0))
+        return fail(ctx, RXG_ERR_BAD_ARG, "%s: the prior's degrees of freedom must exceed %s - 1 (nu_%c0=%g, %s=%d)", who,
+                    a.name == 'p' ? "d" : "m", a.name, (double)a.nu0, a.name == 'p' ? "d" : "m", a.k);
+    *nu0 = (double)a.nu0;
+    double ld_w = 0.0;
+    if (!host_spd(a.inv_scale0, a.k, Psi0, logdet_Psi0))
+        return fail(ctx, RXG_ERR_BAD_ARG, "%s: inv_scale_%c0 is not symmetric positive definite", who, a.name);
+    if (!host_spd(a.init_E_W, a.k, W0, &ld_w))
+        return fail(ctx, RXG_ERR_BAD_ARG, "%s: init_E_W%c is not symmetric positive definite", who, a.name);
+    return RXG_OK;
+}
+
+// the one validation and dispatch path of rxg_lgssm_vmp_wishart_f32 and rxg_lgssm_vmp_noise_f32
+int vmp_noise(rxg_ctx* ctx, const char* who, int d, int m, int T, int64_t batch, int iterations, const float* A,
+              const float* B, const float* m0, const float* S0, const float* u, const NoiseArg& np, const NoiseArg& nq,
+              const float* y, const uint8_t* ymask, float* post_mean, float* post_cov, double* free_energy, int32_t* status,
+              unsigned flags) {
+    if (!ctx) return RXG_ERR_BAD_ARG;
+    const unsigned accepted = RXG_PTR_DEVICE | RXG_TRANSITION_FIRST | RXG_MASK_SHARED | RXG_ASYNC;
+    if (flags & ~accepted)
+        return fail(ctx, RXG_ERR_UNSUPPORTED, "%s: flags 0x%x are not supported (per-chain models, input sequences and the "
+                                              "shared covariance output do not apply: the covariances depend on the chain "
+                                              "through w)", who, flags & ~accepted);
+    if (!(flags & RXG_PTR_DEVICE)) return fail(ctx, RXG_ERR_UNSUPPORTED, "%s takes device pointers", who);
+    if (d < 1 || d > 6 || m < 1 || m > 6)
+        return fail(ctx, RXG_ERR_UNSUPPORTED, "%s: d and m must be in 1..6 (got d=%d, m=%d)", who, d, m);
+    if (T < 1 || batch < 1 || iterations < 1)
+        return fail(ctx, RXG_ERR_BAD_ARG, "%s: T, batch and iterations must be >= 1", who);
+    if (!A || !B || !m0 || !S0 || !y || !post_mean || !post_cov)
+        return fail(ctx, RXG_ERR_BAD_ARG, "%s: null pointer argument", who);
+    int rc;
+    if ((rc = check_noise(ctx, who, np)) != RXG_OK || (rc = check_noise(ctx, who, nq)) != RXG_OK) return rc;
+    if (!np.learned() && !nq.learned())
+        return fail(ctx, RXG_ERR_BAD_ARG, "%s: P and Q are both known: that is the plain smoother (rxg_lgssm_smooth_f32)", who);
+    VmpWishHost h = {};
+    h.A = A; h.B = B; h.m0 = m0; h.S0 = S0; h.u = u; h.P = np.known; h.Q = nq.known;
+    if (nq.learned() && (rc = prior_of(ctx, who, nq, &h.nu0, h.Psi0, &h.logdet_Psi0, h.W0)) != RXG_OK) return rc;
+    if (np.learned() && (rc = prior_of(ctx, who, np, &h.nu_p0, h.Psi_p0, &h.logdet_Psi_p0, h.Wp0)) != RXG_OK) return rc;
+    RXG_CUDA(ctx, cudaSetDevice(ctx->device));
+    VmpNoiseIO io;
+    io.y = y; io.ymask = nullptr; io.tmask = nullptr;
+    io.mean = post_mean; io.cov = post_cov; io.df = nq.df; io.inv_scale = nq.inv_scale; io.fe = free_energy;
+    io.status = status; io.df_p = np.df; io.inv_scale_p = np.inv_scale;
+    io.T = T; io.iterations = iterations; io.tf = (flags & RXG_TRANSITION_FIRST) ? 1 : 0;
+    io.batch = batch;
+    if (ymask) {
+        if (flags & RXG_MASK_SHARED) {
+            LgssmCall c = {};
+            const int rs = stage_shared_mask(ctx, T, ymask, c);
+            if (rs != RXG_OK) return rs;
+            io.tmask = c.tmask;
+        } else {
+            io.ymask = ymask;
+        }
+    }
+    rc = !np.learned() ? dispatch_shape<LEARN_Q>(ctx, d, m, h, io)
+                       : (nq.learned() ? dispatch_shape<LEARN_PQ>(ctx, d, m, h, io) : dispatch_shape<LEARN_P>(ctx, d, m, h, io));
+    if (rc != RXG_OK) return rc;
+    if (!(flags & RXG_ASYNC)) RXG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return RXG_OK;
+}
+}  // namespace
 
 }  // namespace rxg
 
@@ -331,50 +548,23 @@ extern "C" int rxg_lgssm_vmp_wishart_f32(rxg_ctx* ctx, int d, int m, int T, int6
                                          float nu0, const float* inv_scale0, const float* init_E_W, const float* y,
                                          const uint8_t* ymask, float* post_mean, float* post_cov, float* df,
                                          float* inv_scale, double* free_energy, int32_t* status, unsigned flags) {
-    if (!ctx) return RXG_ERR_BAD_ARG;
-    const unsigned accepted = RXG_PTR_DEVICE | RXG_TRANSITION_FIRST | RXG_MASK_SHARED | RXG_ASYNC;
-    if (flags & ~accepted)
-        return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_vmp_wishart: flags 0x%x are not supported (per-chain models, input "
-                                              "sequences and the shared covariance output do not apply: the covariances "
-                                              "depend on the chain through w)", flags & ~accepted);
-    if (!(flags & RXG_PTR_DEVICE)) return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_vmp_wishart takes device pointers");
-    if (d < 1 || d > 6 || m < 1 || m > 6)
-        return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_vmp_wishart: d and m must be in 1..6 (got d=%d, m=%d)", d, m);
-    if (T < 1 || batch < 1 || iterations < 1)
-        return fail(ctx, RXG_ERR_BAD_ARG, "lgssm_vmp_wishart: T, batch and iterations must be >= 1");
-    if (!A || !B || !P || !m0 || !S0 || !inv_scale0 || !init_E_W || !y || !post_mean || !post_cov || !df || !inv_scale)
-        return fail(ctx, RXG_ERR_BAD_ARG, "lgssm_vmp_wishart: null pointer argument");
-    if (!((double)nu0 > (double)(m - 1)) || !isfinite(nu0))
-        return fail(ctx, RXG_ERR_BAD_ARG, "lgssm_vmp_wishart: the prior's degrees of freedom must exceed m - 1 (nu0=%g, m=%d)",
-                    (double)nu0, m);
-    VmpWishHost h;
-    h.A = A; h.B = B; h.P = P; h.m0 = m0; h.S0 = S0; h.u = u;
-    h.nu0 = (double)nu0;
-    double ld_w = 0.0;
-    if (!host_spd(inv_scale0, m, h.Psi0, &h.logdet_Psi0))
-        return fail(ctx, RXG_ERR_BAD_ARG, "lgssm_vmp_wishart: inv_scale0 is not symmetric positive definite");
-    if (!host_spd(init_E_W, m, h.W0, &ld_w))
-        return fail(ctx, RXG_ERR_BAD_ARG, "lgssm_vmp_wishart: init_E_W is not symmetric positive definite");
-    RXG_CUDA(ctx, cudaSetDevice(ctx->device));
-    VmpWishIO io;
-    io.y = y; io.ymask = nullptr; io.tmask = nullptr;
-    io.mean = post_mean; io.cov = post_cov; io.df = df; io.inv_scale = inv_scale; io.fe = free_energy; io.status = status;
-    io.T = T; io.iterations = iterations; io.tf = (flags & RXG_TRANSITION_FIRST) ? 1 : 0;
-    io.batch = batch;
-    if (ymask) {
-        if (flags & RXG_MASK_SHARED) {
-            LgssmCall c = {};
-            const int rc = stage_shared_mask(ctx, T, ymask, c);
-            if (rc != RXG_OK) return rc;
-            io.tmask = c.tmask;
-        } else {
-            io.ymask = ymask;
-        }
-    }
-    const int rc = dispatch(ctx, d, m, h, io);
-    if (rc != RXG_OK) return rc;
-    if (!(flags & RXG_ASYNC)) RXG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return RXG_OK;
+    const NoiseArg np = {'p', d, P, nullptr, nullptr, 0.f, nullptr, nullptr};
+    const NoiseArg nq = {'q', m, nullptr, inv_scale0, init_E_W, nu0, df, inv_scale};
+    return vmp_noise(ctx, "lgssm_vmp_wishart", d, m, T, batch, iterations, A, B, m0, S0, u, np, nq, y, ymask, post_mean,
+                     post_cov, free_energy, status, flags);
+}
+
+extern "C" int rxg_lgssm_vmp_noise_f32(rxg_ctx* ctx, int d, int m, int T, int64_t batch, int iterations, const float* A,
+                                       const float* B, const float* m0, const float* S0, const float* u, const float* P,
+                                       float nu_p0, const float* inv_scale_p0, const float* init_E_Wp, const float* Q,
+                                       float nu_q0, const float* inv_scale_q0, const float* init_E_Wq, const float* y,
+                                       const uint8_t* ymask, float* post_mean, float* post_cov, float* df_p,
+                                       float* inv_scale_p, float* df_q, float* inv_scale_q, double* free_energy,
+                                       int32_t* status, unsigned flags) {
+    const NoiseArg np = {'p', d, P, inv_scale_p0, init_E_Wp, nu_p0, df_p, inv_scale_p};
+    const NoiseArg nq = {'q', m, Q, inv_scale_q0, init_E_Wq, nu_q0, df_q, inv_scale_q};
+    return vmp_noise(ctx, "lgssm_vmp_noise", d, m, T, batch, iterations, A, B, m0, S0, u, np, nq, y, ymask, post_mean,
+                     post_cov, free_energy, status, flags);
 }
 
 #endif  // RXG_VMP_M

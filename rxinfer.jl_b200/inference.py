@@ -108,6 +108,26 @@ class linear_gaussian_ssm_wishart_precision:
     prior_on_previous_state: bool = False
 
 
+@dataclass
+class linear_gaussian_ssm_wishart_noise:
+    """LGSSM with an unknown process precision matrix per series, alone or together with an unknown observation precision:
+    ``w_p ~ p_prior; w_q ~ q_prior; x[1] ~ x0; x[t] ~ N(A x[t-1] + u, precision = w_p); y[t] ~ N(B x[t], precision = w_q)``,
+    run with ``constraints = q(x, w_p, w_q) = q(x)q(w_p)q(w_q)``, ``initialization = q(w_p) = p_init, q(w_q) = q_init`` and
+    ``iterations``.  Each noise is either known (``P`` / ``Q``, a covariance) or learned (``*_prior`` and ``*_init`` as
+    ``Wishart(df, scale)``, both required); at least one is learned.  ``x0 = (mean, cov)``."""
+    A: np.ndarray
+    B: np.ndarray
+    x0: tuple
+    P: np.ndarray = None
+    Q: np.ndarray = None
+    p_prior: Wishart = None
+    p_init: Wishart = None
+    q_prior: Wishart = None
+    q_init: Wishart = None
+    u: object = None
+    prior_on_previous_state: bool = False
+
+
 class KeepLast:
     """``predictvars`` / ``returnvars`` marker: keep the result of the last iteration (the reference's ``KeepLast()``)."""
 
@@ -218,7 +238,7 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             raise NotImplementedError(f"options {sorted(bad)} are outside the batched hot path")
     if data is not None and datastream is not None:
         raise ValueError("`data` and `datastream` are mutually exclusive")    # reference: inference.jl argument check
-    if isinstance(model, linear_gaussian_ssm_wishart_precision):
+    if isinstance(model, (linear_gaussian_ssm_wishart_precision, linear_gaussian_ssm_wishart_noise)):
         if predictvars is not None:
             raise NotImplementedError("predictvars: predictions of the Wishart-precision LGSSM are outside the batched hot path")
         if data is not None and "u" in data:
@@ -336,6 +356,32 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]),
                                                "w": WishartFast(r["df"], r["inv_scale"])},
                                    model=model, free_energy=r["free_energy"])
+        if isinstance(model, linear_gaussian_ssm_wishart_noise):
+            kw = {}
+            for name in ("p", "q"):
+                known, prior, init = getattr(model, name.upper()), getattr(model, f"{name}_prior"), getattr(model, f"{name}_init")
+                if known is not None:
+                    kw[name.upper()] = known
+                elif prior is not None and init is not None:
+                    kw[f"{name}_prior"], kw[f"{name}_init"] = (prior.df, prior.inv_scale()), init.mean()
+                else:
+                    kw[f"{name}_prior"], kw[f"{name}_init"] = prior, init    # Context names what is missing
+                if known is not None and (prior is not None or init is not None):
+                    raise ValueError(f"{name.upper()} is known: pass either {name.upper()} or {name}_prior / {name}_init")
+            r = ctx.lgssm_vmp_noise(y, model.A, model.B, model.x0[0], model.x0[1], **kw, u=model.u, mask=mask,
+                                    transition_first=model.prior_on_previous_state, iterations=iterations or 1,
+                                    want_free_energy=bool(free_energy))
+            bad = r["status"] != 0
+            if bool(bad.any()):
+                codes = sorted({L.STATUS_NAMES.get(int(c), str(int(c))) for c in r["status"][bad].unique().tolist()})
+                raise L.RxGaussError(L.RXG_ERR_NOT_SPD if "NOT_SPD" in codes else int(r["status"][bad][0]),
+                                     f"{int(bad.sum())} of {bad.numel()} chains flagged {codes}")
+            # x = KeepLast(), w_p / w_q = KeepEach() (leading iteration axis) for the learned precisions
+            post = {"x": MvNormalMeanCovariance(r["mean"], r["cov"])}
+            for name in ("p", "q"):
+                if r[f"df_{name}"] is not None:
+                    post[f"w_{name}"] = WishartFast(r[f"df_{name}"], r[f"inv_scale_{name}"])
+            return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
         if isinstance(model, latent_autoregressive):
             yy = y[:, 0] if y.dim() == 3 else y
             r = ctx.lar_vmp(yy.contiguous(), model.order, model.tau, iterations=iterations or 1, gamma_prior=model.gamma_prior,

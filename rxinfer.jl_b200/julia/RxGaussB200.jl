@@ -211,6 +211,13 @@ lgssm_vmp_wishart(ctx, d, m, T, batch, its, A, B, P, m0, S0, u, nu0, iS0, EW0, y
         (Ptr{Cvoid}, Cint, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, Cfloat, F32P, F32P, F32P, Ptr{UInt8},
          F32P, F32P, F32P, F32P, Ptr{Float64}, Ptr{Int32}, Cuint),
         ctx.handle, d, m, T, batch, its, A, B, P, m0, S0, u, nu0, iS0, EW0, y, mask, mean, cov, df, iS, fe, st, fl))
+lgssm_vmp_noise(ctx, d, m, T, batch, its, A, B, m0, S0, u, P, nup, iSp0, EWp0, Q, nuq, iSq0, EWq0, y, mask, mean, cov,
+                dfp, iSp, dfq, iSq, fe, st, fl) =
+    check(ctx, ccall((:rxg_lgssm_vmp_noise_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, Cfloat, F32P, F32P, F32P, Cfloat, F32P,
+         F32P, F32P, Ptr{UInt8}, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Float64}, Ptr{Int32}, Cuint),
+        ctx.handle, d, m, T, batch, its, A, B, m0, S0, u, P, nup, iSp0, EWp0, Q, nuq, iSq0, EWq0, y, mask, mean, cov,
+        dfp, iSp, dfq, iSq, fe, st, fl))
 mv_iid_wishart_vmp(ctx, d, N, batch, its, mu0, L0, nu0, iS0, EP0, y, mm, mc, df, iS, st, fl) =
     check(ctx, ccall((:rxg_mv_iid_wishart_vmp_f32, LIB), Cint,
         (Ptr{Cvoid}, Cint, Cint, Int64, Cint, F32P, F32P, Cfloat, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Int32}, Cuint),
@@ -700,6 +707,49 @@ function lgssm_wishart(ctx::Context, y::Array{Float32, 3}; A::Matrix, B::Matrix,
         Ptr{UInt8}(C_NULL), mean.ptr, cov.ptr, df.ptr, iS.ptr, Ptr{Float64}(dfe.ptr), Ptr{Int32}(st.ptr), fl)
     fe = reshape(reinterpret(Float64, vec(download(dfe))), batch, iterations)
     return download(mean), download(cov), download(df), download(iS), fe, reinterpret(Int32, download(st))
+end
+
+"""VMP around the multivariate smoother with an unknown process precision matrix per series, alone or together with an
+unknown observation precision (`rxg_lgssm_vmp_noise_f32`; `constraints = q(x, w_p, w_q) = q(x)q(w_p)q(w_q)`); host data
+`y[batch, m, T]`.  Each noise is either known (`P` / `Q`, a covariance) or learned: `p_prior = (df, inverse scale)` of its
+Wishart prior and `p_init` = E[w_p] of the initial q(w_p), both required (likewise `q_prior` / `q_init`).  Returns q(x) of
+the last iteration (mean `[batch, d, T]`, cov `[batch, d, d, T]`), q(w_p) and q(w_q) after every iteration (df
+`[batch, iterations]`, inverse scale `[batch, k, k, iterations]`; `nothing` for a known noise), the Bethe free energy
+`[batch, iterations]` (Float64) and the per-series status."""
+function lgssm_wishart_noise(ctx::Context, y::Array{Float32, 3}; A::Matrix, B::Matrix, x0 = nothing, u = nothing,
+                             P = nothing, p_prior = nothing, p_init = nothing, Q = nothing, q_prior = nothing,
+                             q_init = nothing, iterations = 10, transition_first = false)
+    batch, m, T = size(y)
+    d = size(A, 1)
+    for (name, known, prior, init) in (("P", P, p_prior, p_init), ("Q", Q, q_prior, q_init))
+        known === nothing || (prior === nothing && init === nothing) ||
+            throw(ArgumentError("$name is known: pass either $name or its prior / init"))
+        known !== nothing || (prior !== nothing && init !== nothing) ||
+            throw(ArgumentError("$name is learned: pass its prior = (df, inverse scale) and init = E[w] (no default q(w))"))
+    end
+    P === nothing || Q === nothing || throw(ArgumentError("P and Q are both known: that is the plain smoother"))
+    m0, S0 = x0 === nothing ? (zeros(Float32, d), Matrix{Float32}(100I, d, d)) : (Float32.(x0[1]), Float32.(x0[2]))
+    rowmajor(M) = M === nothing ? nothing : Matrix{Float32}(permutedims(M))       # row-major host matrices for the C side
+    At, Bt, S0t, Pt, Qt = rowmajor(A), rowmajor(B), rowmajor(S0), rowmajor(P), rowmajor(Q)
+    nup, iSp0, EWp0 = P === nothing ? (Float32(p_prior[1]), rowmajor(p_prior[2]), rowmajor(p_init)) : (0f0, nothing, nothing)
+    nuq, iSq0, EWq0 = Q === nothing ? (Float32(q_prior[1]), rowmajor(q_prior[2]), rowmajor(q_init)) : (0f0, nothing, nothing)
+    uv = u === nothing ? nothing : Float32.(u)
+    ptr(M) = M === nothing ? NULLF : pointer(M)
+    dy = upload(ctx, y)
+    mean, cov = DeviceArray(ctx, batch, d, T), DeviceArray(ctx, batch, d, d, T)
+    dfp, iSp = P === nothing ? (DeviceArray(ctx, batch, iterations), DeviceArray(ctx, batch, d, d, iterations)) : (nothing, nothing)
+    dfq, iSq = Q === nothing ? (DeviceArray(ctx, batch, iterations), DeviceArray(ctx, batch, m, m, iterations)) : (nothing, nothing)
+    dptr(a) = a === nothing ? NULLF : a.ptr
+    dfe = DeviceArray(ctx, 2 * batch * iterations)                  # fp64 output: two Float32 slots per value
+    st = DeviceArray(ctx, batch)
+    fl = RXG_PTR_DEVICE | (transition_first ? RXG_TRANSITION_FIRST : UInt32(0))
+    GC.@preserve At Bt m0 S0t uv Pt iSp0 EWp0 Qt iSq0 EWq0 Lib.lgssm_vmp_noise(ctx, d, m, T, batch, iterations, pointer(At),
+        pointer(Bt), pointer(m0), pointer(S0t), ptr(uv), ptr(Pt), nup, ptr(iSp0), ptr(EWp0), ptr(Qt), nuq, ptr(iSq0), ptr(EWq0),
+        dy.ptr, Ptr{UInt8}(C_NULL), mean.ptr, cov.ptr, dptr(dfp), dptr(iSp), dptr(dfq), dptr(iSq), Ptr{Float64}(dfe.ptr),
+        Ptr{Int32}(st.ptr), fl)
+    fe = reshape(reinterpret(Float64, vec(download(dfe))), batch, iterations)
+    dl(a) = a === nothing ? nothing : download(a)
+    return download(mean), download(cov), dl(dfp), dl(iSp), dl(dfq), dl(iSq), fe, reinterpret(Int32, download(st))
 end
 
 """Fused structured VMP of the latent autoregressive model (lar_tests.jl:52-122); `y[batch, T]`.  Returns the reference's
