@@ -218,7 +218,8 @@ int rxg_wishart_mean_f32(rxg_ctx*, int64_t n, int d, const float* df, const floa
  *   m ~ MvNormal(mu0, inv(Lambda0)),  P ~ Wishart(nu0, inv(inv_scale0)),  y[i] ~ MvNormal(m, inv(P)),  q(m) q(P)
  * [ref: model, constraints and initialisation test/models/iid/mv_iid_precision_tests.jl:10-41].  y[N][d][batch];
  * init_E_P[d][d] = mean of the initial q(P) (host); outputs q(m) = (m_mean[d][batch], m_cov[d][d][batch]),
- * q(P) = Wishart(df[batch], inv(inv_scale[d][d][batch])).  d <= 6.                                                */
+ * q(P) = Wishart(df[batch], inv(inv_scale[d][d][batch])).  d <= 6 (d = 7.. -> RXG_ERR_UNSUPPORTED); d, N, iterations
+ * >= 1 and nu0 > d - 1, else RXG_ERR_BAD_ARG.  Device pointers (RXG_ERR_UNSUPPORTED otherwise).                  */
 int rxg_mv_iid_wishart_vmp_f32(rxg_ctx*, int d, int N, int64_t batch, int iterations, const float* mu0,
                                const float* Lambda0, float nu0, const float* inv_scale0, const float* init_E_P,
                                const float* y, float* m_mean, float* m_cov, float* df, float* inv_scale,
@@ -346,7 +347,8 @@ int rxg_lgssm_filter_f32(rxg_ctx*, int d, int m, int T, int64_t batch, const flo
  * (d = m = 1): y[t] ~ N(x[t], 1/tau), tau ~ Gamma(a0, b0), q(x) q(tau)
  * [ref: rules of test/models/aliases/aliases_gamma_tests.jl; use case
  *  test/callbacks/benchmark_tests.jl:8-37].  y[T][batch]; outputs post_mean/var[T][batch],
- * shape/rate[batch].                                                                            */
+ * shape/rate[batch].  T, iterations >= 1 and v_proc, v0, a0, b0, init_E_tau > 0, else
+ * RXG_ERR_BAD_ARG.  Device pointers (RXG_ERR_UNSUPPORTED otherwise).                            */
 int rxg_lgssm_vmp_gamma_f32(rxg_ctx*, int T, int64_t batch, int iterations, float a, float v_proc,
                             float m0, float v0, float a0, float b0, float init_E_tau,
                             const float* y, float* post_mean, float* post_var, float* shape,

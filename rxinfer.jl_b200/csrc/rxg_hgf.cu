@@ -497,6 +497,10 @@ int rxg_lgssm_vmp_gamma_fe_f32(rxg_ctx* ctx, int T, int64_t batch, int iteration
     if (!ctx) return RXG_ERR_BAD_ARG;
     if (T < 1 || batch < 1 || iterations < 1 || !y || !post_mean || !post_var || !shape || !rate)
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, "lgssm_vmp_gamma: bad argument");
+    // variances, the Gamma prior and the initial E[tau] must be positive (NaN is refused too): lgammaf(a0), logf(b0), the
+    // observation variance 1 / E[tau] and the RTS gain's division by the predicted variance need it
+    if (!(v_proc > 0.f) || !(v0 > 0.f) || !(a0 > 0.f) || !(b0 > 0.f) || !(init_E_tau > 0.f))
+        return rxg::fail(ctx, RXG_ERR_BAD_ARG, "lgssm_vmp_gamma: v_proc, v0, a0, b0 and init_E_tau must be positive");
     if (!(flags & RXG_PTR_DEVICE)) return rxg::fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_vmp_gamma takes device pointers");
     RXG_CUDA(ctx, cudaSetDevice(ctx->device));
     vmp_gamma_kernel<<<(unsigned)((batch + 127) / 128), 128, 0, ctx->stream>>>(

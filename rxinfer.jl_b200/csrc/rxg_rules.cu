@@ -648,6 +648,8 @@ int rxg_mv_iid_wishart_vmp_f32(rxg_ctx* ctx, int d, int N, int64_t batch, int it
         !m_cov || !df || !inv_scale)
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, "mv_iid_wishart_vmp: bad argument");
     if (d > 6) return rxg::fail(ctx, RXG_ERR_UNSUPPORTED, "mv_iid_wishart_vmp: d=%d unsupported (1-6)", d);
+    if (!(nu0 > (float)(d - 1)))                        // a proper Wishart prior, as the LGSSM Wishart entries require
+        return rxg::fail(ctx, RXG_ERR_BAD_ARG, "mv_iid_wishart_vmp: nu0 must exceed d - 1");
     RXG_CUDA(ctx, cudaSetDevice(ctx->device));
     // prior block (host) -> device workspace: mu0[d], Lambda0[d*d], nu0, invS0[d*d], E[P]_init[d*d]
     const int dd = d * d;
