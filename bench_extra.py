@@ -7,6 +7,7 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
   python bench_extra.py --which inputs       (opt-in: known per-step inputs u[t], shared and per-chain sequences)
   python bench_extra.py --which vmp_wishart  (opt-in: Wishart-precision VMP around the smoother vs the composed path)
   python bench_extra.py --which vmp_noise    (opt-in: learned process precision, alone and with the observation precision)
+  python bench_extra.py --which vmp_transition (opt-in: learned transition matrix, alone and with the noise precisions)
 """
 from __future__ import annotations
 
@@ -266,6 +267,78 @@ def bench_vmp_noise(ctx, peak):
         torch.cuda.empty_cache()
 
 
+def vmp_transition_counts(d, m, learn):
+    """Bytes and FLOPs per (chain, step, iteration) of one non-final iteration of the transition-learning VMP (learn =
+    "A", "AP", "APQ"): vmp_wishart_counts of the noise part plus, per step, the tilt exp(-1/2 x' Xi x) (S L, L' S L,
+    a d x d Cholesky, Z = S L Ls^-T, the mean and the downdate) and the source-state statistics (X = G Ss (I - A G)' -
+    C A', Sxx, Sxr).  The fp64 d^2 x d^2 algebra runs once per iteration, not per step, and is not counted."""
+    tri = lambda n: n * (n + 1) // 2
+    noise = learn.replace("A", "")
+    if noise:
+        by, _, fl = vmp_wishart_counts(d, m, False, learn=noise)
+    else:       # A alone: y read forward only, plus the stash in both directions
+        by = 4 * m + 2 * 4 * (d + tri(d))
+        _, _, fl = vmp_wishart_counts(d, m, False, learn="P")
+        fl -= 2 * (3 * d ** 3 + 2 * tri(d) * d + d * d + tri(d))      # no R_p pair term
+    tilt = d ** 3 + tri(d) * d + d ** 3 // 6 + d ** 3 // 2 + d * d + d * d // 2 + d * d + tri(d) * d
+    stats = d ** 3 + d ** 3 + d ** 3 + d ** 3 + d * d + tri(d) + d * d
+    return by, fl + 2 * (tilt + stats)
+
+
+def bench_vmp_transition(ctx, peak):
+    """Learned transition matrix (rxg_lgssm_vmp_transition_f32: A alone, A + P, A + P + Q) against the learned noise
+    precisions with A known (rxg_lgssm_vmp_noise_f32, learn P + Q), alternated in one run on the same data; kernel time
+    from CUDA events around the launch (rxg_set_profiling)."""
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(16)
+    T, nb, its = 1000, 65536, 10
+    for d in (4, 2):
+        m = d
+        mod = notebook_model_f32() if d == 4 else notebook_model_d2_f32()
+        y = torch.randn(T, m, nb, device="cuda", generator=g) * 3.3
+        q_prior, q_init = (m + 2.0, 10.0 * np.eye(m)), 0.1 * np.eye(m)
+        p_prior, p_init = (d + 2.0, 0.1 * np.eye(d)), np.linalg.inv(np.asarray(mod["P"], np.float64))
+        n = d * d
+        a_prior = (np.asarray(mod["A"], np.float64).reshape(-1), np.eye(n))
+        a_init = (np.asarray(mod["A"], np.float64).reshape(-1), 0.01 * np.eye(n))
+        common = dict(a_prior=a_prior, a_init=a_init, iterations=its)
+        calls = {"PQ": lambda: ctx.lgssm_vmp_noise(y, mod["A"], mod["B"], mod["m0"], mod["S0"], p_prior=p_prior,
+                                                   p_init=p_init, q_prior=q_prior, q_init=q_init, iterations=its),
+                 "A": lambda: ctx.lgssm_vmp_transition(y, mod["B"], mod["m0"], mod["S0"], P=mod["P"], Q=mod["Q"], **common),
+                 "AP": lambda: ctx.lgssm_vmp_transition(y, mod["B"], mod["m0"], mod["S0"], p_prior=p_prior, p_init=p_init,
+                                                        Q=mod["Q"], **common),
+                 "APQ": lambda: ctx.lgssm_vmp_transition(y, mod["B"], mod["m0"], mod["S0"], p_prior=p_prior,
+                                                         p_init=p_init, q_prior=q_prior, q_init=q_init, **common)}
+        kern = {k: [] for k in calls}
+        call = {k: [] for k in calls}
+        for _ in range(3):
+            for k, fn in calls.items():
+                call[k].append(timed(fn, warm=2, reps=3))
+                ctx.set_profiling(True)
+                fn()
+                kern[k].append(ctx.profile_last_ms()[0])
+                ctx.set_profiling(False)
+        for k in calls:
+            kms, cms = float(np.median(kern[k])), float(np.median(call[k]))
+            if k == "PQ":
+                bf, _, fl = vmp_wishart_counts(d, m, False, learn="PQ")
+            else:
+                bf, fl = vmp_transition_counts(d, m, k)
+            nn = T * nb * its
+            t_hbm, t_fp32 = bf * nn / (peak * 1e9), fl * nn / 67e12
+            print(json.dumps({"what": f"transition-learning VMP around the smoother, learn {k} (lgssm_vmp_wishart_kernel)",
+                              "learn": k, "d": d, "m": m, "T": T, "batch": nb, "iterations": its, "kernel_ms": kms,
+                              "kernel_ms_runs": kern[k], "call_ms": cms, "ms_per_iteration": kms / its,
+                              "bytes_per_chain_step_iteration": bf, "flops_per_chain_step_iteration": fl,
+                              "achieved_GBs": bf * nn / kms / 1e6, "achieved_TFLOPs": fl * nn / kms / 1e9,
+                              "bound": "hbm" if t_hbm >= t_fp32 else "fp32",
+                              "kernel_frac_of_hbm_bound": t_hbm * 1e3 / kms,
+                              "kernel_frac_of_bound": max(t_hbm, t_fp32) * 1e3 / kms,
+                              "peak_hbm_gbs": peak, "peak_fp32_tflops": 67, "gpu": gname, "power_limit": plim}), flush=True)
+        del y
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -281,6 +354,8 @@ def main():
         bench_vmp_wishart(ctx, peak)
     if "vmp_noise" in which:
         bench_vmp_noise(ctx, peak)
+    if "vmp_transition" in which:
+        bench_vmp_transition(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

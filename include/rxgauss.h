@@ -400,6 +400,29 @@ int rxg_lgssm_vmp_noise_f32(rxg_ctx*, int d, int m, int T, int64_t batch, int it
                             const float* inv_scale_q0, const float* init_E_Wq, const float* y, const uint8_t* ymask,
                             float* post_mean, float* post_cov, float* df_p, float* inv_scale_p, float* df_q,
                             float* inv_scale_q, double* free_energy, int32_t* status, unsigned flags);
+/* The same VMP that also learns the TRANSITION MATRIX per chain (RxInfer's ContinuousTransition node with a Gaussian
+ * prior on a = vec(A), reshaped linearly to A):
+ *   a ~ N(a_mean0, a_cov0); w_p ~ Wishart(nu_p0, inv(inv_scale_p0)) (else P known); w_q likewise (else Q known);
+ *   x[1] ~ N(m0, S0) (RXG_TRANSITION_FIRST: one transition earlier); x[t] ~ N(A x[t-1] + u, inv(w_p));
+ *   y[t] ~ N(B x[t], inv(w_q)); q(x) q(a) q(w_p) q(w_q), q(x) structured over the chain.
+ * a is indexed row-major, a[i*d + j] = A[i][j], like every matrix of this ABI: a_mean0 / a_init_mean [d][d],
+ * a_cov0 / a_init_cov [d*d][d*d] (SPD), the prior and E[a], cov(a) of the initial q(a), shared by every chain.  Each
+ * noise is known or learned as for rxg_lgssm_vmp_noise_f32; both known is allowed (A alone is learned).  One iteration:
+ * q(x) under (E[A], E[w_p], E[w_q]) with the factor exp(-1/2 x' Xi x), Xi = E[(A - E[A])' E[w_p] (A - E[A])], on the
+ * source state of every transition; then q(a) (with the E[w_p] of that q(x)), q(w_p) (with the new q(a)) and q(w_q).
+ * Outputs a_mean[iterations][d][d][batch] and a_cov[iterations][d*d][d*d][batch] (after EVERY iteration), the noise
+ * outputs and free_energy as rxg_lgssm_vmp_noise_f32 (the Bethe free energy gains KL(q(a) || prior)).  d in 1..4, m in
+ * 1..6, device data, else RXG_ERR_UNSUPPORTED, as are the flags rxg_lgssm_vmp_noise_f32 refuses; a non-SPD a_cov0 /
+ * a_init_cov, a missing a_mean / a_cov and every argument rxg_lgssm_vmp_noise_f32 refuses except two known noises give
+ * RXG_ERR_BAD_ARG.  status[b] flags a non-positive pivot (also of Xi and of the precision of q(a)).              */
+int rxg_lgssm_vmp_transition_f32(rxg_ctx*, int d, int m, int T, int64_t batch, int iterations, const float* a_mean0,
+                                 const float* a_cov0, const float* a_init_mean, const float* a_init_cov, const float* B,
+                                 const float* m0, const float* S0, const float* u, const float* P, float nu_p0,
+                                 const float* inv_scale_p0, const float* init_E_Wp, const float* Q, float nu_q0,
+                                 const float* inv_scale_q0, const float* init_E_Wq, const float* y, const uint8_t* ymask,
+                                 float* post_mean, float* post_cov, float* a_mean, float* a_cov, float* df_p,
+                                 float* inv_scale_p, float* df_q, float* inv_scale_q, double* free_energy, int32_t* status,
+                                 unsigned flags);
 /* Hierarchical Gaussian Filter, streaming, `iters` VMP iterations per datum
  * [ref: test/models/statespace/hgf_tests.jl:10-69; loop src/inference/streaming.jl:349-407].
  * y[T][batch]; init = (m_z, v_z, m_x, v_x); out[T][4][batch] = (m_x, v_x, m_z, v_z).            */

@@ -18,7 +18,8 @@ def __getattr__(name):   # lazy: these import torch
         return getattr(context, name)
     if name in ("infer", "InferenceResult", "linear_gaussian_ssm_smoothing", "linear_gaussian_ssm_filtering",
                 "hgf", "univariate_lgssm_gamma_precision", "kalman_gamma_streaming", "latent_autoregressive",
-                "linear_gaussian_ssm_wishart_precision", "linear_gaussian_ssm_wishart_noise", "default_context",
+                "linear_gaussian_ssm_wishart_precision", "linear_gaussian_ssm_wishart_noise",
+                "linear_gaussian_ssm_continuous_transition", "default_context",
                 "KeepLast", "KeepEach"):
         from . import inference
         return getattr(inference, name)

@@ -85,6 +85,9 @@ SIGNATURES = {
                                           u8p, fp, fp, fp, fp, POINTER(c_double), i32p, c_uint]),
     "rxg_lgssm_vmp_noise_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, c_int, fp, fp, fp, fp, fp, fp, c_float, fp, fp, fp,
                                         c_float, fp, fp, fp, u8p, fp, fp, fp, fp, fp, fp, POINTER(c_double), i32p, c_uint]),
+    "rxg_lgssm_vmp_transition_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, c_int, fp, fp, fp, fp, fp, fp, fp, fp, fp, c_float,
+                                             fp, fp, fp, c_float, fp, fp, fp, u8p, fp, fp, fp, fp, fp, fp, fp, fp, POINTER(c_double),
+                                             i32p, c_uint]),
     "rxg_hgf_filter_f32": (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_float, c_float, c_float, fp, fp, fp, c_uint]),
     "rxg_hgf_filter_fe_f32": (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_float, c_float, c_float, fp, fp, fp, fp, fp, c_uint]),
     "rxg_lgssm_filter_chunk_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, c_uint]),

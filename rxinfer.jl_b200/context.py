@@ -409,13 +409,30 @@ class Context:
         after every iteration (None for a known noise), free_energy[iterations, batch] fp64 or None, status[batch])."""
         if y.dim() != 3:
             raise ValueError(f"y: expected [T, m, batch], got shape {tuple(y.shape)}")
-        T, m, batch = y.shape
         d = np.asarray(A).shape[-1]
+        T, m, batch, iterations, keep, nus = self._vmp_noise_setup(
+            y, d, dict(A=A), dict(A=(d, d)), B, m0, S0, P, Q, p_prior, p_init, q_prior, q_init, u, iterations, False)
+        mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
+        mean, cov, out, fe, fe_p, st = self._vmp_noise_outputs(T, d, m, batch, iterations, nus, want_free_energy)
+        hp = lambda k: keep[k][1] if k in keep else L.as_fp(0)
+        self._check(self.lib.rxg_lgssm_vmp_noise_f32(
+            self.h, d, m, T, batch, iterations, hp("A"), hp("B"), hp("m0"), hp("S0"), hp("u"),
+            hp("P"), nus.get("p", 0.0), hp("inv_scale_p0"), hp("init_E_Wp"),
+            hp("Q"), nus.get("q", 0.0), hp("inv_scale_q0"), hp("init_E_Wq"),
+            _fp(y), mask_p, _fp(mean), _fp(cov), _fp(out["df_p"]), _fp(out["inv_scale_p"]), _fp(out["df_q"]),
+            _fp(out["inv_scale_q"]), fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
+        return dict(mean=mean, cov=cov, **out, free_energy=fe, status=st)
+
+    def _vmp_noise_setup(self, y, d, mats, shapes, B, m0, S0, P, Q, p_prior, p_init, q_prior, q_init, u, iterations,
+                         both_known_ok):
+        """Shared argument handling of the noise-learning VMP entries: each noise known or (prior, init); host model
+        arrays converted to row-major fp32 and shape-checked (kept alive in ``keep``); y validated."""
+        T, m, batch = y.shape
         iterations = int(iterations)
         if iterations < 1:
             raise ValueError(f"iterations must be >= 1, got {iterations}")
-        shapes = dict(A=(d, d), B=(m, d), m0=(d,), S0=(d, d))
-        mats = dict(A=A, B=B, m0=m0, S0=S0)
+        shapes = dict(shapes, B=(m, d), m0=(d,), S0=(d, d))
+        mats = dict(mats, B=B, m0=m0, S0=S0)
         nus = {}
         for name, k, known, prior, init in (("p", d, P, p_prior, p_init), ("q", m, Q, q_prior, q_init)):
             if known is not None:
@@ -429,7 +446,7 @@ class Context:
             nus[name] = float(prior[0])
             shapes[f"inv_scale_{name}0"], mats[f"inv_scale_{name}0"] = (k, k), prior[1]
             shapes[f"init_E_W{name}"], mats[f"init_E_W{name}"] = (k, k), init
-        if not nus:
+        if not nus and not both_known_ok:
             raise ValueError("P and Q are both known: that is the plain smoother (Context.lgssm)")
         if u is not None:
             shapes["u"], mats["u"] = (d,), u
@@ -440,7 +457,9 @@ class Context:
                 raise ValueError(f"{k}: expected shape {shapes[k]}, got {a.shape}")
             keep[k] = (a, p)
         self._io(y, "y", True)
-        mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
+        return T, m, batch, iterations, keep, nus
+
+    def _vmp_noise_outputs(self, T, d, m, batch, iterations, nus, want_free_energy):
         mean, cov = self.empty(T, d, batch), self.empty(T, d, d, batch)
         out = {}
         for name, k in (("p", d), ("q", m)):
@@ -450,14 +469,43 @@ class Context:
         fe = self.empty(iterations, batch, dtype=torch.float64) if want_free_energy else None
         st = self.empty(batch, dtype=torch.int32)
         fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
+        return mean, cov, out, fe, fe_p, st
+
+    def lgssm_vmp_transition(self, y, B, m0, S0, *, a_prior, a_init, P=None, Q=None, p_prior=None, p_init=None,
+                             q_prior=None, q_init=None, u=None, mask=None, transition_first=False, iterations=10,
+                             want_free_energy=False, asynchronous=False):
+        """VMP around the smoother that also learns the transition matrix A per chain (``rxg_lgssm_vmp_transition_f32``,
+        RxInfer's ContinuousTransition with a linear reshape): a = vec(A) ~ N(ma0, Va0), x[t] ~ N(A x[t-1] + u, inv(w_p)),
+        y[t] ~ N(B x[t], inv(w_q)), q(x) q(a) q(w_p) q(w_q).  ``a_prior = (ma0, Va0)`` and ``a_init = (E[a], cov(a))`` of
+        the initial q(a) (required: an uninformed q(a) makes the first sweep meaningless), in the ABI's row-major order
+        a[i * d + j] = A[i, j]: means [d, d] (or [d * d]), covariances [d * d, d * d].  Each noise as for
+        :meth:`lgssm_vmp_noise`; both may be known.  d <= 4.  Returns the dict of :meth:`lgssm_vmp_noise` plus
+        a_mean[iterations, d, d, batch] and a_cov[iterations, d * d, d * d, batch] after every iteration."""
+        if y.dim() != 3:
+            raise ValueError(f"y: expected [T, m, batch], got shape {tuple(y.shape)}")
+        d = np.asarray(S0).shape[-1]
+        n = d * d
+        if not (isinstance(a_prior, (tuple, list)) and len(a_prior) == 2):
+            raise ValueError("a_prior: expected (mean [d, d], covariance [d * d, d * d])")
+        if not (isinstance(a_init, (tuple, list)) and len(a_init) == 2):
+            raise ValueError("a_init: expected (E[a] [d, d], cov(a) [d * d, d * d]) of the initial q(a)")
+        mats = dict(a_mean0=np.asarray(a_prior[0]).reshape(-1), a_cov0=a_prior[1],
+                    a_init_mean=np.asarray(a_init[0]).reshape(-1), a_init_cov=a_init[1])
+        shapes = dict(a_mean0=(n,), a_cov0=(n, n), a_init_mean=(n,), a_init_cov=(n, n))
+        T, m, batch, iterations, keep, nus = self._vmp_noise_setup(
+            y, d, mats, shapes, B, m0, S0, P, Q, p_prior, p_init, q_prior, q_init, u, iterations, True)
+        mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
+        mean, cov, out, fe, fe_p, st = self._vmp_noise_outputs(T, d, m, batch, iterations, nus, want_free_energy)
+        a_mean, a_cov = self.empty(iterations, d, d, batch), self.empty(iterations, n, n, batch)
         hp = lambda k: keep[k][1] if k in keep else L.as_fp(0)
-        self._check(self.lib.rxg_lgssm_vmp_noise_f32(
-            self.h, d, m, T, batch, iterations, hp("A"), hp("B"), hp("m0"), hp("S0"), hp("u"),
+        self._check(self.lib.rxg_lgssm_vmp_transition_f32(
+            self.h, d, m, T, batch, iterations, hp("a_mean0"), hp("a_cov0"), hp("a_init_mean"), hp("a_init_cov"),
+            hp("B"), hp("m0"), hp("S0"), hp("u"),
             hp("P"), nus.get("p", 0.0), hp("inv_scale_p0"), hp("init_E_Wp"),
             hp("Q"), nus.get("q", 0.0), hp("inv_scale_q0"), hp("init_E_Wq"),
-            _fp(y), mask_p, _fp(mean), _fp(cov), _fp(out["df_p"]), _fp(out["inv_scale_p"]), _fp(out["df_q"]),
-            _fp(out["inv_scale_q"]), fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
-        return dict(mean=mean, cov=cov, **out, free_energy=fe, status=st)
+            _fp(y), mask_p, _fp(mean), _fp(cov), _fp(a_mean), _fp(a_cov), _fp(out["df_p"]), _fp(out["inv_scale_p"]),
+            _fp(out["df_q"]), _fp(out["inv_scale_q"]), fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
+        return dict(mean=mean, cov=cov, a_mean=a_mean, a_cov=a_cov, **out, free_energy=fe, status=st)
 
     # ------------------------------------------------------------------ per-rule kernels
     def _mat(self, M):

@@ -53,6 +53,29 @@ __device__ __forceinline__ void chain_update(const Mat<float, M, D>& B, const Ma
     }
 }
 
+// absorb the factor exp(-1/2 x' L L' x) into (mu, S), covariance form (nothing singular is inverted):
+//   Sm = I + L' S L = Ls Ls',  Z = S L Ls^-T,  S -= Z Z',  mu -= Z Ls^-1 L' mu
+// want_nle: acc_nle += 1/2 (|Ls^-1 L' mu|^2 + log det Sm), the factor's negative log-normaliser under N(mu, S).
+template <int D>
+__device__ __forceinline__ void chain_tilt(const Mat<float, D, D>& L, bool want_nle, Vec<float, D>& mu,
+                                           Mat<float, D, D>& S, bool& bad, double& acc_nle) {
+    Mat<float, D, D> SL = mul(S, L);
+    Mat<float, D, D> Sm = sym_mul_nt_add(transpose(SL), transpose(L), identity<float, D>());
+    Chol<float, D> ch = want_nle ? cholesky<float, D, true>(Sm, bad) : cholesky<float, D, false>(Sm, bad);
+    Mat<float, D, D> Z = solve_right_Lt(SL, ch.L);
+    Vec<float, D> z = solve_L(ch.L, mulv_t(L, mu));
+    Vec<float, D> dm = mulv(Z, z);
+#pragma unroll
+    for (int i = 0; i < D; ++i) mu(i) -= dm(i);
+    S = sym_downdate(S, Z);
+    if (want_nle) {
+        float q = 0.f;
+#pragma unroll
+        for (int k = 0; k < D; ++k) q = __fmaf_rn(z(k), z(k), q);
+        acc_nle += (double)(0.5f * q - ch.neg_half_logdet);
+    }
+}
+
 // pair hook of an RTS step without lag-one statistics
 struct NoPair {
     template <int D>

@@ -128,6 +128,35 @@ class linear_gaussian_ssm_wishart_noise:
     prior_on_previous_state: bool = False
 
 
+@dataclass
+class linear_gaussian_ssm_continuous_transition:
+    """LGSSM that learns its transition matrix per series (RxInfer's ``ContinuousTransition`` with
+    ``CTMeta(a -> reshape(a, d, d))``): ``a ~ MvNormal(mean = ma0, covariance = Va0); x[1] ~ x0;
+    x[t] ~ ContinuousTransition(x[t-1], a, w_p) (+ u); y[t] ~ N(B x[t], precision = w_q)``, run with
+    ``constraints = q(x, a, w_p, w_q) = q(x)q(a)q(w_p)q(w_q)``, ``initialization = q(a) = a_init, ...`` and ``iterations``.
+    ``a_prior`` / ``a_init`` are ``(mean, covariance)`` of vec(A) in Julia's column-major order (vec(A)[j d + i] =
+    A[i, j]); ``a_init`` is required.  Each noise is known (``P`` / ``Q``, a covariance) or learned (``*_prior`` and
+    ``*_init`` as ``Wishart(df, scale)``); both may be known.  ``x0 = (mean, cov)``."""
+    B: np.ndarray
+    x0: tuple
+    a_prior: tuple
+    a_init: tuple = None
+    P: np.ndarray = None
+    Q: np.ndarray = None
+    p_prior: Wishart = None
+    p_init: Wishart = None
+    q_prior: Wishart = None
+    q_init: Wishart = None
+    u: object = None
+    prior_on_previous_state: bool = False
+
+
+def vec_order(d):
+    """perm with row_major = col_major[perm] (and col_major = row_major[perm]: a transpose is an involution) for vec(A)
+    of a d x d matrix: Julia's vec is column-major, the C ABI's a[i * d + j] = A[i, j] row-major."""
+    return np.array([(r % d) * d + r // d for r in range(d * d)])
+
+
 class KeepLast:
     """``predictvars`` / ``returnvars`` marker: keep the result of the last iteration (the reference's ``KeepLast()``)."""
 
@@ -238,7 +267,8 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             raise NotImplementedError(f"options {sorted(bad)} are outside the batched hot path")
     if data is not None and datastream is not None:
         raise ValueError("`data` and `datastream` are mutually exclusive")    # reference: inference.jl argument check
-    if isinstance(model, (linear_gaussian_ssm_wishart_precision, linear_gaussian_ssm_wishart_noise)):
+    if isinstance(model, (linear_gaussian_ssm_wishart_precision, linear_gaussian_ssm_wishart_noise,
+                          linear_gaussian_ssm_continuous_transition)):
         if predictvars is not None:
             raise NotImplementedError("predictvars: predictions of the Wishart-precision LGSSM are outside the batched hot path")
         if data is not None and "u" in data:
@@ -378,6 +408,44 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
                                      f"{int(bad.sum())} of {bad.numel()} chains flagged {codes}")
             # x = KeepLast(), w_p / w_q = KeepEach() (leading iteration axis) for the learned precisions
             post = {"x": MvNormalMeanCovariance(r["mean"], r["cov"])}
+            for name in ("p", "q"):
+                if r[f"df_{name}"] is not None:
+                    post[f"w_{name}"] = WishartFast(r[f"df_{name}"], r[f"inv_scale_{name}"])
+            return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
+        if isinstance(model, linear_gaussian_ssm_continuous_transition):
+            kw = {}
+            for name in ("p", "q"):
+                known, prior, init = getattr(model, name.upper()), getattr(model, f"{name}_prior"), getattr(model, f"{name}_init")
+                if known is not None and (prior is not None or init is not None):
+                    raise ValueError(f"{name.upper()} is known: pass either {name.upper()} or {name}_prior / {name}_init")
+                if known is not None:
+                    kw[name.upper()] = known
+                elif prior is not None and init is not None:
+                    kw[f"{name}_prior"], kw[f"{name}_init"] = (prior.df, prior.inv_scale()), init.mean()
+                else:
+                    kw[f"{name}_prior"], kw[f"{name}_init"] = prior, init    # Context names what is missing
+            if model.a_init is None:
+                raise ValueError("a_init: q(a) needs an initial (mean, covariance) (an uninformed q(a) makes the first "
+                                 "sweep meaningless)")
+            d = np.asarray(model.x0[1]).shape[-1]
+            pm = vec_order(d)
+            rowmajor = lambda mc: (np.asarray(mc[0], np.float64).reshape(-1)[pm],
+                                   np.asarray(mc[1], np.float64)[np.ix_(pm, pm)])
+            r = ctx.lgssm_vmp_transition(y, model.B, model.x0[0], model.x0[1], a_prior=rowmajor(model.a_prior),
+                                         a_init=rowmajor(model.a_init), **kw, u=model.u, mask=mask,
+                                         transition_first=model.prior_on_previous_state, iterations=iterations or 1,
+                                         want_free_energy=bool(free_energy))
+            bad = r["status"] != 0
+            if bool(bad.any()):
+                codes = sorted({L.STATUS_NAMES.get(int(c), str(int(c))) for c in r["status"][bad].unique().tolist()})
+                raise L.RxGaussError(L.RXG_ERR_NOT_SPD if "NOT_SPD" in codes else int(r["status"][bad][0]),
+                                     f"{int(bad.sum())} of {bad.numel()} chains flagged {codes}")
+            # x = KeepLast(); a, w_p / w_q = KeepEach() (leading iteration axis); a over vec(A) in column-major order
+            pt = torch.as_tensor(pm, device=r["a_mean"].device)
+            its_, nb = r["a_mean"].shape[0], r["a_mean"].shape[-1]
+            a_mu = r["a_mean"].reshape(its_, d * d, nb)[:, pt]
+            a_S = r["a_cov"][:, pt][:, :, pt]
+            post = {"x": MvNormalMeanCovariance(r["mean"], r["cov"]), "a": MvNormalMeanCovariance(a_mu, a_S)}
             for name in ("p", "q"):
                 if r[f"df_{name}"] is not None:
                     post[f"w_{name}"] = WishartFast(r[f"df_{name}"], r[f"inv_scale_{name}"])

@@ -218,6 +218,14 @@ lgssm_vmp_noise(ctx, d, m, T, batch, its, A, B, m0, S0, u, P, nup, iSp0, EWp0, Q
          F32P, F32P, Ptr{UInt8}, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Float64}, Ptr{Int32}, Cuint),
         ctx.handle, d, m, T, batch, its, A, B, m0, S0, u, P, nup, iSp0, EWp0, Q, nuq, iSq0, EWq0, y, mask, mean, cov,
         dfp, iSp, dfq, iSq, fe, st, fl))
+lgssm_vmp_transition(ctx, d, m, T, batch, its, am0, aV0, ami, aVi, B, m0, S0, u, P, nup, iSp0, EWp0, Q, nuq, iSq0, EWq0, y,
+                     mask, mean, cov, am, aV, dfp, iSp, dfq, iSq, fe, st, fl) =
+    check(ctx, ccall((:rxg_lgssm_vmp_transition_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Cfloat, F32P, F32P,
+         F32P, Cfloat, F32P, F32P, F32P, Ptr{UInt8}, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Float64}, Ptr{Int32},
+         Cuint),
+        ctx.handle, d, m, T, batch, its, am0, aV0, ami, aVi, B, m0, S0, u, P, nup, iSp0, EWp0, Q, nuq, iSq0, EWq0, y, mask,
+        mean, cov, am, aV, dfp, iSp, dfq, iSq, fe, st, fl))
 mv_iid_wishart_vmp(ctx, d, N, batch, its, mu0, L0, nu0, iS0, EP0, y, mm, mc, df, iS, st, fl) =
     check(ctx, ccall((:rxg_mv_iid_wishart_vmp_f32, LIB), Cint,
         (Ptr{Cvoid}, Cint, Cint, Int64, Cint, F32P, F32P, Cfloat, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Int32}, Cuint),
@@ -750,6 +758,57 @@ function lgssm_wishart_noise(ctx::Context, y::Array{Float32, 3}; A::Matrix, B::M
     fe = reshape(reinterpret(Float64, vec(download(dfe))), batch, iterations)
     dl(a) = a === nothing ? nothing : download(a)
     return download(mean), download(cov), dl(dfp), dl(iSp), dl(dfq), dl(iSq), fe, reinterpret(Int32, download(st))
+end
+
+"""VMP around the multivariate smoother that also learns the transition matrix per series (`ContinuousTransition`
+with `CTMeta(a -> reshape(a, d, d))`, `rxg_lgssm_vmp_transition_f32`; `constraints = q(x, a, w_p, w_q) =
+q(x)q(a)q(w_p)q(w_q)`); host data `y[batch, m, T]`.  `a_prior = (mean, covariance)` of `a = vec(A)` (column-major, as
+`vec` orders it) and `a_init` = (mean, covariance) of the initial q(a), required.  Each noise as for
+`lgssm_wishart_noise`; both may be known.  Returns q(x) of the last iteration, q(a) after every iteration (mean
+`[batch, d*d, iterations]`, covariance `[batch, d*d, d*d, iterations]`, in `vec` order), q(w_p) and q(w_q) as
+`lgssm_wishart_noise` returns them, the Bethe free energy `[batch, iterations]` (Float64) and the per-series status."""
+function lgssm_continuous_transition(ctx::Context, y::Array{Float32, 3}; B::Matrix, a_prior, a_init = nothing,
+                                     x0 = nothing, u = nothing, P = nothing, p_prior = nothing, p_init = nothing,
+                                     Q = nothing, q_prior = nothing, q_init = nothing, iterations = 10,
+                                     transition_first = false)
+    batch, m, T = size(y)
+    d = size(B, 2)
+    n = d * d
+    a_init === nothing && throw(ArgumentError("a_init: q(a) needs an initial (mean, covariance) (no default q(a))"))
+    for (name, known, prior, init) in (("P", P, p_prior, p_init), ("Q", Q, q_prior, q_init))
+        known === nothing || (prior === nothing && init === nothing) ||
+            throw(ArgumentError("$name is known: pass either $name or its prior / init"))
+        known !== nothing || (prior !== nothing && init !== nothing) ||
+            throw(ArgumentError("$name is learned: pass its prior = (df, inverse scale) and init = E[w] (no default q(w))"))
+    end
+    p = vec(permutedims(reshape(1:n, d, d)))                  # vec (column-major) index of row-major a[i*d + j]
+    m0, S0 = x0 === nothing ? (zeros(Float32, d), Matrix{Float32}(100I, d, d)) : (Float32.(x0[1]), Float32.(x0[2]))
+    rowmajor(M) = M === nothing ? nothing : Matrix{Float32}(permutedims(M))       # row-major host matrices for the C side
+    am0, ami = Float32.(vec(a_prior[1])[p]), Float32.(vec(a_init[1])[p])
+    aV0, aVi = rowmajor(a_prior[2][p, p]), rowmajor(a_init[2][p, p])
+    Bt, S0t, Pt, Qt = rowmajor(B), rowmajor(S0), rowmajor(P), rowmajor(Q)
+    nup, iSp0, EWp0 = P === nothing ? (Float32(p_prior[1]), rowmajor(p_prior[2]), rowmajor(p_init)) : (0f0, nothing, nothing)
+    nuq, iSq0, EWq0 = Q === nothing ? (Float32(q_prior[1]), rowmajor(q_prior[2]), rowmajor(q_init)) : (0f0, nothing, nothing)
+    uv = u === nothing ? nothing : Float32.(u)
+    ptr(M) = M === nothing ? NULLF : pointer(M)
+    dy = upload(ctx, y)
+    mean, cov = DeviceArray(ctx, batch, d, T), DeviceArray(ctx, batch, d, d, T)
+    am, aV = DeviceArray(ctx, batch, n, iterations), DeviceArray(ctx, batch, n, n, iterations)
+    dfp, iSp = P === nothing ? (DeviceArray(ctx, batch, iterations), DeviceArray(ctx, batch, d, d, iterations)) : (nothing, nothing)
+    dfq, iSq = Q === nothing ? (DeviceArray(ctx, batch, iterations), DeviceArray(ctx, batch, m, m, iterations)) : (nothing, nothing)
+    dptr(a) = a === nothing ? NULLF : a.ptr
+    dfe = DeviceArray(ctx, 2 * batch * iterations)                  # fp64 output: two Float32 slots per value
+    st = DeviceArray(ctx, batch)
+    fl = RXG_PTR_DEVICE | (transition_first ? RXG_TRANSITION_FIRST : UInt32(0))
+    GC.@preserve am0 aV0 ami aVi Bt m0 S0t uv Pt iSp0 EWp0 Qt iSq0 EWq0 Lib.lgssm_vmp_transition(ctx, d, m, T, batch,
+        iterations, pointer(am0), pointer(aV0), pointer(ami), pointer(aVi), pointer(Bt), pointer(m0), pointer(S0t), ptr(uv),
+        ptr(Pt), nup, ptr(iSp0), ptr(EWp0), ptr(Qt), nuq, ptr(iSq0), ptr(EWq0), dy.ptr, Ptr{UInt8}(C_NULL), mean.ptr,
+        cov.ptr, am.ptr, aV.ptr, dptr(dfp), dptr(iSp), dptr(dfq), dptr(iSq), Ptr{Float64}(dfe.ptr), Ptr{Int32}(st.ptr), fl)
+    fe = reshape(reinterpret(Float64, vec(download(dfe))), batch, iterations)
+    dl(a) = a === nothing ? nothing : download(a)
+    a_mean, a_cov = download(am)[:, p, :], download(aV)[:, p, p, :]     # back to vec order
+    return download(mean), download(cov), a_mean, a_cov, dl(dfp), dl(iSp), dl(dfq), dl(iSq), fe,
+           reinterpret(Int32, download(st))
 end
 
 """Fused structured VMP of the latent autoregressive model (lar_tests.jl:52-122); `y[batch, T]`.  Returns the reference's
