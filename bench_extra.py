@@ -8,6 +8,7 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
   python bench_extra.py --which vmp_wishart  (opt-in: Wishart-precision VMP around the smoother vs the composed path)
   python bench_extra.py --which vmp_noise    (opt-in: learned process precision, alone and with the observation precision)
   python bench_extra.py --which vmp_transition (opt-in: learned transition matrix, alone and with the noise precisions)
+  python bench_extra.py --which gmm          (opt-in: Gaussian-mixture VMP, d = 2 / K = 3 and d = 4 / K = 8)
 """
 from __future__ import annotations
 
@@ -339,6 +340,43 @@ def bench_vmp_transition(ctx, peak):
         torch.cuda.empty_cache()
 
 
+def bench_gmm(ctx, peak):
+    """Gaussian-mixture VMP (rxg_gmm_vmp_f32), N = 500 points per data set, 25 iterations, 65 536 data sets, free energy
+    on; time from CUDA events around the call (host validation and the constant upload included, both O(K d^3)).  Per
+    point, component and iteration the data pass does ~(d + 2 tri(d) + 4) fp32 flops, ~(3 + 2 d + 2 tri(d)) fp64 flops
+    and reads the component's constants (4 (d + tri(d) + 1) B) and updates its fp64 accumulators (16 (1 + d + tri(d)) B)
+    in shared memory; the bound is the largest of the HBM, fp32, fp64 and shared-memory times."""
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(17)
+    N, nb, its = 500, 65536, 25
+    sm = torch.cuda.get_device_properties(0).multi_processor_count
+    smem_tbs = sm * 128 * 1.98e9 / 1e12                          # 128 B / clock / SM at the 1.98 GHz boost clock
+    for d, K in ((2, 3), (4, 8)):
+        tri = d * (d + 1) // 2
+        centres = torch.randn(K, d, device="cuda", generator=g) * 10.0
+        lab = torch.randint(0, K, (N, nb), device="cuda", generator=g)
+        y = (centres[lab].permute(0, 2, 1) + torch.randn(N, d, nb, device="cuda", generator=g)).contiguous()
+        eye = np.tile(np.eye(d), (K, 1, 1))
+        args = (np.ones(K), np.zeros((K, d)), 1e4 * eye, np.full(K, d + 1.0), eye, np.ones(K),
+                centres.cpu().numpy() + 1.0, 10.0 * eye, np.full(K, d + 1.0), eye)
+        runs = [timed(lambda: ctx.gmm_vmp(y, *args, iterations=its), warm=2, reps=3) for _ in range(3)]
+        ms = float(np.median(runs))
+        n = N * nb * its
+        by = 4 * d
+        f32_fl, f64_fl = K * (d + 2 * tri + 4), K * (3 + 2 * d + 2 * tri)
+        sh = K * (4 * (d + tri + 1) + 16 * (1 + d + tri))
+        t = {"hbm": by * n / (peak * 1e9), "fp32": f32_fl * n / 67e12, "fp64": f64_fl * n / 34e12, "shared": sh * n / (smem_tbs * 1e12)}
+        bound = max(t, key=t.get)
+        print(json.dumps({"what": "Gaussian-mixture VMP (gmm_vmp_kernel), free energy on", "d": d, "K": K, "N": N, "batch": nb,
+                          "iterations": its, "ms": ms, "ms_runs": runs, "ms_per_iteration": ms / its,
+                          "bytes_per_chain": N * d * 4 * its, "achieved_GBs": by * n / ms / 1e6,
+                          "bound": bound, "bound_ms": {k: v * 1e3 for k, v in t.items()}, "frac_of_bound": t[bound] * 1e3 / ms,
+                          "peak_hbm_gbs": peak, "peak_fp32_tflops": 67, "peak_fp64_tflops": 34, "shared_tbs": smem_tbs,
+                          "gpu": gname, "power_limit": plim}), flush=True)
+        del y
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -356,6 +394,8 @@ def main():
         bench_vmp_noise(ctx, peak)
     if "vmp_transition" in which:
         bench_vmp_transition(ctx, peak)
+    if "gmm" in which:
+        bench_gmm(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

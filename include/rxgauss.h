@@ -251,6 +251,28 @@ int rxg_ar_vmp_f32(rxg_ctx*, int order, int N, int64_t batch, int iterations, fl
 int rxg_lar_vmp_f32(rxg_ctx*, int order, int T, int64_t batch, int iterations, const float* params, const float* y,
                     float* x_mean, float* x_cov, float* theta_mean, float* theta_cov, float* gamma_shape,
                     float* gamma_rate, double* free_energy, int32_t* status, unsigned flags);
+/* Fused mean-field VMP of the Gaussian mixture model, `batch` independent data sets, all iterations in one launch:
+ *   s ~ Dirichlet(alpha0), m[k] ~ MvNormal(mu0[k], V0[k]), W[k] ~ Wishart(nu0[k], S0[k]) (precision; S0 the scale),
+ *   z[i] ~ Categorical(s), y[i] ~ NormalMixture(z[i], m, W), q(s) prod q(m[k]) prod q(W[k]) prod q(z[i]), initialised to
+ *   Dirichlet(alpha_init), MvNormal(m_init[k], Vm_init[k]), Wishart(nu_init[k], S_init[k])
+ *   [ref: test/models/mixtures/gmm_multivariate_tests.jl:4-24, :37-64; gmm_univariate_tests.jl:6-26 is the d = 1, K = 2
+ *   case with Beta(a, b) = Dirichlet([a, b]) and Gamma(shape, rate) = Wishart(2 shape, 1 / (2 rate))].  Priors and initial
+ *   marginals are HOST arrays shared by every chain: alpha0[K], mu0[K][d], V0[K][d][d], nu0[K], S0[K][d][d], likewise the
+ *   *_init.  y[N][d][batch].  Outputs of the last iteration: alpha[K][batch], m_mean[K][d][batch], m_cov[K][d][d][batch],
+ *   w_df[K][batch], w_inv_scale[K][d][d][batch] (q(W[k]) = Wishart(w_df, inv(w_inv_scale))).  Optional (NULL = not
+ *   wanted): free_energy[iterations][batch] (fp64, Bethe free energy after every iteration), z_prob[N][K][batch] (q(z) of
+ *   the last iteration), the KeepEach histories hist_alpha[iterations][K][batch], hist_m_mean[iterations][K][d][batch],
+ *   hist_m_cov[iterations][K][d][d][batch], hist_w_df[iterations][K][batch], hist_w_inv_scale[iterations][K][d][d][batch],
+ *   status[batch] (RXG_ERR_NOT_SPD for a chain whose update met a non-SPD matrix).  Per iteration: q(z), then q(m[k]) with
+ *   the previous E[W[k]], q(W[k]) with the new q(m[k]), q(s).  1 <= d <= 4 and 2 <= K <= 8, else RXG_ERR_UNSUPPORTED;
+ *   N, batch, iterations >= 1, alpha0 and alpha_init > 0, nu0 and nu_init > d - 1, V0, S0, Vm_init, S_init symmetric
+ *   positive definite, else RXG_ERR_BAD_ARG.  Device pointers (RXG_ERR_UNSUPPORTED otherwise).                        */
+int rxg_gmm_vmp_f32(rxg_ctx*, int d, int K, int N, int64_t batch, int iterations, const float* alpha0, const float* mu0,
+                    const float* V0, const float* nu0, const float* S0, const float* alpha_init, const float* m_init,
+                    const float* Vm_init, const float* nu_init, const float* S_init, const float* y, float* alpha,
+                    float* m_mean, float* m_cov, float* w_df, float* w_inv_scale, double* free_energy, float* z_prob,
+                    float* hist_alpha, float* hist_m_mean, float* hist_m_cov, float* hist_w_df, float* hist_w_inv_scale,
+                    int32_t* status, unsigned flags);
 /* prod(GammaShapeRate, GammaShapeRate) = (a1 + a2 - 1, b1 + b2)                                 */
 int rxg_prod_gamma_f32(rxg_ctx*, int64_t n, const float* a1, const float* b1, const float* a2,
                        const float* b2, float* a, float* b, unsigned flags);

@@ -8,8 +8,8 @@ loudly if it is missing or no GPU is present -- there is no CPU fallback.
 """
 from . import _lib
 from ._lib import RxGaussError
-from .distributions import (GammaShapeRate, MvNormalMeanCovariance, MvNormalWeightedMeanPrecision,
-                            NormalMeanVariance, PointMass, Wishart, WishartFast, vague)
+from .distributions import (Beta, Categorical, Dirichlet, GammaShapeRate, MvNormalMeanCovariance,
+                            MvNormalWeightedMeanPrecision, NormalMeanVariance, PointMass, Wishart, WishartFast, vague)
 
 
 def __getattr__(name):   # lazy: these import torch
@@ -19,7 +19,8 @@ def __getattr__(name):   # lazy: these import torch
     if name in ("infer", "InferenceResult", "linear_gaussian_ssm_smoothing", "linear_gaussian_ssm_filtering",
                 "hgf", "univariate_lgssm_gamma_precision", "kalman_gamma_streaming", "latent_autoregressive",
                 "linear_gaussian_ssm_wishart_precision", "linear_gaussian_ssm_wishart_noise",
-                "linear_gaussian_ssm_continuous_transition", "default_context",
+                "linear_gaussian_ssm_continuous_transition", "gaussian_mixture", "MeanField", "BetheFactorization",
+                "default_context",
                 "KeepLast", "KeepEach"):
         from . import inference
         return getattr(inference, name)

@@ -698,6 +698,48 @@ class Context:
                                              ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
         return dict(x_mean=xm, x_cov=xc, theta_mean=tm, theta_cov=tc, gamma_shape=gs, gamma_rate=gr, free_energy=fe, status=st)
 
+    def gmm_vmp(self, y, alpha0, mu0, V0, nu0, S0, alpha_init, m_init, Vm_init, nu_init, S_init, iterations=10,
+                want_free_energy=True, want_z=False, keep_each=False):
+        """Fused mean-field VMP of the Gaussian mixture model (``rxg_gmm_vmp_f32``); y[N, d, batch] on the device.
+        Priors and initial marginals are host arrays shared by every chain: alpha0[K], mu0[K, d], V0[K, d, d] (covariance),
+        nu0[K], S0[K, d, d] (Wishart scale); the same for the initial q(s), q(m), q(W).  Returns the last iteration's
+        ``alpha[K, batch]``, ``m_mean[K, d, batch]``, ``m_cov[K, d, d, batch]``, ``w_df[K, batch]``,
+        ``w_inv_scale[K, d, d, batch]``, ``free_energy[iterations, batch]`` (fp64), ``z_prob[N, K, batch]`` (with
+        ``want_z``), ``status[batch]`` and, with ``keep_each``, ``hist_*`` with a leading iteration axis."""
+        self._dev(y)
+        if y.dim() != 3:
+            raise ValueError("gmm_vmp: y must be [N, d, batch]")
+        N, d, batch = y.shape
+        K = int(np.asarray(alpha0).shape[0])
+        shapes = dict(alpha0=(K,), mu0=(K, d), V0=(K, d, d), nu0=(K,), S0=(K, d, d), alpha_init=(K,), m_init=(K, d),
+                      Vm_init=(K, d, d), nu_init=(K,), S_init=(K, d, d))
+        vals = dict(alpha0=alpha0, mu0=mu0, V0=V0, nu0=nu0, S0=S0, alpha_init=alpha_init, m_init=m_init, Vm_init=Vm_init,
+                    nu_init=nu_init, S_init=S_init)
+        keep = {}
+        for k, shp in shapes.items():
+            a = np.asarray(vals[k], dtype=np.float64)
+            if a.shape != shp:
+                raise ValueError(f"gmm_vmp: {k} must have shape {shp} (K = {K}, d = {d}), got {a.shape}")
+            keep[k] = _model32(a)
+        its = int(iterations)
+        al, mm, mc = self.empty(K, batch), self.empty(K, d, batch), self.empty(K, d, d, batch)
+        df, iS = self.empty(K, batch), self.empty(K, d, d, batch)
+        fe = self.empty(its, batch, dtype=torch.float64) if want_free_energy else None
+        z = self.empty(N, K, batch) if want_z else None
+        h = dict(hist_alpha=self.empty(its, K, batch), hist_m_mean=self.empty(its, K, d, batch),
+                 hist_m_cov=self.empty(its, K, d, d, batch), hist_w_df=self.empty(its, K, batch),
+                 hist_w_inv_scale=self.empty(its, K, d, d, batch)) if keep_each else {}
+        st = self.empty(batch, dtype=torch.int32)
+        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
+        self._check(self.lib.rxg_gmm_vmp_f32(self.h, d, K, N, batch, its, *(keep[k][1] for k in shapes), _fp(y), _fp(al),
+                                             _fp(mm), _fp(mc), _fp(df), _fp(iS), fe_p, _fp(z),
+                                             *(_fp(h.get(k)) for k in ("hist_alpha", "hist_m_mean", "hist_m_cov",
+                                                                         "hist_w_df", "hist_w_inv_scale")),
+                                             ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+        out = dict(alpha=al, m_mean=mm, m_cov=mc, w_df=df, w_inv_scale=iS, free_energy=fe, z_prob=z, status=st)
+        out.update(h)
+        return out
+
     def prod_gamma(self, a1, b1, a2, b2):
         return self._six(self.lib.rxg_prod_gamma_f32, a1, b1, a2, b2)
 

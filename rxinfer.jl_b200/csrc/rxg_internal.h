@@ -68,6 +68,9 @@ int fail(rxg_ctx* ctx, int code, const char* fmt, ...);
 int check_cuda(rxg_ctx* ctx, cudaError_t e, const char* what);
 // returns device pointer of >= bytes (grow-only); nullptr on failure (error recorded)
 void* workspace(rxg_ctx* ctx, size_t bytes);
+// host: fp64 Cholesky of the symmetrised (A + A')/2 of an n x n matrix (n <= 16), then its inverse; false if it is not
+// symmetric positive definite (or not finite); log det on success
+bool host_spd_inv(const float* a, int n, double* inv, double* logdet);
 void* staging(rxg_ctx* ctx, size_t bytes);
 void* predict_scratch(rxg_ctx* ctx, size_t bytes);
 // device word that gain kernels OR a 1 into when a Cholesky pivot is non-positive (cleared by begin_bad_flag)

@@ -769,7 +769,10 @@ int dispatch_shape(rxg_ctx* ctx, int d, int m, const VmpWishHost& h, const VmpTr
 #undef RXG_VMP_CASE
 }
 
+}  // namespace
+
 // fp64 Cholesky of the symmetrised n x n matrix on the host (n <= 16), then its inverse: false if it is not SPD
+// (declared in rxg_internal.h: the Gaussian-mixture entry validates its host matrices with it too)
 bool host_spd_inv(const float* a, int n, double* inv, double* logdet) {
     double L[256] = {}, Li[256] = {};
     double ld = 0.0;
@@ -802,6 +805,8 @@ bool host_spd_inv(const float* a, int n, double* inv, double* logdet) {
     *logdet = ld;
     return true;
 }
+
+namespace {
 
 // the transition matrix of rxg_lgssm_vmp_transition_f32: its Gaussian prior, the initial q(a) and the outputs
 struct TransArg {

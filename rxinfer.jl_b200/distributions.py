@@ -98,9 +98,51 @@ class Wishart:
         return float(self.df) * np.asarray(self.scale, dtype=np.float64)
 
 
-def vague(kind, like: torch.Tensor):
+@dataclass
+class Dirichlet:
+    """``Dirichlet(alpha)``: ``alpha[K]`` (host, a prior or an initial marginal) or ``alpha[..., K, n]`` (posteriors)."""
+    alpha: object
+
+    def mean(self):
+        a = self.alpha
+        return a / a.sum(dim=-2, keepdim=True) if isinstance(a, torch.Tensor) else np.asarray(a, np.float64) / np.sum(a)
+
+
+@dataclass
+class Beta:
+    """``Beta(a, b)`` = ``Dirichlet([a, b])``: the weight of the first of two components."""
+    a: object
+    b: object
+
+    def mean(self):
+        return self.a / (self.a + self.b)
+
+
+@dataclass
+class Categorical:
+    """``Categorical(p)``: ``p[..., K, n]``."""
+    p: torch.Tensor
+
+    def probvec(self):
+        return self.p
+
+
+def vague(kind, like=None):
     """``vague(NormalMeanVariance)`` = N(0, 1e12); ``vague(GammaShapeRate)`` = Gamma(1, 1e-12)
-    (TinyHugeNumbers, upstream)."""
+    (TinyHugeNumbers, upstream); ``vague(Beta)`` = Beta(1, 1); ``vague(Dirichlet, K)`` = Dirichlet(ones(K)).
+    With a tensor ``like`` the parameters are tensors shaped like it, else host floats."""
+    if kind is Beta:
+        return Beta(1.0, 1.0)
+    if kind is Dirichlet:
+        if not isinstance(like, (int, np.integer)) or like < 1:
+            raise TypeError("vague(Dirichlet, K) needs the number of components K")
+        return Dirichlet(np.ones(int(like)))
+    if like is None:
+        if kind is NormalMeanVariance:
+            return NormalMeanVariance(0.0, 1e12)
+        if kind is GammaShapeRate:
+            return GammaShapeRate(1.0, 1e-12)
+        raise TypeError(kind)
     if kind is NormalMeanVariance:
         return NormalMeanVariance(torch.zeros_like(like), torch.full_like(like, 1e12))
     if kind is GammaShapeRate:

@@ -18,7 +18,8 @@ import torch
 
 from . import _lib as L
 from .context import Context
-from .distributions import GammaShapeRate, MvNormalMeanCovariance, NormalMeanVariance, Wishart, WishartFast
+from .distributions import (Beta, Categorical, Dirichlet, GammaShapeRate, MvNormalMeanCovariance, NormalMeanVariance, Wishart,
+                            WishartFast)
 
 
 # --------------------------------------------------------------------------- recognised models
@@ -151,6 +152,108 @@ class linear_gaussian_ssm_continuous_transition:
     prior_on_previous_state: bool = False
 
 
+@dataclass
+class gaussian_mixture:
+    """Gaussian mixture model (RxInfer test/models/mixtures/gmm_multivariate_tests.jl:4-24):
+    ``s ~ alpha0; m[k] ~ m_prior[k]; w[k] ~ w_prior[k]; z[i] ~ Categorical(s); y[i] ~ NormalMixture(switch = z[i], m = m,
+    p = w)``, run with ``constraints = MeanField()``, ``initialization = {"s": ..., "m": [...], "w": [...]}`` and
+    ``iterations``.  Multivariate spelling: ``Dirichlet``, ``MvNormalMeanCovariance``, ``Wishart(df, scale)``.  Univariate
+    spelling (gmm_univariate_tests.jl:6-26, K = 2): ``Beta(a, b)`` (= Dirichlet([a, b])), ``NormalMeanVariance``,
+    ``GammaShapeRate(shape, rate)`` (= Wishart(2 shape, 1 / (2 rate))), ``vague(Beta)`` / ``vague(GammaShapeRate)``."""
+    K: int
+    alpha0: object
+    m_prior: list
+    w_prior: list
+
+
+class MeanField:
+    """``constraints = MeanField()``: the naive mean-field factorisation q(s) prod q(m[k]) prod q(w[k]) prod q(z[i])."""
+
+    def __eq__(self, other):
+        return isinstance(other, MeanField)
+
+    def __hash__(self):
+        return hash(MeanField)
+
+
+class BetheFactorization:
+    """``BetheFactorization()``: the reference's default constraints (no factorisation of the local joints)."""
+
+    def __eq__(self, other):
+        return isinstance(other, BetheFactorization)
+
+    def __hash__(self):
+        return hash(BetheFactorization)
+
+
+def _weights(x, K, what):
+    if isinstance(x, Beta):
+        if K != 2:
+            raise ValueError(f"{what}: Beta weights describe K = 2 components, the model has K = {K}")
+        return np.array([float(x.a), float(x.b)])
+    if isinstance(x, Dirichlet):
+        a = np.asarray(x.alpha, np.float64).reshape(-1)
+        if a.shape != (K,):
+            raise ValueError(f"{what}: Dirichlet over {a.shape[0]} components, the model has K = {K}")
+        return a
+    raise TypeError(f"{what}: expected Dirichlet or Beta, got {type(x).__name__}")
+
+
+def _gaussians(xs, K, what):
+    if len(xs) != K:
+        raise ValueError(f"{what}: {len(xs)} marginals for K = {K} components")
+    mu, V = [], []
+    for x in xs:
+        if isinstance(x, NormalMeanVariance):
+            mu.append(np.array([float(x.m)])); V.append(np.array([[float(x.v)]]))
+        elif isinstance(x, MvNormalMeanCovariance):
+            mu.append(np.asarray(x.mu, np.float64).reshape(-1)); V.append(np.asarray(x.Sigma, np.float64))
+        else:
+            raise TypeError(f"{what}: expected NormalMeanVariance or MvNormalMeanCovariance, got {type(x).__name__}")
+    return np.stack(mu), np.stack(V)
+
+
+def _precisions(xs, K, what):
+    if len(xs) != K:
+        raise ValueError(f"{what}: {len(xs)} marginals for K = {K} components")
+    nu, S = [], []
+    for x in xs:
+        if isinstance(x, GammaShapeRate):          # Gamma(shape a, rate b) = Wishart(2a, 1 / (2b)) in one dimension
+            nu.append(2.0 * float(x.a)); S.append(np.array([[1.0 / (2.0 * float(x.b))]]))
+        elif isinstance(x, Wishart):
+            nu.append(float(x.df)); S.append(np.asarray(x.scale, np.float64))
+        else:
+            raise TypeError(f"{what}: expected Wishart or GammaShapeRate, got {type(x).__name__}")
+    return np.array(nu), np.stack(S)
+
+
+def gaussian_mixture_arrays(model, initialization):
+    """The model and its ``initialization`` in the Dirichlet / MvNormal / Wishart form of the C entry: a dict of host
+    arrays alpha0[K], mu0[K, d], V0[K, d, d], nu0[K], S0[K, d, d] and the same for the initial marginals (``*_init``,
+    ``Vm_init``), plus ``univariate`` (the model was written with Beta / Normal / Gamma)."""
+    K = int(model.K)
+    if not isinstance(initialization, dict) or not {"s", "m", "w"} <= set(initialization):
+        raise ValueError("gaussian_mixture needs initialization = {'s': q(s), 'm': [q(m[k])], 'w': [q(w[k])]}")
+    out = dict(alpha0=_weights(model.alpha0, K, "alpha0"), alpha_init=_weights(initialization["s"], K, "initialization['s']"))
+    out["mu0"], out["V0"] = _gaussians(model.m_prior, K, "m_prior")
+    out["m_init"], out["Vm_init"] = _gaussians(initialization["m"], K, "initialization['m']")
+    out["nu0"], out["S0"] = _precisions(model.w_prior, K, "w_prior")
+    out["nu_init"], out["S_init"] = _precisions(initialization["w"], K, "initialization['w']")
+    d = out["mu0"].shape[1]
+    for k in ("m_init", "V0", "Vm_init", "S0", "S_init"):
+        if out[k].shape[1] != d:
+            raise ValueError(f"{k}: dimension {out[k].shape[1]}, the means have d = {d}")
+    out["univariate"] = isinstance(model.alpha0, Beta)
+    return out
+
+
+def check_mean_field(constraints):
+    """The mixture node's rules exist for the naive mean-field only, as in the reference (the same message)."""
+    if not isinstance(constraints, MeanField):
+        raise ValueError("NormalMixture: the factorisation around the node must be the naive mean-field "
+                         "q(z) q(s) q(m[1]) ... q(m[K]) q(w[1]) ... q(w[K]); pass constraints = MeanField()")
+
+
 def vec_order(d):
     """perm with row_major = col_major[perm] (and col_major = row_major[perm]: a transpose is an involution) for vec(A)
     of a d x d matrix: Julia's vec is column-major, the C ABI's a[i * d + j] = A[i, j] row-major."""
@@ -255,6 +358,7 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
     With ``datastream=`` (an iterable of time-chunks, or ``None`` + ``autoupdates`` for a push-driven
     engine) the call returns an ``RxInferenceEngine`` (streaming.py), as the reference does when
     ``autoupdates`` is given (/root/reference/src/inference/inference.jl:577-733 dispatch)."""
+    constraints = kwargs.pop("constraints", None) if isinstance(model, gaussian_mixture) else None
     for k in kwargs:
         if k in _UNSUPPORTED:
             raise NotImplementedError(
@@ -449,6 +553,37 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             for name in ("p", "q"):
                 if r[f"df_{name}"] is not None:
                     post[f"w_{name}"] = WishartFast(r[f"df_{name}"], r[f"inv_scale_{name}"])
+            return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
+        if isinstance(model, gaussian_mixture):
+            check_mean_field(constraints)
+            if predictvars is not None:
+                raise NotImplementedError("predictvars: predictions of the Gaussian mixture are outside the batched hot path")
+            keep_each = isinstance(returnvars, KeepEach)
+            if returnvars is not None and not isinstance(returnvars, (KeepEach, KeepLast)):
+                raise NotImplementedError(f"returnvars={returnvars!r}: the Gaussian mixture returns KeepEach() or KeepLast()")
+            arr = gaussian_mixture_arrays(model, initialization)
+            yy = y[:, None] if y.dim() == 2 else y          # univariate data may come as [N, batch]
+            if yy.shape[1] != arr["mu0"].shape[1]:
+                raise ValueError(f"data['y'] has d = {yy.shape[1]}, the model's means d = {arr['mu0'].shape[1]}")
+            r = ctx.gmm_vmp(yy.contiguous(), *(arr[k] for k in ("alpha0", "mu0", "V0", "nu0", "S0", "alpha_init", "m_init",
+                                                                 "Vm_init", "nu_init", "S_init")),
+                            iterations=iterations or 1, want_free_energy=bool(free_energy), want_z=True, keep_each=keep_each)
+            bad = r["status"] != 0
+            if bool(bad.any()):
+                raise L.RxGaussError(L.RXG_ERR_NOT_SPD, f"{int(bad.sum())} of {bad.numel()} chains flagged NOT_SPD")
+            pre = "hist_" if keep_each else ""           # KeepEach: a leading iteration axis on every posterior
+            al, mm, mc = r[pre + "alpha"], r[pre + "m_mean"], r[pre + "m_cov"]
+            df, iS = r[pre + "w_df"], r[pre + "w_inv_scale"]
+            K = int(model.K)
+            if arr["univariate"]:
+                post = {"s": Beta(al[..., 0, :], al[..., 1, :]),
+                        "m": [NormalMeanVariance(mm[..., k, 0, :], mc[..., k, 0, 0, :]) for k in range(K)],
+                        "w": [GammaShapeRate(df[..., k, :] / 2, iS[..., k, 0, 0, :] / 2) for k in range(K)]}
+            else:
+                post = {"s": Dirichlet(al),
+                        "m": [MvNormalMeanCovariance(mm[..., k, :, :], mc[..., k, :, :, :]) for k in range(K)],
+                        "w": [WishartFast(df[..., k, :], iS[..., k, :, :, :]) for k in range(K)]}
+            post["z"] = Categorical(r["z_prob"])
             return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
         if isinstance(model, latent_autoregressive):
             yy = y[:, 0] if y.dim() == 3 else y

@@ -241,6 +241,14 @@ lar_vmp(ctx, order, T, batch, its, params, y, xm, xc, tm, tc, gs, gr, fe, st, fl
         (Ptr{Cvoid}, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Float64}, Ptr{Int32}, Cuint),
         ctx.handle, order, T, batch, its, params, y, xm, xc, tm, tc, gs, gr, fe, st, fl))
 
+gmm_vmp(ctx, d, K, N, batch, its, a0, mu0, V0, nu0, S0, ai, mi, Vi, nui, Si, y, al, mm, mc, df, iS, fe, z, hal, hmm, hmc, hdf, hiS,
+        st, fl) =
+    check(ctx, ccall((:rxg_gmm_vmp_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P,
+         F32P, F32P, Ptr{Float64}, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Int32}, Cuint),
+        ctx.handle, d, K, N, batch, its, a0, mu0, V0, nu0, S0, ai, mi, Vi, nui, Si, y, al, mm, mc, df, iS, fe, z, hal, hmm, hmc, hdf,
+        hiS, st, fl))
+
 # ---- diagnostics
 selftest_umma(ctx, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_f32, LIB), Cint, (Ptr{Cvoid}, F32P, F32P, F32P, Cuint), ctx.handle, A, B, D, fl))
 selftest_umma_shape(ctx, n, k, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_shape_f32, LIB), Cint, (Ptr{Cvoid}, Cint, Cint, F32P, F32P, F32P, Cuint), ctx.handle, n, k, A, B, D, fl))
@@ -831,6 +839,35 @@ function latent_ar(ctx::Context, y::Matrix{Float32}, order::Integer, τ::Real; i
     Lib.device_free(ctx, fe)
     return (x_mean = download(xm), x_cov = download(xc), θ_mean = download(tm), θ_cov = download(tc), γ_shape = download(gs),
             γ_rate = download(gr), free_energy = fe_host)
+end
+
+"""Fused mean-field VMP of the Gaussian mixture model (gmm_multivariate_tests.jl:4-64, `rxg_gmm_vmp_f32`); `y[batch, d, N]`.
+`alpha0`, `nu0` are `K` vectors, `mu0` a `d x K` matrix (one column per component), `V0`, `S0` `d x d x K` arrays (covariance,
+Wishart scale); the `init` NamedTuple `(alpha, m, Vm, nu, S)` holds the initial marginals in the same shapes.  The univariate
+model (gmm_univariate_tests.jl) is d = 1 with Beta(a, b) = Dirichlet([a, b]) and Gamma(shape, rate) = Wishart(2 shape,
+1 / (2 rate)).  Returns the KeepEach posteriors (trailing iteration axis): alpha `[batch, K, its]`, m mean `[batch, d, K, its]`,
+m cov `[batch, d, d, K, its]`, W df `[batch, K, its]`, W inverse scale `[batch, d, d, K, its]`, q(z) of the last iteration
+`[batch, K, N]`, the Bethe free energy `[batch, its]` (Float64) and the per-series status."""
+function gaussian_mixture(ctx::Context, y::Array{Float32, 3}; alpha0, mu0, V0, nu0, S0, init, iterations = 10)
+    batch, d, N = size(y)
+    K = length(alpha0)
+    dy = upload(ctx, y)
+    al, mm, mc = DeviceArray(ctx, batch, K), DeviceArray(ctx, batch, d, K), DeviceArray(ctx, batch, d, d, K)
+    df, iS = DeviceArray(ctx, batch, K), DeviceArray(ctx, batch, d, d, K)
+    z = DeviceArray(ctx, batch, K, N)
+    hal, hmm, hmc = DeviceArray(ctx, batch, K, iterations), DeviceArray(ctx, batch, d, K, iterations), DeviceArray(ctx, batch, d, d, K, iterations)
+    hdf, hiS = DeviceArray(ctx, batch, K, iterations), DeviceArray(ctx, batch, d, d, K, iterations)
+    st = DeviceArray(ctx, batch)
+    fe = Lib.device_alloc(ctx, 8 * batch * iterations)
+    h = [Float32.(collect(x)) for x in (alpha0, mu0, V0, nu0, S0, init.alpha, init.m, init.Vm, init.nu, init.S)]
+    GC.@preserve h Lib.gmm_vmp(ctx, d, K, N, batch, iterations, (pointer(x) for x in h)..., dy.ptr, al.ptr, mm.ptr, mc.ptr, df.ptr,
+                               iS.ptr, Ptr{Float64}(fe), z.ptr, hal.ptr, hmm.ptr, hmc.ptr, hdf.ptr, hiS.ptr,
+                               Ptr{Int32}(st.ptr), RXG_PTR_DEVICE)
+    fe_host = Array{Float64}(undef, batch, iterations)
+    GC.@preserve fe_host Lib.memcpy_d2h(ctx, pointer(fe_host), fe, 8 * batch * iterations)
+    Lib.device_free(ctx, fe)
+    return (s = download(hal), m_mean = download(hmm), m_cov = download(hmc), w_df = download(hdf), w_inv_scale = download(hiS),
+            z = download(z), free_energy = fe_host, status = reinterpret(Int32, download(st)))
 end
 
 # ---------------------------------------------------------------------------------------------- 4. pattern recogniser + infer_batched
