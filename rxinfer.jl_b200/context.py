@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes
 from ctypes import c_void_p
+from types import SimpleNamespace
 
 import numpy as np
 import torch
@@ -340,39 +341,19 @@ class Context:
         initial q(w) (default: the mean of ``vague(Wishart, m)``, m * 1e12 I).  Returns dict(mean[T, d, batch],
         cov[T, d, d, batch] of the last iteration, df[iterations, batch], inv_scale[iterations, m, m, batch] after every
         iteration, free_energy[iterations, batch] fp64 or None, status[batch])."""
-        if y.dim() != 3:
-            raise ValueError(f"y: expected [T, m, batch], got shape {tuple(y.shape)}")
-        T, m, batch = y.shape
+        m = self._vmp_dims(y)[1]
         d = np.asarray(A).shape[-1]
-        iterations = int(iterations)
-        if iterations < 1:
-            raise ValueError(f"iterations must be >= 1, got {iterations}")
-        nu0, inv_scale0 = (m + 1.0, np.eye(m)) if w_prior is None else w_prior
+        if w_prior is None:
+            w_prior = (m + 1.0, np.eye(m))
         if init_E_W is None:
             init_E_W = m * 1e12 * np.eye(m)                     # mean of vague(Wishart, m): df = m, scale 1e12 I
-        shapes = dict(A=(d, d), B=(m, d), P=(d, d), m0=(d,), S0=(d, d), inv_scale0=(m, m), init_E_W=(m, m))
-        mats = dict(A=A, B=B, P=P, m0=m0, S0=S0, inv_scale0=inv_scale0, init_E_W=init_E_W)
-        if u is not None:
-            shapes["u"], mats["u"] = (d,), u
-        keep = {}
-        for k, v in mats.items():
-            a, p = _model32(v)
-            if a.shape != shapes[k]:
-                raise ValueError(f"{k}: expected shape {shapes[k]}, got {a.shape}")
-            keep[k] = (a, p)
-        self._io(y, "y", True)
-        mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
-        mean, cov = self.empty(T, d, batch), self.empty(T, d, d, batch)
-        df, iS = self.empty(iterations, batch), self.empty(iterations, m, m, batch)
-        fe = self.empty(iterations, batch, dtype=torch.float64) if want_free_energy else None
-        st = self.empty(batch, dtype=torch.int32)
-        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
-        up = keep["u"][1] if "u" in keep else L.as_fp(0)
-        self._check(self.lib.rxg_lgssm_vmp_wishart_f32(
-            self.h, d, m, T, batch, iterations, keep["A"][1], keep["B"][1], keep["P"][1], keep["m0"][1], keep["S0"][1], up,
-            float(nu0), keep["inv_scale0"][1], keep["init_E_W"][1], _fp(y), mask_p, _fp(mean), _fp(cov), _fp(df), _fp(iS),
-            fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
-        return dict(mean=mean, cov=cov, df=df, inv_scale=iS, free_energy=fe, status=st)
+        c = self._vmp_setup(y, d, dict(A=A), dict(A=(d, d)), B, m0, S0, P, None, None, None, w_prior, init_E_W, u, iterations,
+                            mask, transition_first, asynchronous, want_free_energy, q_keys=("inv_scale0", "init_E_W"))
+        self._check(self.lib.rxg_lgssm_vmp_wishart_f32(       # this entry has no known Q and no outputs for P
+            *c.head, c.hp("A"), c.hp("B"), c.hp("P"), c.hp("m0"), c.hp("S0"), c.hp("u"), *c.q[1:], *c.io, *c.w_out[2:],
+            *c.tail))
+        return dict(mean=c.mean, cov=c.cov, df=c.out["df_q"], inv_scale=c.out["inv_scale_q"], free_energy=c.fe,
+                    status=c.st)
 
     def _vmp_mask_flags(self, mask, T, batch, keep, transition_first, asynchronous):
         """Mask pointer and flags of the Wishart VMP entries: a [T, batch] device mask per chain or a [T] pattern shared by
@@ -407,32 +388,36 @@ class Context:
         ``mask`` as for :meth:`lgssm_vmp_wishart`.  Returns dict(mean[T, d, batch], cov[T, d, d, batch] of the last
         iteration, df_p[iterations, batch] / inv_scale_p[iterations, d, d, batch] and df_q / inv_scale_q ([.., m, m, ..])
         after every iteration (None for a known noise), free_energy[iterations, batch] fp64 or None, status[batch])."""
+        self._vmp_dims(y)
+        d = np.asarray(A).shape[-1]
+        c = self._vmp_setup(y, d, dict(A=A), dict(A=(d, d)), B, m0, S0, P, p_prior, p_init, Q, q_prior, q_init, u, iterations,
+                            mask, transition_first, asynchronous, want_free_energy, both_known_ok=False)
+        self._check(self.lib.rxg_lgssm_vmp_noise_f32(
+            *c.head, c.hp("A"), c.hp("B"), c.hp("m0"), c.hp("S0"), c.hp("u"), *c.p, *c.q, *c.io, *c.w_out, *c.tail))
+        return dict(mean=c.mean, cov=c.cov, **c.out, free_energy=c.fe, status=c.st)
+
+    @staticmethod
+    def _vmp_dims(y):
         if y.dim() != 3:
             raise ValueError(f"y: expected [T, m, batch], got shape {tuple(y.shape)}")
-        d = np.asarray(A).shape[-1]
-        T, m, batch, iterations, keep, nus = self._vmp_noise_setup(
-            y, d, dict(A=A), dict(A=(d, d)), B, m0, S0, P, Q, p_prior, p_init, q_prior, q_init, u, iterations, False)
-        mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
-        mean, cov, out, fe, fe_p, st = self._vmp_noise_outputs(T, d, m, batch, iterations, nus, want_free_energy)
-        hp = lambda k: keep[k][1] if k in keep else L.as_fp(0)
-        self._check(self.lib.rxg_lgssm_vmp_noise_f32(
-            self.h, d, m, T, batch, iterations, hp("A"), hp("B"), hp("m0"), hp("S0"), hp("u"),
-            hp("P"), nus.get("p", 0.0), hp("inv_scale_p0"), hp("init_E_Wp"),
-            hp("Q"), nus.get("q", 0.0), hp("inv_scale_q0"), hp("init_E_Wq"),
-            _fp(y), mask_p, _fp(mean), _fp(cov), _fp(out["df_p"]), _fp(out["inv_scale_p"]), _fp(out["df_q"]),
-            _fp(out["inv_scale_q"]), fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
-        return dict(mean=mean, cov=cov, **out, free_energy=fe, status=st)
+        return y.shape
 
-    def _vmp_noise_setup(self, y, d, mats, shapes, B, m0, S0, P, Q, p_prior, p_init, q_prior, q_init, u, iterations,
-                         both_known_ok):
-        """Shared argument handling of the noise-learning VMP entries: each noise known or (prior, init); host model
-        arrays converted to row-major fp32 and shape-checked (kept alive in ``keep``); y validated."""
+    def _vmp_setup(self, y, d, mats, shapes, B, m0, S0, P, p_prior, p_init, Q, q_prior, q_init, u, iterations, mask,
+                   transition_first, asynchronous, want_free_energy, both_known_ok=True,
+                   q_keys=("inv_scale_q0", "init_E_Wq")):
+        """Shared argument handling of the Wishart VMP entries: each noise known or (prior, init), its host arrays named
+        ``inv_scale_p0`` / ``init_E_Wp`` and ``q_keys`` in the error texts; host model arrays converted to row-major fp32
+        and shape-checked (kept alive in ``keep``); then y and the mask validated and the outputs allocated.  Returns the
+        pieces of the C call: ``head`` (context and sizes), ``hp(key)`` (a host array's pointer, null if absent), ``p`` /
+        ``q`` (known, nu0, inv_scale0, init_E_W), ``io`` (y, mask, mean, cov), ``w_out`` (df_p, inv_scale_p, df_q,
+        inv_scale_q; null for a known noise), ``tail`` (free energy, status, flags), next to the output tensors."""
         T, m, batch = y.shape
         iterations = int(iterations)
         if iterations < 1:
             raise ValueError(f"iterations must be >= 1, got {iterations}")
         shapes = dict(shapes, B=(m, d), m0=(d,), S0=(d, d))
         mats = dict(mats, B=B, m0=m0, S0=S0)
+        keys = dict(p=("inv_scale_p0", "init_E_Wp"), q=q_keys)
         nus = {}
         for name, k, known, prior, init in (("p", d, P, p_prior, p_init), ("q", m, Q, q_prior, q_init)):
             if known is not None:
@@ -444,8 +429,8 @@ class Context:
                 raise ValueError(f"{name.upper()} is learned: pass {name}_prior = (nu0, inv_scale0) and {name}_init = E[w] "
                                  f"of the initial q(w_{name}) (there is no default initial q(w))")
             nus[name] = float(prior[0])
-            shapes[f"inv_scale_{name}0"], mats[f"inv_scale_{name}0"] = (k, k), prior[1]
-            shapes[f"init_E_W{name}"], mats[f"init_E_W{name}"] = (k, k), init
+            for key, v in zip(keys[name], (prior[1], init)):
+                shapes[key], mats[key] = (k, k), v
         if not nus and not both_known_ok:
             raise ValueError("P and Q are both known: that is the plain smoother (Context.lgssm)")
         if u is not None:
@@ -457,19 +442,23 @@ class Context:
                 raise ValueError(f"{k}: expected shape {shapes[k]}, got {a.shape}")
             keep[k] = (a, p)
         self._io(y, "y", True)
-        return T, m, batch, iterations, keep, nus
-
-    def _vmp_noise_outputs(self, T, d, m, batch, iterations, nus, want_free_energy):
-        mean, cov = self.empty(T, d, batch), self.empty(T, d, d, batch)
-        out = {}
+        mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
+        c = SimpleNamespace(keep=keep, iterations=iterations, batch=batch, mean=self.empty(T, d, batch),
+                            cov=self.empty(T, d, d, batch), out={})
         for name, k in (("p", d), ("q", m)):
             learned = name in nus
-            out[f"df_{name}"] = self.empty(iterations, batch) if learned else None
-            out[f"inv_scale_{name}"] = self.empty(iterations, k, k, batch) if learned else None
-        fe = self.empty(iterations, batch, dtype=torch.float64) if want_free_energy else None
-        st = self.empty(batch, dtype=torch.int32)
-        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
-        return mean, cov, out, fe, fe_p, st
+            c.out[f"df_{name}"] = self.empty(iterations, batch) if learned else None
+            c.out[f"inv_scale_{name}"] = self.empty(iterations, k, k, batch) if learned else None
+        c.fe = self.empty(iterations, batch, dtype=torch.float64) if want_free_energy else None
+        c.st = self.empty(batch, dtype=torch.int32)
+        c.hp = lambda k: keep[k][1] if k in keep else L.as_fp(0)
+        c.head = (self.h, d, m, T, batch, iterations)
+        c.p, c.q = ((c.hp(name.upper()), nus.get(name, 0.0), *map(c.hp, keys[name])) for name in ("p", "q"))
+        c.io = (_fp(y), mask_p, _fp(c.mean), _fp(c.cov))
+        c.w_out = tuple(_fp(c.out[k]) for k in ("df_p", "inv_scale_p", "df_q", "inv_scale_q"))
+        c.tail = (ctypes.cast(c_void_p(c.fe.data_ptr() if c.fe is not None else None), ctypes.POINTER(ctypes.c_double)),
+                  ctypes.cast(c_void_p(c.st.data_ptr()), L.i32p), flags)
+        return c
 
     def lgssm_vmp_transition(self, y, B, m0, S0, *, a_prior, a_init, P=None, Q=None, p_prior=None, p_init=None,
                              q_prior=None, q_init=None, u=None, mask=None, transition_first=False, iterations=10,
@@ -481,8 +470,7 @@ class Context:
         a[i * d + j] = A[i, j]: means [d, d] (or [d * d]), covariances [d * d, d * d].  Each noise as for
         :meth:`lgssm_vmp_noise`; both may be known.  d <= 4.  Returns the dict of :meth:`lgssm_vmp_noise` plus
         a_mean[iterations, d, d, batch] and a_cov[iterations, d * d, d * d, batch] after every iteration."""
-        if y.dim() != 3:
-            raise ValueError(f"y: expected [T, m, batch], got shape {tuple(y.shape)}")
+        self._vmp_dims(y)
         d = np.asarray(S0).shape[-1]
         n = d * d
         if not (isinstance(a_prior, (tuple, list)) and len(a_prior) == 2):
@@ -492,20 +480,13 @@ class Context:
         mats = dict(a_mean0=np.asarray(a_prior[0]).reshape(-1), a_cov0=a_prior[1],
                     a_init_mean=np.asarray(a_init[0]).reshape(-1), a_init_cov=a_init[1])
         shapes = dict(a_mean0=(n,), a_cov0=(n, n), a_init_mean=(n,), a_init_cov=(n, n))
-        T, m, batch, iterations, keep, nus = self._vmp_noise_setup(
-            y, d, mats, shapes, B, m0, S0, P, Q, p_prior, p_init, q_prior, q_init, u, iterations, True)
-        mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
-        mean, cov, out, fe, fe_p, st = self._vmp_noise_outputs(T, d, m, batch, iterations, nus, want_free_energy)
-        a_mean, a_cov = self.empty(iterations, d, d, batch), self.empty(iterations, n, n, batch)
-        hp = lambda k: keep[k][1] if k in keep else L.as_fp(0)
+        c = self._vmp_setup(y, d, mats, shapes, B, m0, S0, P, p_prior, p_init, Q, q_prior, q_init, u, iterations, mask,
+                            transition_first, asynchronous, want_free_energy)
+        a_mean, a_cov = self.empty(c.iterations, d, d, c.batch), self.empty(c.iterations, n, n, c.batch)
         self._check(self.lib.rxg_lgssm_vmp_transition_f32(
-            self.h, d, m, T, batch, iterations, hp("a_mean0"), hp("a_cov0"), hp("a_init_mean"), hp("a_init_cov"),
-            hp("B"), hp("m0"), hp("S0"), hp("u"),
-            hp("P"), nus.get("p", 0.0), hp("inv_scale_p0"), hp("init_E_Wp"),
-            hp("Q"), nus.get("q", 0.0), hp("inv_scale_q0"), hp("init_E_Wq"),
-            _fp(y), mask_p, _fp(mean), _fp(cov), _fp(a_mean), _fp(a_cov), _fp(out["df_p"]), _fp(out["inv_scale_p"]),
-            _fp(out["df_q"]), _fp(out["inv_scale_q"]), fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p), flags))
-        return dict(mean=mean, cov=cov, a_mean=a_mean, a_cov=a_cov, **out, free_energy=fe, status=st)
+            *c.head, c.hp("a_mean0"), c.hp("a_cov0"), c.hp("a_init_mean"), c.hp("a_init_cov"), c.hp("B"), c.hp("m0"),
+            c.hp("S0"), c.hp("u"), *c.p, *c.q, *c.io, _fp(a_mean), _fp(a_cov), *c.w_out, *c.tail))
+        return dict(mean=c.mean, cov=c.cov, a_mean=a_mean, a_cov=a_cov, **c.out, free_energy=c.fe, status=c.st)
 
     # ------------------------------------------------------------------ per-rule kernels
     def _mat(self, M):

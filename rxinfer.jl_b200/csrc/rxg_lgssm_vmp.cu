@@ -114,42 +114,9 @@ __device__ __forceinline__ double digamma_d(double x) {      // psi(x), x > 0: r
     return r + log(x) - 0.5 * i - i2 * (1.0 / 12 - i2 * (1.0 / 120 - i2 * (1.0 / 252 - i2 * (1.0 / 240 - i2 * (1.0 / 132)))));
 }
 
-// RTS pair hook: V = cov(x_{t+1} - A x_t | y) = (I - A G) Ss (I - A G)' + A C A', Ss the smoothed covariance at t+1
-template <int D>
-struct PairCov {
-    const Mat<float, D, D>& A;
-    Mat<float, D, D>& V;
-    __device__ __forceinline__ void operator()(const Mat<float, D, D>& G, const Mat<float, D, D>& C,
-                                               const Mat<float, D, D>& Ss) const {
-        Mat<float, D, D> F = mul(A, G);
-#pragma unroll
-        for (int i = 0; i < D; ++i)
-#pragma unroll
-            for (int j = 0; j < D; ++j) F(i, j) = (i == j ? 1.f : 0.f) - F(i, j);
-        Mat<float, D, D> AC = mul(A, C), Z = {};
-        Mat<float, D, D> FS = mul(F, Ss);
-        V = sym_mul_nt_add(FS, F, sym_mul_nt_add(AC, A, Z));
-    }
-};
-
-// R_p += e e' + V, e = mnext - A ms - u: one transition's term (fp32) folded into the fp64 lower triangle
-template <int D>
-__device__ __forceinline__ void accumulate_pair(double* Rp, const Mat<float, D, D>& A, const Vec<float, D>& u,
-                                                const Vec<float, D>& mnext, const Vec<float, D>& ms,
-                                                const Mat<float, D, D>& V) {
-    Vec<float, D> e = mulv(A, ms);
-#pragma unroll
-    for (int k = 0; k < D; ++k) e(k) = mnext(k) - (e(k) + u(k));
-    int q = 0;
-#pragma unroll
-    for (int k = 0; k < D; ++k)
-#pragma unroll
-        for (int l = 0; l <= k; ++l) Rp[q++] += (double)__fmaf_rn(e(k), e(l), V(k, l));
-}
-
-// RTS pair hook of the A-learning model: X = cov(x_t, x_{t+1} - A x_t | y) = G Ss (I - A G)' - C A' and, when P is
-// learned, V as PairCov forms it
-template <int D, bool WANT_V>
+// RTS pair hook, Ss the smoothed covariance at t+1 and F = I - A G: with WANT_V (P learned)
+// V = cov(x_{t+1} - A x_t | y) = F Ss F' + A C A', with WANT_X (A learned) X = cov(x_t, x_{t+1} - A x_t | y) = G Ss F' - C A'
+template <int D, bool WANT_X, bool WANT_V>
 struct PairStats {
     const Mat<float, D, D>& A;
     Mat<float, D, D>& V;
@@ -161,9 +128,11 @@ struct PairStats {
         for (int i = 0; i < D; ++i)
 #pragma unroll
             for (int j = 0; j < D; ++j) F(i, j) = (i == j ? 1.f : 0.f) - F(i, j);
-        Mat<float, D, D> GS = mul(G, Ss), GSF = mul_nt(GS, F), CA = mul_nt(C, A);
+        if constexpr (WANT_X) {
+            Mat<float, D, D> GS = mul(G, Ss), GSF = mul_nt(GS, F), CA = mul_nt(C, A);
 #pragma unroll
-        for (int i = 0; i < D * D; ++i) X.a[i] = GSF.a[i] - CA.a[i];
+            for (int i = 0; i < D * D; ++i) X.a[i] = GSF.a[i] - CA.a[i];
+        }
         if constexpr (WANT_V) {
             Mat<float, D, D> AC = mul(A, C), Z = {};
             Mat<float, D, D> FS = mul(F, Ss);
@@ -172,9 +141,9 @@ struct PairStats {
     }
 };
 
-// one transition's source-state statistics folded into fp64: Sxx += Ss + ms ms' (lower triangle), Sxr += X + ms e',
-// e = mnext - A ms - u; with WANT_RP also R_p += e e' + V (accumulate_pair)
-template <int D, bool WANT_RP>
+// one transition's term (fp32) folded into the fp64 sums, e = mnext - A ms - u: with WANT_RP R_p += e e' + V (lower
+// triangle); with WANT_S the source-state statistics Sxx += Ss + ms ms' (lower triangle), Sxr += X + ms e'
+template <int D, bool WANT_S, bool WANT_RP>
 __device__ __forceinline__ void accumulate_stats(double* Rp, double* Sxx, double* Sxr, const Mat<float, D, D>& A,
                                                  const Vec<float, D>& u, const Vec<float, D>& mnext,
                                                  const Vec<float, D>& ms, const Mat<float, D, D>& Ss,
@@ -187,14 +156,16 @@ __device__ __forceinline__ void accumulate_stats(double* Rp, double* Sxx, double
     for (int k = 0; k < D; ++k)
 #pragma unroll
         for (int l = 0; l <= k; ++l) {
-            Sxx[q] += (double)__fmaf_rn(ms(k), ms(l), Ss(k, l));
+            if constexpr (WANT_S) Sxx[q] += (double)__fmaf_rn(ms(k), ms(l), Ss(k, l));
             if constexpr (WANT_RP) Rp[q] += (double)__fmaf_rn(e(k), e(l), V(k, l));
             ++q;
         }
+    if constexpr (WANT_S) {
 #pragma unroll
-    for (int k = 0; k < D; ++k)
+        for (int k = 0; k < D; ++k)
 #pragma unroll
-        for (int l = 0; l < D; ++l) Sxr[k * D + l] += (double)__fmaf_rn(ms(k), e(l), X(k, l));
+            for (int l = 0; l < D; ++l) Sxr[k * D + l] += (double)__fmaf_rn(ms(k), e(l), X(k, l));
+    }
 }
 
 // the fp32 factor L (L L' = Xi) of the tilt of one sweep, Xi[j][k] = sum_{i,l} W[i][l] Sa[(i,j),(l,k)] (fp64)
@@ -581,16 +552,11 @@ lgssm_vmp_wishart_kernel(const __grid_constant__ VmpModel<D, M, LEARN> mdl, cons
             for (int k = 0; k < M; ++k) yv(k) = py[k];
             const bool ob = po;
             if (t > 0) prefetch(t - 1);
-            if constexpr (LA) {
+            if constexpr (LA || LP) {
                 const Vec<float, D> mnext = mus;
                 Mat<float, D, D> V, X;
-                chain_rts(Ab, Pb, u, NoInput{}, muf, Sf, mus, Ss, bad, PairStats<D, LP>{Ab, V, X});
-                accumulate_stats<D, LP>(Rp, Sxx, Sxr, Ab, u, mnext, mus, Ss, V, X);
-            } else if constexpr (LP) {
-                const Vec<float, D> mnext = mus;
-                Mat<float, D, D> V;
-                chain_rts(A, Pb, u, NoInput{}, muf, Sf, mus, Ss, bad, PairCov<D>{A, V});
-                accumulate_pair(Rp, A, u, mnext, mus, V);
+                chain_rts(Ab, Pb, u, NoInput{}, muf, Sf, mus, Ss, bad, PairStats<D, LA, LP>{Ab, V, X});
+                accumulate_stats<D, LA, LP>(Rp, Sxx, Sxr, Ab, u, mnext, mus, Ss, V, X);
             } else {
                 chain_rts(A, Pb, u, NoInput{}, muf, Sf, mus, Ss, bad);
             }
@@ -606,25 +572,23 @@ lgssm_vmp_wishart_kernel(const __grid_constant__ VmpModel<D, M, LEARN> mdl, cons
                 if (ob) accumulate(mus, Ss, yv);
             }
         }
-        if constexpr (LA) {
-            if (io.tf) {   // the transition from the (tilted) prior state into x[1], as below
+        if constexpr (LA || LP) {
+            // the transition from the prior state (tilted when A is learned) into x[1]: one more RTS step from (m0, S0),
+            // not written out
+            if (io.tf) {
                 Vec<float, D> m0v, mx = mus;
-                Mat<float, D, D> S0t = S0, Sx = Ss, V, X;
+                Mat<float, D, D> S0t, Sx = Ss, V, X;
 #pragma unroll
                 for (int i = 0; i < D; ++i) m0v(i) = mdl.m0[i];
-                double unused = 0.0;
-                chain_tilt(Lx, false, m0v, S0t, bad, unused);
-                chain_rts(Ab, Pb, u, NoInput{}, m0v, S0t, mx, Sx, bad, PairStats<D, LP>{Ab, V, X});
-                accumulate_stats<D, LP>(Rp, Sxx, Sxr, Ab, u, mus, mx, Sx, V, X);
-            }
-        } else if constexpr (LP) {
-            if (io.tf) {   // the transition from the prior state into x[1]: one more RTS step from (m0, S0), not written out
-                Vec<float, D> m0v, mx = mus;
-                Mat<float, D, D> Sx = Ss, V;
-#pragma unroll
-                for (int i = 0; i < D; ++i) m0v(i) = mdl.m0[i];
-                chain_rts(A, Pb, u, NoInput{}, m0v, S0, mx, Sx, bad, PairCov<D>{A, V});
-                accumulate_pair(Rp, A, u, mus, mx, V);
+                if constexpr (LA) {
+                    double unused = 0.0;
+                    S0t = S0;
+                    chain_tilt(Lx, false, m0v, S0t, bad, unused);
+                }
+                // bound, not copied, when A is known: a copy of S0 changes the learn-P kernels' instruction schedule
+                const Mat<float, D, D>& S0b = LA ? S0t : S0;
+                chain_rts(Ab, Pb, u, NoInput{}, m0v, S0b, mx, Sx, bad, PairStats<D, LA, LP>{Ab, V, X});
+                accumulate_stats<D, LA, LP>(Rp, Sxx, Sxr, Ab, u, mus, mx, Sx, V, X);
             }
         }
         mu = mus;
@@ -727,54 +691,9 @@ RXG_VMP_EXTERN(RXG_VMP_DECL_A, 4)
 #undef RXG_VMP_EXTERN
 
 namespace {
-// fp64 Cholesky of the symmetrised (A + A')/2 on the host: false if it is not SPD; log det on success
-bool host_spd(const float* a, int m, double* sym, double* logdet) {
-    double L[36] = {};
-    for (int i = 0; i < m; ++i)
-        for (int j = 0; j < m; ++j) sym[i * m + j] = 0.5 * ((double)a[i * m + j] + (double)a[j * m + i]);
-    double ld = 0.0;
-    for (int j = 0; j < m; ++j) {
-        double s = sym[j * m + j];
-        for (int k = 0; k < j; ++k) s -= L[j * m + k] * L[j * m + k];
-        if (!(s > 0.0) || !isfinite(s)) return false;
-        L[j * m + j] = sqrt(s);
-        ld += 2.0 * log(L[j * m + j]);
-        for (int i = j + 1; i < m; ++i) {
-            double t = sym[i * m + j];
-            for (int k = 0; k < j; ++k) t -= L[i * m + k] * L[j * m + k];
-            L[i * m + j] = t / L[j * m + j];
-        }
-    }
-    *logdet = ld;
-    return true;
-}
-
-template <int LEARN>
-int dispatch_shape(rxg_ctx* ctx, int d, int m, const VmpWishHost& h, const VmpTransIO& io) {
-#define RXG_VMP_CASE(DD, MM) case DD * 16 + MM: return launch_vmp_wishart<DD, MM, LEARN>(ctx, h, io);
-#define RXG_VMP_ROW(DD) RXG_VMP_CASE(DD, 1) RXG_VMP_CASE(DD, 2) RXG_VMP_CASE(DD, 3) RXG_VMP_CASE(DD, 4) \
-                        RXG_VMP_CASE(DD, 5) RXG_VMP_CASE(DD, 6)
-    if constexpr ((LEARN & LEARN_A) != 0) {
-        switch (d * 16 + m) {
-            RXG_VMP_ROW(1) RXG_VMP_ROW(2) RXG_VMP_ROW(3) RXG_VMP_ROW(4)
-            default: return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_vmp: d must be in 1..4 and m in 1..6 (got d=%d, m=%d)", d, m);
-        }
-    } else {
-        switch (d * 16 + m) {
-            RXG_VMP_ROW(1) RXG_VMP_ROW(2) RXG_VMP_ROW(3) RXG_VMP_ROW(4) RXG_VMP_ROW(5) RXG_VMP_ROW(6)
-            default: return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_vmp: d and m must be in 1..6 (got d=%d, m=%d)", d, m);
-        }
-    }
-#undef RXG_VMP_ROW
-#undef RXG_VMP_CASE
-}
-
-}  // namespace
-
-// fp64 Cholesky of the symmetrised n x n matrix on the host (n <= 16), then its inverse: false if it is not SPD
-// (declared in rxg_internal.h: the Gaussian-mixture entry validates its host matrices with it too)
-bool host_spd_inv(const float* a, int n, double* inv, double* logdet) {
-    double L[256] = {}, Li[256] = {};
+// fp64 Cholesky L L' of the symmetrised (A + A')/2 on the host (n <= 16): false if it is not SPD or not finite; L
+// (lower, the rest untouched) and log det on success
+bool host_chol(const float* a, int n, double* L, double* logdet) {
     double ld = 0.0;
     for (int j = 0; j < n; ++j) {
         double s = 0.5 * ((double)a[j * n + j] + (double)a[j * n + j]);
@@ -788,6 +707,44 @@ bool host_spd_inv(const float* a, int n, double* inv, double* logdet) {
             L[i * n + j] = t / L[j * n + j];
         }
     }
+    *logdet = ld;
+    return true;
+}
+
+// the symmetrised matrix itself, checked to be SPD
+bool host_spd(const float* a, int m, double* sym, double* logdet) {
+    double L[36];
+    for (int i = 0; i < m; ++i)
+        for (int j = 0; j < m; ++j) sym[i * m + j] = 0.5 * ((double)a[i * m + j] + (double)a[j * m + i]);
+    return host_chol(a, m, L, logdet);
+}
+
+// the kernel of (learn, d, m): the instantiations of RXG_VMP_DECL (d = 1..6) and RXG_VMP_DECL_A (d = 1..4)
+int dispatch_vmp(rxg_ctx* ctx, int learn, int d, int m, const VmpWishHost& h, const VmpTransIO& io) {
+#define RXG_VMP_CASE(LL, DD, MM) case ((LL) * 8 + DD) * 8 + MM: return launch_vmp_wishart<DD, MM, LL>(ctx, h, io);
+#define RXG_VMP_ROW(LL, DD) RXG_VMP_CASE(LL, DD, 1) RXG_VMP_CASE(LL, DD, 2) RXG_VMP_CASE(LL, DD, 3) \
+                            RXG_VMP_CASE(LL, DD, 4) RXG_VMP_CASE(LL, DD, 5) RXG_VMP_CASE(LL, DD, 6)
+#define RXG_VMP_D4(LL) RXG_VMP_ROW(LL, 1) RXG_VMP_ROW(LL, 2) RXG_VMP_ROW(LL, 3) RXG_VMP_ROW(LL, 4)
+#define RXG_VMP_D6(LL) RXG_VMP_D4(LL) RXG_VMP_ROW(LL, 5) RXG_VMP_ROW(LL, 6)
+    switch ((learn * 8 + d) * 8 + m) {
+        RXG_VMP_D6(LEARN_Q) RXG_VMP_D6(LEARN_P) RXG_VMP_D6(LEARN_PQ)
+        RXG_VMP_D4(LEARN_A) RXG_VMP_D4(LEARN_A | LEARN_Q) RXG_VMP_D4(LEARN_A | LEARN_P) RXG_VMP_D4(LEARN_A | LEARN_PQ)
+        default:     // not reached: vmp_noise() has refused every other combination
+            return fail(ctx, RXG_ERR_UNSUPPORTED, "lgssm_vmp: no kernel for learn=%d, d=%d, m=%d", learn, d, m);
+    }
+#undef RXG_VMP_D6
+#undef RXG_VMP_D4
+#undef RXG_VMP_ROW
+#undef RXG_VMP_CASE
+}
+
+}  // namespace
+
+// fp64 Cholesky of the symmetrised n x n matrix on the host (n <= 16), then its inverse: false if it is not SPD
+// (declared in rxg_internal.h: the Gaussian-mixture entry validates its host matrices with it too)
+bool host_spd_inv(const float* a, int n, double* inv, double* logdet) {
+    double L[256], Li[256] = {};
+    if (!host_chol(a, n, L, logdet)) return false;
     for (int j = 0; j < n; ++j) {
         Li[j * n + j] = 1.0 / L[j * n + j];
         for (int i = j + 1; i < n; ++i) {
@@ -802,7 +759,6 @@ bool host_spd_inv(const float* a, int n, double* inv, double* logdet) {
             for (int k = (r > c ? r : c); k < n; ++k) s += Li[k * n + r] * Li[k * n + c];
             inv[r * n + c] = s;
         }
-    *logdet = ld;
     return true;
 }
 
@@ -916,16 +872,8 @@ int vmp_noise(rxg_ctx* ctx, const char* who, int d, int m, int T, int64_t batch,
             io.ymask = ymask;
         }
     }
-    if (ta) {
-        rc = np.learned() ? (nq.learned() ? dispatch_shape<LEARN_A | LEARN_PQ>(ctx, d, m, h, io)
-                                          : dispatch_shape<LEARN_A | LEARN_P>(ctx, d, m, h, io))
-                          : (nq.learned() ? dispatch_shape<LEARN_A | LEARN_Q>(ctx, d, m, h, io)
-                                          : dispatch_shape<LEARN_A>(ctx, d, m, h, io));
-    } else {
-        rc = !np.learned() ? dispatch_shape<LEARN_Q>(ctx, d, m, h, io)
-                           : (nq.learned() ? dispatch_shape<LEARN_PQ>(ctx, d, m, h, io) : dispatch_shape<LEARN_P>(ctx, d, m, h, io));
-    }
-    if (rc != RXG_OK) return rc;
+    const int learn = (ta ? LEARN_A : 0) | (np.learned() ? LEARN_P : 0) | (nq.learned() ? LEARN_Q : 0);
+    if ((rc = dispatch_vmp(ctx, learn, d, m, h, io)) != RXG_OK) return rc;
     if (!(flags & RXG_ASYNC)) RXG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return RXG_OK;
 }

@@ -347,6 +347,39 @@ def _predict_keys(predictvars, model, data):
     return keys
 
 
+def _raise_flagged(status, prefix="", suffix=""):
+    """Raise ``RxGaussError`` when the kernel flagged some chains: RXG_ERR_NOT_SPD if any chain is NOT_SPD, else the first
+    flagged chain's code; the message counts the chains and names the codes."""
+    bad = status != 0
+    if bool(bad.any()):
+        codes = sorted({L.STATUS_NAMES.get(int(c), str(int(c))) for c in status[bad].unique().tolist()})
+        raise L.RxGaussError(L.RXG_ERR_NOT_SPD if "NOT_SPD" in codes else int(status[bad][0]),
+                             f"{prefix}{int(bad.sum())} of {bad.numel()} chains flagged {codes}{suffix}")
+
+
+def _noise_kwargs(model):
+    """The P / Q arguments of ``Context.lgssm_vmp_noise`` / ``lgssm_vmp_transition`` from a model whose noises are each
+    known (``P`` / ``Q``) or learned (``*_prior`` / ``*_init`` as ``Wishart``)."""
+    kw = {}
+    for name in ("p", "q"):
+        known, prior, init = getattr(model, name.upper()), getattr(model, f"{name}_prior"), getattr(model, f"{name}_init")
+        if known is not None and (prior is not None or init is not None):
+            raise ValueError(f"{name.upper()} is known: pass either {name.upper()} or {name}_prior / {name}_init")
+        if known is not None:
+            kw[name.upper()] = known
+        elif prior is not None and init is not None:
+            kw[f"{name}_prior"], kw[f"{name}_init"] = (prior.df, prior.inv_scale()), init.mean()
+        else:
+            kw[f"{name}_prior"], kw[f"{name}_init"] = prior, init    # Context names what is missing
+    return kw
+
+
+def _noise_posteriors(r):
+    """``w_p`` / ``w_q`` of the learned precisions from a noise-learning result (KeepEach: leading iteration axis)."""
+    return {f"w_{name}": WishartFast(r[f"df_{name}"], r[f"inv_scale_{name}"]) for name in ("p", "q")
+            if r[f"df_{name}"] is not None}
+
+
 def infer(*, model, iterations=None, free_energy=False, returnvars=None, options=None,
           initialization=None, autoupdates=None, keephistory=None, historyvars=None,
           catch_exception=False, showprogress=False, session=None, warn=True, allow_node_contraction=False,
@@ -429,13 +462,9 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
                                       u=model.u, inputs=inputs, mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain,
                                       cov_shared_out=cov_shared_out, transition_first=model.prior_on_previous_state,
                                       want_status=True)
-                bad = r["status"] != 0
-                if bool(bad.any()):      # e.g. a chain whose D_t = Q - B S_s B' is not SPD has no usable prediction
-                    codes = sorted({L.STATUS_NAMES.get(int(c), str(int(c))) for c in r["status"][bad].unique().tolist()})
-                    raise L.RxGaussError(L.RXG_ERR_NOT_SPD if "NOT_SPD" in codes else int(r["status"][bad][0]),
-                                         f"predictions: {int(bad.sum())} of {bad.numel()} chains flagged {codes} (NOT_SPD: "
-                                         "Q - B S_s B' is not SPD, the observations dominate beyond the fp32 posterior "
-                                         "covariances)")
+                # e.g. a chain whose D_t = Q - B S_s B' is not SPD has no usable prediction
+                _raise_flagged(r["status"], "predictions: ", " (NOT_SPD: Q - B S_s B' is not SPD, the observations dominate "
+                                                             "beyond the fp32 posterior covariances)")
                 T = y.shape[0]
                 mean, cov = r["mean"], r["cov"]
                 if horizon > 0:          # posteriors["x"] covers x[1..T+H], as model_1's x covers n + 2 states
@@ -481,53 +510,21 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
                                       w_prior=(model.w_prior.df, model.w_prior.inv_scale()), init_E_W=model.w_init.mean(),
                                       u=model.u, mask=mask, transition_first=model.prior_on_previous_state,
                                       want_free_energy=bool(free_energy))
-            bad = r["status"] != 0
-            if bool(bad.any()):
-                codes = sorted({L.STATUS_NAMES.get(int(c), str(int(c))) for c in r["status"][bad].unique().tolist()})
-                raise L.RxGaussError(L.RXG_ERR_NOT_SPD if "NOT_SPD" in codes else int(r["status"][bad][0]),
-                                     f"{int(bad.sum())} of {bad.numel()} chains flagged {codes}")
+            _raise_flagged(r["status"])
             # returnvars of the reference's call under `iterations`: x = KeepLast() here, w = KeepEach() (iteration axis)
             return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]),
                                                "w": WishartFast(r["df"], r["inv_scale"])},
                                    model=model, free_energy=r["free_energy"])
         if isinstance(model, linear_gaussian_ssm_wishart_noise):
-            kw = {}
-            for name in ("p", "q"):
-                known, prior, init = getattr(model, name.upper()), getattr(model, f"{name}_prior"), getattr(model, f"{name}_init")
-                if known is not None:
-                    kw[name.upper()] = known
-                elif prior is not None and init is not None:
-                    kw[f"{name}_prior"], kw[f"{name}_init"] = (prior.df, prior.inv_scale()), init.mean()
-                else:
-                    kw[f"{name}_prior"], kw[f"{name}_init"] = prior, init    # Context names what is missing
-                if known is not None and (prior is not None or init is not None):
-                    raise ValueError(f"{name.upper()} is known: pass either {name.upper()} or {name}_prior / {name}_init")
-            r = ctx.lgssm_vmp_noise(y, model.A, model.B, model.x0[0], model.x0[1], **kw, u=model.u, mask=mask,
-                                    transition_first=model.prior_on_previous_state, iterations=iterations or 1,
-                                    want_free_energy=bool(free_energy))
-            bad = r["status"] != 0
-            if bool(bad.any()):
-                codes = sorted({L.STATUS_NAMES.get(int(c), str(int(c))) for c in r["status"][bad].unique().tolist()})
-                raise L.RxGaussError(L.RXG_ERR_NOT_SPD if "NOT_SPD" in codes else int(r["status"][bad][0]),
-                                     f"{int(bad.sum())} of {bad.numel()} chains flagged {codes}")
+            r = ctx.lgssm_vmp_noise(y, model.A, model.B, model.x0[0], model.x0[1], **_noise_kwargs(model), u=model.u,
+                                    mask=mask, transition_first=model.prior_on_previous_state,
+                                    iterations=iterations or 1, want_free_energy=bool(free_energy))
+            _raise_flagged(r["status"])
             # x = KeepLast(), w_p / w_q = KeepEach() (leading iteration axis) for the learned precisions
-            post = {"x": MvNormalMeanCovariance(r["mean"], r["cov"])}
-            for name in ("p", "q"):
-                if r[f"df_{name}"] is not None:
-                    post[f"w_{name}"] = WishartFast(r[f"df_{name}"], r[f"inv_scale_{name}"])
-            return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
+            return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]), **_noise_posteriors(r)},
+                                   model=model, free_energy=r["free_energy"])
         if isinstance(model, linear_gaussian_ssm_continuous_transition):
-            kw = {}
-            for name in ("p", "q"):
-                known, prior, init = getattr(model, name.upper()), getattr(model, f"{name}_prior"), getattr(model, f"{name}_init")
-                if known is not None and (prior is not None or init is not None):
-                    raise ValueError(f"{name.upper()} is known: pass either {name.upper()} or {name}_prior / {name}_init")
-                if known is not None:
-                    kw[name.upper()] = known
-                elif prior is not None and init is not None:
-                    kw[f"{name}_prior"], kw[f"{name}_init"] = (prior.df, prior.inv_scale()), init.mean()
-                else:
-                    kw[f"{name}_prior"], kw[f"{name}_init"] = prior, init    # Context names what is missing
+            kw = _noise_kwargs(model)
             if model.a_init is None:
                 raise ValueError("a_init: q(a) needs an initial (mean, covariance) (an uninformed q(a) makes the first "
                                  "sweep meaningless)")
@@ -539,21 +536,15 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
                                          a_init=rowmajor(model.a_init), **kw, u=model.u, mask=mask,
                                          transition_first=model.prior_on_previous_state, iterations=iterations or 1,
                                          want_free_energy=bool(free_energy))
-            bad = r["status"] != 0
-            if bool(bad.any()):
-                codes = sorted({L.STATUS_NAMES.get(int(c), str(int(c))) for c in r["status"][bad].unique().tolist()})
-                raise L.RxGaussError(L.RXG_ERR_NOT_SPD if "NOT_SPD" in codes else int(r["status"][bad][0]),
-                                     f"{int(bad.sum())} of {bad.numel()} chains flagged {codes}")
+            _raise_flagged(r["status"])
             # x = KeepLast(); a, w_p / w_q = KeepEach() (leading iteration axis); a over vec(A) in column-major order
             pt = torch.as_tensor(pm, device=r["a_mean"].device)
             its_, nb = r["a_mean"].shape[0], r["a_mean"].shape[-1]
             a_mu = r["a_mean"].reshape(its_, d * d, nb)[:, pt]
             a_S = r["a_cov"][:, pt][:, :, pt]
-            post = {"x": MvNormalMeanCovariance(r["mean"], r["cov"]), "a": MvNormalMeanCovariance(a_mu, a_S)}
-            for name in ("p", "q"):
-                if r[f"df_{name}"] is not None:
-                    post[f"w_{name}"] = WishartFast(r[f"df_{name}"], r[f"inv_scale_{name}"])
-            return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
+            return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]),
+                                               "a": MvNormalMeanCovariance(a_mu, a_S), **_noise_posteriors(r)},
+                                   model=model, free_energy=r["free_energy"])
         if isinstance(model, gaussian_mixture):
             check_mean_field(constraints)
             if predictvars is not None:
