@@ -9,6 +9,7 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
   python bench_extra.py --which vmp_noise    (opt-in: learned process precision, alone and with the observation precision)
   python bench_extra.py --which vmp_transition (opt-in: learned transition matrix, alone and with the noise precisions)
   python bench_extra.py --which gmm          (opt-in: Gaussian-mixture VMP, d = 2 / K = 3 and d = 4 / K = 8)
+  python bench_extra.py --which hmm          (opt-in: hidden Markov model VMP, K = M = 3 and K = 8 / M = 16)
 """
 from __future__ import annotations
 
@@ -377,6 +378,35 @@ def bench_gmm(ctx, peak):
         torch.cuda.empty_cache()
 
 
+def bench_hmm(ctx, peak):
+    """Hidden Markov model VMP (rxg_hmm_vmp_f32), T = 1000 steps, 20 iterations, 65 536 chains, A and B learned, free
+    energy on; time from CUDA events around the call (host validation and the constant upload included, both O(M K)).
+    Algorithmic bytes per (chain, step): (2 + 8 K) per iteration (x read twice, the forward stash written and read once)
+    plus 4 K for q(s) written at the end; per step and iteration ~4 K^2 fp32 FMAs (forward, backward, outer product).
+    The symbols are uniform (the sweep's cost does not depend on them)."""
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(19)
+    T, nb, its = 1000, 65536, 20
+    for K, M in ((3, 3), (8, 16)):
+        x = torch.randint(0, M, (T, nb), device="cuda", generator=g, dtype=torch.uint8)
+        rng = np.random.default_rng(K)
+        kw = dict(p0=np.full(K, 1.0 / K), A_prior=np.ones((K, K)) + 4 * np.eye(K), A_init=rng.uniform(0.5, 2.0, (K, K)),
+                  B_prior=np.ones((M, K)), B_init=rng.uniform(0.5, 2.0, (M, K)))
+        runs = [timed(lambda: ctx.hmm_vmp(x, **kw, iterations=its), warm=2, reps=3) for _ in range(3)]
+        ms = float(np.median(runs))
+        by = ((2 + 8 * K) * its + 4 * K) * T * nb
+        fl = 2 * 4 * K * K * its * T * nb
+        t = {"hbm": by / (peak * 1e9), "fp32": fl / 67e12}
+        bound = max(t, key=t.get)
+        print(json.dumps({"what": "hidden Markov model VMP (hmm_vmp_kernel), A and B learned, free energy on", "K": K, "M": M,
+                          "T": T, "batch": nb, "iterations": its, "ms": ms, "ms_runs": runs, "ms_per_iteration": ms / its,
+                          "bytes_per_chain_step": by / (T * nb), "achieved_GBs": by / ms / 1e6, "bound": bound,
+                          "bound_ms": {k: v * 1e3 for k, v in t.items()}, "frac_of_bound": t[bound] * 1e3 / ms,
+                          "peak_hbm_gbs": peak, "peak_fp32_tflops": 67, "gpu": gname, "power_limit": plim}), flush=True)
+        del x
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -396,6 +426,8 @@ def main():
         bench_vmp_transition(ctx, peak)
     if "gmm" in which:
         bench_gmm(ctx, peak)
+    if "hmm" in which:
+        bench_hmm(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

@@ -273,6 +273,27 @@ int rxg_gmm_vmp_f32(rxg_ctx*, int d, int K, int N, int64_t batch, int iterations
                     float* m_mean, float* m_cov, float* w_df, float* w_inv_scale, double* free_energy, float* z_prob,
                     float* hist_alpha, float* hist_m_mean, float* hist_m_cov, float* hist_w_df, float* hist_w_inv_scale,
                     int32_t* status, unsigned flags);
+/* Fused structured VMP of the hidden Markov model, `batch` independent chains, all iterations in one launch:
+ *   A ~ DirichletCollection(A_prior) (K x K, column j = p(s_t | s_{t-1} = j)), B ~ DirichletCollection(B_prior) (M x K,
+ *   column j = p(x_t | s_t = j)), s_0 ~ Categorical(p0), s[t] ~ DiscreteTransition(s[t-1], A), x[t] ~
+ *   DiscreteTransition(s[t], B), q(s, s_0) q(A) q(B), initialised to DirichletCollection(A_init), (B_init)
+ *   [ref: test/models/statespace/hmm_tests.jl:8-45; a known A as in test/inference/inference_tests.jl:2062-2088].  Either
+ *   matrix is learned (prior and init non-NULL, its *_known NULL) or known (*_known, a probability matrix, the other two
+ *   NULL).  Host arrays shared by every chain, row-major [row][column] (row = next state or symbol, column = conditioning
+ *   state): p0[K], A_*[K][K], B_*[M][K].  x[T][batch] uint8 symbols 0..M-1, 255 = missing (a pure transition step).
+ *   Outputs: s_prob[T][K][batch] (q(s_t) of the last iteration; also the forward stash), and optional (NULL = not wanted):
+ *   s0_prob[K][batch], A_alpha[K][K][batch] / B_alpha[M][K][batch] (of a learned matrix), free_energy[iterations][batch]
+ *   (fp64, Bethe free energy after every iteration; -log p(x) with both matrices known), the KeepEach histories
+ *   hist_s[iterations][T][K][batch], hist_A[iterations][K][K][batch], hist_B[iterations][M][K][batch], status[batch]
+ *   (RXG_ERR_BAD_ARG for a chain with a symbol >= M other than 255, read as missing; RXG_ERR_NAN for a chain whose data are
+ *   impossible under its model).  Per iteration: forward-backward with the previous q(A), q(B), then both updated.
+ *   2 <= K <= 8 and 2 <= M <= 16, else RXG_ERR_UNSUPPORTED; T, batch, iterations >= 1, Dirichlet parameters > 0, p0 and
+ *   the columns of a known matrix non-negative with sum 1 (within 1e-5), else RXG_ERR_BAD_ARG.  Device pointers
+ *   (RXG_ERR_UNSUPPORTED otherwise).                                                                                  */
+int rxg_hmm_vmp_f32(rxg_ctx*, int K, int M, int T, int64_t batch, int iterations, const float* p0, const float* A_prior,
+                    const float* A_init, const float* A_known, const float* B_prior, const float* B_init,
+                    const float* B_known, const uint8_t* x, float* s_prob, float* s0_prob, float* A_alpha, float* B_alpha,
+                    double* free_energy, float* hist_s, float* hist_A, float* hist_B, int32_t* status, unsigned flags);
 /* prod(GammaShapeRate, GammaShapeRate) = (a1 + a2 - 1, b1 + b2)                                 */
 int rxg_prod_gamma_f32(rxg_ctx*, int64_t n, const float* a1, const float* b1, const float* a2,
                        const float* b2, float* a, float* b, unsigned flags);

@@ -8,7 +8,7 @@ loudly if it is missing or no GPU is present -- there is no CPU fallback.
 """
 from . import _lib
 from ._lib import RxGaussError
-from .distributions import (Beta, Categorical, Dirichlet, GammaShapeRate, MvNormalMeanCovariance,
+from .distributions import (Beta, Categorical, Dirichlet, DirichletCollection, GammaShapeRate, MvNormalMeanCovariance,
                             MvNormalWeightedMeanPrecision, NormalMeanVariance, PointMass, Wishart, WishartFast, vague)
 
 
@@ -20,6 +20,7 @@ def __getattr__(name):   # lazy: these import torch
                 "hgf", "univariate_lgssm_gamma_precision", "kalman_gamma_streaming", "latent_autoregressive",
                 "linear_gaussian_ssm_wishart_precision", "linear_gaussian_ssm_wishart_noise",
                 "linear_gaussian_ssm_continuous_transition", "gaussian_mixture", "MeanField", "BetheFactorization",
+                "hidden_markov_model", "HMMConstraints",
                 "default_context",
                 "KeepLast", "KeepEach"):
         from . import inference

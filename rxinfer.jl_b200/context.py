@@ -721,6 +721,57 @@ class Context:
         out.update(h)
         return out
 
+    def hmm_vmp(self, x, p0, A_prior=None, A_init=None, A_known=None, B_prior=None, B_init=None, B_known=None,
+                iterations=1, want_free_energy=True, keep_each=False):
+        """Fused structured VMP of the hidden Markov model (``rxg_hmm_vmp_f32``); x[T, batch] uint8 symbols on the device
+        (255 = missing).  p0[K] and each matrix are host arrays shared by every chain, columns = conditionals: A learned
+        (``A_prior`` and ``A_init``, Dirichlet parameters [K, K]) or known (``A_known``, a probability matrix); B likewise
+        with shape [M, K].  Returns ``s_prob[T, K, batch]``, ``s0_prob[K, batch]``, ``A_alpha[K, K, batch]`` /
+        ``B_alpha[M, K, batch]`` (None when known), ``free_energy[iterations, batch]`` (fp64), ``status[batch]`` and, with
+        ``keep_each``, ``hist_s`` / ``hist_A`` / ``hist_B`` with a leading iteration axis."""
+        if not (x.is_cuda and x.dtype == torch.uint8 and x.is_contiguous() and x.dim() == 2):
+            raise ValueError("hmm_vmp: x must be a contiguous uint8 CUDA tensor [T, batch]")
+        if x.device.index != self.device:
+            raise ValueError(f"hmm_vmp: x lives on cuda:{x.device.index}, this context is bound to cuda:{self.device}")
+        T, batch = x.shape
+        K = int(np.asarray(p0).reshape(-1).shape[0])
+        B_any = B_known if B_known is not None else B_prior
+        if B_any is None:
+            raise ValueError("hmm_vmp: pass either B_prior and B_init (B learned) or B_known")
+        M = int(np.asarray(B_any).shape[0])
+        vals = dict(p0=(p0, (K,)), A_prior=(A_prior, (K, K)), A_init=(A_init, (K, K)), A_known=(A_known, (K, K)),
+                    B_prior=(B_prior, (M, K)), B_init=(B_init, (M, K)), B_known=(B_known, (M, K)))
+        keep = {}
+        for k, (v, shp) in vals.items():
+            if v is None:
+                keep[k] = (None, L.as_fp(0))
+                continue
+            a = np.asarray(v, dtype=np.float64)
+            if a.shape != shp:
+                raise ValueError(f"hmm_vmp: {k} must have shape {shp} (K = {K}, M = {M}), got {a.shape}")
+            keep[k] = _model32(a)
+        learn_A, learn_B = A_known is None, B_known is None
+        its = int(iterations)
+        sp, s0 = self.empty(T, K, batch), self.empty(K, batch)
+        Aa = self.empty(K, K, batch) if learn_A else None
+        Ba = self.empty(M, K, batch) if learn_B else None
+        fe = self.empty(its, batch, dtype=torch.float64) if want_free_energy else None
+        h = {}
+        if keep_each:
+            h["hist_s"] = self.empty(its, T, K, batch)
+            h["hist_A"] = self.empty(its, K, K, batch) if learn_A else None
+            h["hist_B"] = self.empty(its, M, K, batch) if learn_B else None
+        st = self.empty(batch, dtype=torch.int32)
+        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
+        self._check(self.lib.rxg_hmm_vmp_f32(self.h, K, M, T, batch, its, *(keep[k][1] for k in vals),
+                                             ctypes.cast(c_void_p(x.data_ptr()), L.u8p), _fp(sp), _fp(s0), _fp(Aa),
+                                             _fp(Ba), fe_p, _fp(h.get("hist_s")), _fp(h.get("hist_A")),
+                                             _fp(h.get("hist_B")), ctypes.cast(c_void_p(st.data_ptr()), L.i32p),
+                                             L.PTR_DEVICE))
+        out = dict(s_prob=sp, s0_prob=s0, A_alpha=Aa, B_alpha=Ba, free_energy=fe, status=st)
+        out.update(h)
+        return out
+
     def prod_gamma(self, a1, b1, a2, b2):
         return self._six(self.lib.rxg_prod_gamma_f32, a1, b1, a2, b2)
 

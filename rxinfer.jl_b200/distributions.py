@@ -119,6 +119,21 @@ class Beta:
 
 
 @dataclass
+class DirichletCollection:
+    """``DirichletCollection(alpha)``: a matrix whose columns are independent Dirichlets (column j is the distribution
+    conditioned on state j).  ``alpha[R, C]`` (host, a prior or an initial marginal) or ``alpha[..., R, C, n]``
+    (posteriors)."""
+    alpha: object
+
+    def mean(self):
+        a = self.alpha
+        if isinstance(a, torch.Tensor):
+            return a / a.sum(dim=-3, keepdim=True)
+        a = np.asarray(a, np.float64)
+        return a / a.sum(axis=0, keepdims=True)
+
+
+@dataclass
 class Categorical:
     """``Categorical(p)``: ``p[..., K, n]``."""
     p: torch.Tensor
@@ -129,7 +144,8 @@ class Categorical:
 
 def vague(kind, like=None):
     """``vague(NormalMeanVariance)`` = N(0, 1e12); ``vague(GammaShapeRate)`` = Gamma(1, 1e-12)
-    (TinyHugeNumbers, upstream); ``vague(Beta)`` = Beta(1, 1); ``vague(Dirichlet, K)`` = Dirichlet(ones(K)).
+    (TinyHugeNumbers, upstream); ``vague(Beta)`` = Beta(1, 1); ``vague(Dirichlet, K)`` = Dirichlet(ones(K));
+    ``vague(DirichletCollection, (R, C))`` = DirichletCollection(ones(R, C)); ``vague(Categorical, K)`` = uniform.
     With a tensor ``like`` the parameters are tensors shaped like it, else host floats."""
     if kind is Beta:
         return Beta(1.0, 1.0)
@@ -137,6 +153,14 @@ def vague(kind, like=None):
         if not isinstance(like, (int, np.integer)) or like < 1:
             raise TypeError("vague(Dirichlet, K) needs the number of components K")
         return Dirichlet(np.ones(int(like)))
+    if kind is DirichletCollection:
+        if not (isinstance(like, tuple) and len(like) == 2 and all(isinstance(n, (int, np.integer)) and n >= 1 for n in like)):
+            raise TypeError("vague(DirichletCollection, (R, C)) needs the matrix shape")
+        return DirichletCollection(np.ones(like))
+    if kind is Categorical:
+        if not isinstance(like, (int, np.integer)) or like < 1:
+            raise TypeError("vague(Categorical, K) needs the number of categories K")
+        return Categorical(np.full(int(like), 1.0 / int(like)))
     if like is None:
         if kind is NormalMeanVariance:
             return NormalMeanVariance(0.0, 1e12)

@@ -18,8 +18,8 @@ import torch
 
 from . import _lib as L
 from .context import Context
-from .distributions import (Beta, Categorical, Dirichlet, GammaShapeRate, MvNormalMeanCovariance, NormalMeanVariance, Wishart,
-                            WishartFast)
+from .distributions import (Beta, Categorical, Dirichlet, DirichletCollection, GammaShapeRate, MvNormalMeanCovariance,
+                            NormalMeanVariance, PointMass, Wishart, WishartFast)
 
 
 # --------------------------------------------------------------------------- recognised models
@@ -254,6 +254,82 @@ def check_mean_field(constraints):
                          "q(z) q(s) q(m[1]) ... q(m[K]) q(w[1]) ... q(w[K]); pass constraints = MeanField()")
 
 
+@dataclass
+class hidden_markov_model:
+    """Hidden Markov model (RxInfer test/models/statespace/hmm_tests.jl:8-20): ``s_0 ~ Categorical(p0)``,
+    ``s[t] ~ DiscreteTransition(s[t-1], A)``, ``x[t] ~ DiscreteTransition(s[t], B)``.  ``A`` (K x K) and ``B`` (M x K) are
+    each a ``DirichletCollection`` prior (learned) or a ``PointMass`` probability matrix (known); column j is the
+    distribution conditioned on state j.  Run with ``constraints = HMMConstraints()``, ``initialization = {"A": q(A),
+    "B": q(B)}`` (``DirichletCollection``, for the learned ones; an ``"s"`` entry is accepted and not needed: every
+    iteration starts with the chain) and ``data = {"x": ...}``."""
+    p0: object
+    A: object
+    B: object
+
+
+class HMMConstraints:
+    """``q(s, s_0, A, B) = q(s, s_0) q(A) q(B)`` (hmm_tests.jl:22-24): the chain is kept structured, the matrices apart."""
+
+    def __eq__(self, other):
+        return isinstance(other, HMMConstraints)
+
+    def __hash__(self):
+        return hash(HMMConstraints)
+
+
+def check_hmm_constraints(constraints):
+    if not isinstance(constraints, HMMConstraints):
+        raise ValueError("hidden_markov_model runs the structured factorisation q(s, s_0) q(A) q(B) only; pass "
+                         f"constraints = HMMConstraints() (got {constraints!r})")
+
+
+def hmm_symbols(x, M):
+    """The observations as symbols: a uint8 index tensor [T, batch] (255 = missing) as it is, or a one-hot float tensor
+    [T, M, batch] as the reference passes it (a NaN row is missing).  Soft observations are refused."""
+    if x.dtype == torch.uint8:
+        if x.dim() != 2:
+            raise ValueError(f"data['x'] as symbols must be [T, batch], got {tuple(x.shape)}")
+        return x
+    if x.dim() != 3 or x.shape[1] != M:
+        raise ValueError(f"data['x'] as one-hot vectors must be [T, M = {M}, batch], got {tuple(x.shape)}")
+    miss = torch.isnan(x).any(dim=1)
+    xx = torch.where(torch.isnan(x), torch.zeros_like(x), x)
+    one_hot = ((xx == 0) | (xx == 1)).all(dim=1) & (xx.sum(dim=1) == 1)
+    if not bool((one_hot | miss).all()):
+        raise ValueError("data['x'] must hold one-hot rows (or NaN for a missing step): soft observations are outside the "
+                         "batched hot path")
+    sym = xx.argmax(dim=1).to(torch.uint8)
+    sym[miss] = 255
+    return sym.contiguous()
+
+
+def hmm_arguments(model, initialization):
+    """The keyword arguments of ``Context.hmm_vmp`` for ``model`` and ``initialization``."""
+    p0 = np.asarray(model.p0.p if isinstance(model.p0, Categorical) else model.p0, np.float64).reshape(-1)
+    K = p0.shape[0]
+    init = initialization or {}
+    out = {"p0": p0}
+    for name in ("A", "B"):
+        v = getattr(model, name)
+        if isinstance(v, PointMass):
+            out[f"{name}_known"] = np.asarray(v.value, np.float64)
+            shape = out[f"{name}_known"].shape
+        elif isinstance(v, DirichletCollection):
+            if not isinstance(init.get(name), DirichletCollection):
+                raise ValueError(f"{name} is learned: pass initialization = {{'{name}': DirichletCollection(...)}}, e.g. "
+                                 f"vague(DirichletCollection, {np.asarray(v.alpha).shape})")
+            out[f"{name}_prior"] = np.asarray(v.alpha, np.float64)
+            out[f"{name}_init"] = np.asarray(init[name].alpha, np.float64)
+            shape = out[f"{name}_prior"].shape
+            if out[f"{name}_init"].shape != shape:
+                raise ValueError(f"initialization['{name}'] has shape {out[f'{name}_init'].shape}, the prior {shape}")
+        else:
+            raise TypeError(f"model.{name}: expected DirichletCollection or PointMass, got {type(v).__name__}")
+        if len(shape) != 2 or shape[1] != K or (name == "A" and shape[0] != K):
+            raise ValueError(f"model.{name} has shape {shape}; with K = {K} states A is K x K and B is M x K")
+    return out
+
+
 def vec_order(d):
     """perm with row_major = col_major[perm] (and col_major = row_major[perm]: a transpose is an involution) for vec(A)
     of a d x d matrix: Julia's vec is column-major, the C ABI's a[i * d + j] = A[i, j] row-major."""
@@ -380,6 +456,45 @@ def _noise_posteriors(r):
             if r[f"df_{name}"] is not None}
 
 
+def _infer_hmm(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars, context,
+               catch_exception):
+    """``infer`` of ``hidden_markov_model``: one ``rxg_hmm_vmp_f32`` launch.  ``returnvars`` is KeepLast() / KeepEach() for
+    every variable or a dict over ``s``, ``A``, ``B``; ``s_0`` is the last iteration's."""
+    check_hmm_constraints(constraints)
+    if predictvars is not None:
+        raise NotImplementedError("predictvars: predictions of the hidden Markov model are outside the batched hot path")
+    if data is None or "x" not in data:
+        raise KeyError("hidden_markov_model needs data = {'x': observations}")
+    if isinstance(returnvars, dict):
+        bad = set(returnvars) - {"s", "A", "B", "s_0"}
+        if bad or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
+            raise NotImplementedError(f"returnvars={returnvars!r}: KeepEach() / KeepLast() of s, A, B (and KeepLast() of s_0)")
+        each = {k for k, v in returnvars.items() if isinstance(v, KeepEach)}
+        if "s_0" in each:
+            raise NotImplementedError("returnvars: q(s_0) is kept for the last iteration only (KeepLast)")
+    elif returnvars is None or isinstance(returnvars, (KeepEach, KeepLast)):
+        each = {"s", "A", "B"} if isinstance(returnvars, KeepEach) else set()
+    else:
+        raise NotImplementedError(f"returnvars={returnvars!r}: the hidden Markov model returns KeepEach() or KeepLast()")
+    args = hmm_arguments(model, initialization)
+    M = (args["B_known"] if "B_known" in args else args["B_prior"]).shape[0]
+    x = hmm_symbols(torch.as_tensor(data["x"]), M)
+    try:
+        ctx = context or default_context()
+        x = x.to(f"cuda:{ctx.device}").contiguous()
+        r = ctx.hmm_vmp(x, **args, iterations=iterations or 1, want_free_energy=bool(free_energy), keep_each=bool(each))
+        _raise_flagged(r["status"], "hidden_markov_model: ", " (BAD_ARG: a symbol >= M; NAN: data impossible under the model)")
+        post = {"s": Categorical(r["hist_s"] if "s" in each else r["s_prob"]), "s_0": Categorical(r["s0_prob"])}
+        for name in ("A", "B"):
+            if r[f"{name}_alpha"] is not None:
+                post[name] = DirichletCollection(r[f"hist_{name}"] if name in each else r[f"{name}_alpha"])
+        return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
+    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
+        if catch_exception:
+            return InferenceResult(posteriors={}, model=model, error=e)
+        raise
+
+
 def infer(*, model, iterations=None, free_energy=False, returnvars=None, options=None,
           initialization=None, autoupdates=None, keephistory=None, historyvars=None,
           catch_exception=False, showprogress=False, session=None, warn=True, allow_node_contraction=False,
@@ -391,7 +506,7 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
     With ``datastream=`` (an iterable of time-chunks, or ``None`` + ``autoupdates`` for a push-driven
     engine) the call returns an ``RxInferenceEngine`` (streaming.py), as the reference does when
     ``autoupdates`` is given (/root/reference/src/inference/inference.jl:577-733 dispatch)."""
-    constraints = kwargs.pop("constraints", None) if isinstance(model, gaussian_mixture) else None
+    constraints = kwargs.pop("constraints", None) if isinstance(model, (gaussian_mixture, hidden_markov_model)) else None
     for k in kwargs:
         if k in _UNSUPPORTED:
             raise NotImplementedError(
@@ -404,6 +519,9 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             raise NotImplementedError(f"options {sorted(bad)} are outside the batched hot path")
     if data is not None and datastream is not None:
         raise ValueError("`data` and `datastream` are mutually exclusive")    # reference: inference.jl argument check
+    if isinstance(model, hidden_markov_model):
+        return _infer_hmm(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
+                          context, catch_exception)
     if isinstance(model, (linear_gaussian_ssm_wishart_precision, linear_gaussian_ssm_wishart_noise,
                           linear_gaussian_ssm_continuous_transition)):
         if predictvars is not None:

@@ -249,6 +249,12 @@ gmm_vmp(ctx, d, K, N, batch, its, a0, mu0, V0, nu0, S0, ai, mi, Vi, nui, Si, y, 
         ctx.handle, d, K, N, batch, its, a0, mu0, V0, nu0, S0, ai, mi, Vi, nui, Si, y, al, mm, mc, df, iS, fe, z, hal, hmm, hmc, hdf,
         hiS, st, fl))
 
+hmm_vmp(ctx, K, M, T, batch, its, p0, Ap, Ai, Ak, Bp, Bi, Bk, x, sp, s0, Aa, Ba, fe, hs, hA, hB, st, fl) =
+    check(ctx, ccall((:rxg_hmm_vmp_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{UInt8}, F32P, F32P, F32P, F32P,
+         Ptr{Float64}, F32P, F32P, F32P, Ptr{Int32}, Cuint),
+        ctx.handle, K, M, T, batch, its, p0, Ap, Ai, Ak, Bp, Bi, Bk, x, sp, s0, Aa, Ba, fe, hs, hA, hB, st, fl))
+
 # ---- diagnostics
 selftest_umma(ctx, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_f32, LIB), Cint, (Ptr{Cvoid}, F32P, F32P, F32P, Cuint), ctx.handle, A, B, D, fl))
 selftest_umma_shape(ctx, n, k, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_shape_f32, LIB), Cint, (Ptr{Cvoid}, Cint, Cint, F32P, F32P, F32P, Cuint), ctx.handle, n, k, A, B, D, fl))
@@ -868,6 +874,43 @@ function gaussian_mixture(ctx::Context, y::Array{Float32, 3}; alpha0, mu0, V0, n
     Lib.device_free(ctx, fe)
     return (s = download(hal), m_mean = download(hmm), m_cov = download(hmc), w_df = download(hdf), w_inv_scale = download(hiS),
             z = download(z), free_energy = fe_host, status = reinterpret(Int32, download(st)))
+end
+
+"""Fused structured VMP of the hidden Markov model (hmm_tests.jl:8-45, `rxg_hmm_vmp_f32`); `x[batch, T]` UInt8 symbols 0..M-1
+(255 = missing; one-hot data convert with `argmax(v) - 1`, Julia's argmax being 1-based).  `p0` is a `K` vector; `A` (K x K)
+and `B` (M x K) are each either learned, `(prior = alpha0, init = alpha_init)` with Dirichlet parameter matrices, or known, a
+probability matrix; column j is the distribution conditioned on state j, as `A * s_prev` in the reference (converted to the
+C ABI's row-major layout here, inputs and outputs alike).  Returns the KeepEach posteriors (trailing iteration axis): q(s)
+`[batch, K, T, its]` (the last slot is the last iteration's q(s); the ABI's required `s_prob` buffer is only the sweep's
+stash here and is not downloaded), the Dirichlet parameters of the learned matrices `[batch, K, K, its]` /
+`[batch, M, K, its]` with entry `[b, i, j, n]` = alpha[i, j] (row i, column j, as the prior) (`nothing` when known), q(s_0)
+`[batch, K]`, the Bethe free energy `[batch, its]` (Float64) and the per-chain status."""
+function hidden_markov_model(ctx::Context, x::Matrix{UInt8}; p0, A, B, iterations = 20)
+    batch, T = size(x)
+    K = length(p0)
+    M = B isa NamedTuple ? size(B.prior, 1) : size(B, 1)
+    dx = Lib.device_alloc(ctx, sizeof(x))
+    GC.@preserve x Lib.memcpy_h2d(ctx, dx, Ptr{Cvoid}(pointer(x)), sizeof(x))
+    sp, s0 = DeviceArray(ctx, batch, K, T), DeviceArray(ctx, batch, K)
+    hs = DeviceArray(ctx, batch, K, T, iterations)
+    # C layout [its][row][col][batch] = Julia dims (batch, col, row, its): permuted to (batch, row, col, its) on the way out
+    hA = A isa NamedTuple ? DeviceArray(ctx, batch, K, K, iterations) : nothing
+    hB = B isa NamedTuple ? DeviceArray(ctx, batch, K, M, iterations) : nothing
+    st = DeviceArray(ctx, batch)
+    fe = Lib.device_alloc(ctx, 8 * batch * iterations)
+    side(P) = P isa NamedTuple ? (rowmajor32(P.prior), rowmajor32(P.init), nothing) : (nothing, nothing, rowmajor32(P))
+    h = (Float32.(collect(p0)), side(A)..., side(B)...)
+    ptr(v) = v === nothing ? NULLF : pointer(v)
+    GC.@preserve h Lib.hmm_vmp(ctx, K, M, T, batch, iterations, (ptr(v) for v in h)..., Ptr{UInt8}(dx), sp.ptr, s0.ptr, NULLF,
+                               NULLF, Ptr{Float64}(fe), hs.ptr, hA === nothing ? NULLF : hA.ptr,
+                               hB === nothing ? NULLF : hB.ptr, Ptr{Int32}(st.ptr), RXG_PTR_DEVICE)
+    fe_host = Array{Float64}(undef, batch, iterations)
+    GC.@preserve fe_host Lib.memcpy_d2h(ctx, pointer(fe_host), fe, 8 * batch * iterations)
+    Lib.device_free(ctx, fe)
+    Lib.device_free(ctx, dx)
+    rowcol(d) = d === nothing ? nothing : permutedims(download(d), (1, 3, 2, 4))
+    return (s = download(hs), A = rowcol(hA), B = rowcol(hB),
+            s_0 = download(s0), free_energy = fe_host, status = reinterpret(Int32, download(st)))
 end
 
 # ---------------------------------------------------------------------------------------------- 4. pattern recogniser + infer_batched
