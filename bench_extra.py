@@ -10,6 +10,7 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
   python bench_extra.py --which vmp_transition (opt-in: learned transition matrix, alone and with the noise precisions)
   python bench_extra.py --which gmm          (opt-in: Gaussian-mixture VMP, d = 2 / K = 3 and d = 4 / K = 8)
   python bench_extra.py --which hmm          (opt-in: hidden Markov model VMP, K = M = 3 and K = 8 / M = 16)
+  python bench_extra.py --which hgf_learn    (opt-in: HGF with learned kappa, omega, T = 1000, 20 iterations)
 """
 from __future__ import annotations
 
@@ -407,6 +408,40 @@ def bench_hmm(ctx, peak):
         torch.cuda.empty_cache()
 
 
+def bench_hgf_learn(ctx, peak):
+    """HGF with learned kappa and omega (rxg_hgf_vmp_learn_f32), T = 1000 steps, 20 iterations, 65 536 chains, free energy
+    on; time from CUDA events around the call.  Per (chain, step, iteration): 36 bytes (y read, the old q(x_t+1), q(z_t+1)
+    read and the new q(x_t), q(z_t) written).  MUFU operations, an ESTIMATE counted from the source, not from the SASS:
+    three GH-31 products of 62 ex2 each (31 for exp(c z + d z^2 / 2), 31 for the weights), 3 expf of B, 3 square roots,
+    6 reciprocals (x, the z product and its Gaussian factor, the two fp64 folds' seeds) and, with the free energy, 2 exp,
+    4 log and 2 divisions: ~206.  The two folds sum their moments in fp64, ~3 DFMA per node: ~190 DFMA.  The SFU bound takes
+    16 MUFU results per clock per SM at the card's maximum SM clock; FP64 at 34 TFLOP/s (data sheet, H100 SXM)."""
+    gname, plim = gpu_name_and_power_limit()
+    props = torch.cuda.get_device_properties(0)
+    sm = props.multi_processor_count
+    q = subprocess.run(["nvidia-smi", "--query-gpu=clocks.max.sm", "--format=csv,noheader,nounits"], capture_output=True,
+                       text=True).stdout.split()
+    clk, clk_src = (float(q[0]) * 1e6, "nvidia-smi") if q else (1980e6, "data sheet boost clock, not read")
+    T, nb, its = 1000, 65536, 20
+    from oracle.hgf import generate_data
+    _, _, y = generate_data(T, 1024, kappa=0.8, omega=-0.5, z_variance=0.01, y_variance=0.2, seed=3)
+    y = torch.as_tensor(np.tile(y, (1, nb // 1024)), device="cuda").contiguous()
+    runs = [timed(lambda: ctx.hgf_vmp_learn(y, iterations=its), warm=1, reps=2) for _ in range(3)]
+    ms = float(np.median(runs))
+    n = T * nb * its
+    by, mufu, fl, dfma = 36 * n, 206 * n, 3 * 31 * 8 * n, 190 * n
+    t = {"hbm": by / (peak * 1e9), "sfu_estimate": mufu / (16 * sm * clk), "fp32": fl / 67e12, "fp64": 2 * dfma / 34e12}
+    bound = max(t, key=t.get)
+    st = ctx.hgf_vmp_learn(y, iterations=its)["status"]
+    print(json.dumps({"what": "HGF with learned kappa, omega (hgf_learn_kernel), free energy on", "T": T, "batch": nb,
+                      "iterations": its, "ms": ms, "ms_runs": runs, "ms_per_iteration": ms / its, "bytes_per_chain_step": 36,
+                      "achieved_GBs": by / ms / 1e6, "bound": bound, "bound_ms": {k: v * 1e3 for k, v in t.items()},
+                      "frac_of_bound": t[bound] * 1e3 / ms, "flagged_chains": int((st != 0).sum()), "peak_hbm_gbs": peak,
+                      "sm_count": sm, "max_sm_clock_mhz": clk / 1e6, "clock_source": clk_src, "gpu": gname, "power_limit": plim}), flush=True)
+    del y
+    torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -428,6 +463,8 @@ def main():
         bench_gmm(ctx, peak)
     if "hmm" in which:
         bench_hmm(ctx, peak)
+    if "hgf_learn" in which:
+        bench_hgf_learn(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

@@ -481,6 +481,24 @@ int rxg_hgf_filter_f32(rxg_ctx*, int T, int64_t batch, int iters, float kappa, f
 int rxg_hgf_filter_fe_f32(rxg_ctx*, int T, int64_t batch, int iters, float kappa, float omega,
                           float z_variance, float y_variance, const float init[4], const float* prev,
                           const float* y, float* out, float* free_energy, unsigned flags);
+/* Hierarchical Gaussian Filter with the coupling kappa and the volatility offset omega LEARNED per series: mean-field VMP
+ * over whole series, `batch` independent chains, all iterations in one launch
+ * [ref: model `hgf_1`, test/inference/inference_tests.jl:609-642 (MeanField(), free_energy = true, initialisation
+ *  :624-629); GCV rules and average energy :547-607, variance exp(kappa z + omega)]:
+ *   omega ~ N(prior[2], prior[3]), kappa ~ N(prior[0], prior[1]), x_0 ~ N(prior[4], prior[5]), z[1] ~ N(prior[6], prior[7]),
+ *   z[t] ~ N(z[t-1], precision z_precision) (t >= 2), x[t] ~ GCV(x[t-1], z[t], kappa, omega), y[t] ~ N(x[t], y_variance),
+ *   q(kappa) q(omega) q(x_0) prod q(x[t]) q(z[t]).  prior (HOST, 8 floats: mean, variance of kappa, omega, x_0, z[1]);
+ *   init (HOST, 8 floats: mean, variance of the initial q(kappa), q(omega), q(z[t]), q(x[t]), the last two for every t).
+ *   y[T][batch], NaN = missing step.  Outputs: xz[T][4][batch] = (m_x, v_x, m_z, v_z) of the last iteration (KeepLast),
+ *   kw[2][2][batch] = (mean, variance) of q(kappa), then of q(omega); optional (NULL = not wanted): x0[2][batch] = q(x_0),
+ *   hist_kw[iterations][2][2][batch] (KeepEach of q(kappa), q(omega)), free_energy[iterations][batch] (fp64, the
+ *   mean-field VMP free energy after every iteration), status[batch] (RXG_ERR_NAN for a chain whose update met a
+ *   non-finite value).  Products with the GCV node's ExponentialLinearQuadratic messages are GH-31 moment matching
+ *   (DESIGN.md section 3.19).  T, batch, iterations >= 1, positive finite variances and z_precision, finite means,
+ *   else RXG_ERR_BAD_ARG.  Device pointers (RXG_ERR_UNSUPPORTED otherwise).                                        */
+int rxg_hgf_vmp_learn_f32(rxg_ctx*, int T, int64_t batch, int iterations, const float prior[8], float z_precision,
+                          float y_variance, const float init[8], const float* y, float* x0, float* xz, float* kw,
+                          float* hist_kw, double* free_energy, int32_t* status, unsigned flags);
 
 /* ------------------------------------------------------------------ streaming engine ----------
  * The reference's second entry point: infer(..., autoupdates = ..., keephistory = ...) builds an

@@ -94,6 +94,8 @@ SIGNATURES = {
                                              i32p, c_uint]),
     "rxg_hgf_filter_f32": (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_float, c_float, c_float, fp, fp, fp, c_uint]),
     "rxg_hgf_filter_fe_f32": (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_float, c_float, c_float, fp, fp, fp, fp, fp, c_uint]),
+    "rxg_hgf_vmp_learn_f32": (c_int, [c_void_p, c_int, c_int64, c_int, fp, c_float, c_float, fp, fp, fp, fp, fp, fp,
+                                      POINTER(c_double), i32p, c_uint]),
     "rxg_lgssm_filter_chunk_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, c_uint]),
     "rxg_hgf_filter_chunk_f32": (c_int, [c_void_p, c_int, c_int64, c_int, c_float, c_float, c_float, c_float, fp, fp, fp, c_uint]),
     "rxg_stream_vmp_gamma_f32": (c_int, [c_void_p, c_int, c_int64, c_int, c_float, fp, fp, fp, fp, fp, c_uint]),

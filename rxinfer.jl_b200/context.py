@@ -289,6 +289,36 @@ class Context:
                                                         _fp(mean), _fp(cov), _fp(nle), flags))
         return dict(mean=mean, cov=cov, neg_log_evidence=nle)
 
+    HGF_LEARN_PRIOR = (1.0, 1.0, 0.0, 1.0, 0.0, 1.0, 0.0, 1.0)   # hgf_1: kappa, omega, x_0, z[1] ~ N(mean, variance)
+    HGF_LEARN_INIT = (1.0, 1.0, 0.0, 1.0, 0.0, 1.0, 0.0, 1.0)    # initial q(kappa), q(omega), q(z), q(x)
+
+    def hgf_vmp_learn(self, y, prior=HGF_LEARN_PRIOR, z_precision=1.0, y_variance=1.0, init=HGF_LEARN_INIT, iterations=1,
+                      want_free_energy=True, keep_each=False):
+        """``rxg_hgf_vmp_learn_f32``: mean-field VMP of the HGF with kappa and omega learned per series.  y[T, batch] fp32
+        on the device (NaN = missing step); ``prior`` = (mean, variance) of kappa, omega, x_0, z[1]; ``init`` = (mean,
+        variance) of the initial q(kappa), q(omega), q(z[t]), q(x[t]).  Returns ``xz[T, 4, batch]`` = (m_x, v_x, m_z, v_z),
+        ``x0[2, batch]``, ``kw[2, 2, batch]`` = (mean, variance) of q(kappa) then q(omega), ``free_energy[iterations,
+        batch]`` (fp64) or None, ``status[batch]`` and, with ``keep_each``, ``hist_kw[iterations, 2, 2, batch]``."""
+        if not (y.is_cuda and y.dtype == torch.float32 and y.is_contiguous() and y.dim() == 2):
+            raise ValueError("hgf_vmp_learn: y must be a contiguous float32 CUDA tensor [T, batch]")
+        if y.device.index != self.device:
+            raise ValueError(f"hgf_vmp_learn: y lives on cuda:{y.device.index}, this context is bound to cuda:{self.device}")
+        T, batch = y.shape
+        pr, ini = np.asarray(prior, np.float32).reshape(-1), np.asarray(init, np.float32).reshape(-1)
+        if pr.shape != (8,) or ini.shape != (8,):
+            raise ValueError("hgf_vmp_learn: prior and init are 8 numbers each ((mean, variance) of four variables)")
+        its = int(iterations)
+        xz, x0, kw = self.empty(T, 4, batch), self.empty(2, batch), self.empty(2, 2, batch)
+        hist = self.empty(its, 2, 2, batch) if keep_each else None
+        fe = self.empty(its, batch, dtype=torch.float64) if want_free_energy else None
+        st = self.empty(batch, dtype=torch.int32)
+        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
+        self._check(self.lib.rxg_hgf_vmp_learn_f32(self.h, T, batch, its, pr.ctypes.data_as(L.fp), float(z_precision),
+                                                   float(y_variance), ini.ctypes.data_as(L.fp), _fp(y), _fp(x0), _fp(xz),
+                                                   _fp(kw), _fp(hist), fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p),
+                                                   L.PTR_DEVICE))
+        return dict(xz=xz, x0=x0, kw=kw, hist_kw=hist, free_energy=fe, status=st)
+
     def hgf_filter_chunk(self, y, prev, iters=20, kappa=1.0, omega=0.0, z_variance=0.04, y_variance=0.01, out=None,
                          want_free_energy=False):
         """HGF datastream chunk; ``prev[4, batch]`` = ``out[-1]`` of the previous chunk."""

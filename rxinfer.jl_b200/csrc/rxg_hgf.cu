@@ -22,7 +22,7 @@ __constant__ float c_gh_lw2[31];  // log2 weights (for the ex2-based inner loop)
 // Gauss-Hermite nodes/weights by Newton iteration on the orthonormal recurrence (host, fp64): the textbook scheme
 // (Press et al., Numerical Recipes, `gauher`; the starting guesses 1.85575 / 1.14 / 0.426 / 1.86 / 1.91 are that routine's).
 // Third-party algorithm, not from the reference -- ReactiveMP's GaussHermiteCubature takes its nodes from FastGaussQuadrature.
-static void gauss_hermite_31(double* t, double* w) {
+void gauss_hermite_31(double* t, double* w) {
     const int n = 31;
     const double pim4 = 0.7511255444649425;
     double z = 0, z1, pp = 0;

@@ -20,6 +20,7 @@ struct rxg_ctx {
     long long launches = 0;
     int sm_count = 132;
     bool gh_ready = false;
+    bool gh_learn_ready = false;    // the Gauss-Hermite table of rxg_hgf_learn.cu uploaded to this device
     // optional per-kernel timing of the last fused sweep (bench.py roofline leg)
     bool profile = false;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // gain start, main start, main end, (spare)   // Gauss-Hermite tables uploaded to this device's constant memory
@@ -72,6 +73,8 @@ void* workspace(rxg_ctx* ctx, size_t bytes);
 // symmetric positive definite (or not finite); log det on success
 bool host_spd_inv(const float* a, int n, double* inv, double* logdet);
 void* staging(rxg_ctx* ctx, size_t bytes);
+// rxg_hgf.cu: the 31 Gauss-Hermite nodes and weights (physicists' convention), fp64
+void gauss_hermite_31(double* t, double* w);
 void* predict_scratch(rxg_ctx* ctx, size_t bytes);
 // device word that gain kernels OR a 1 into when a Cholesky pivot is non-positive (cleared by begin_bad_flag)
 int* bad_flag(rxg_ctx* ctx);

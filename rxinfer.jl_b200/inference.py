@@ -330,6 +330,35 @@ def hmm_arguments(model, initialization):
     return out
 
 
+@dataclass
+class hgf_offline:
+    """``@model hgf_1`` (/root/reference/test/inference/inference_tests.jl:609-622) with every hyper-parameter a number:
+    ``ω ~ N(ω_prior)``, ``κ ~ N(κ_prior)``, ``x_0 ~ N(x0_prior)``, ``z[1] ~ N(z1_prior)`` ((mean, variance) each),
+    ``z[t] ~ NormalMeanPrecision(z[t-1], z_precision)``, ``x[t] ~ GCV(x[t-1], z[t], κ, ω)`` (variance exp(κ z + ω)),
+    ``y[t] ~ NormalMeanVariance(x[t], y_variance)``.  κ and ω are learned per series.  Run with ``constraints =
+    MeanField()``, ``initialization = {"κ": ..., "ω": ..., "z": ..., "x": ...}`` (``NormalMeanVariance`` of scalars, as at
+    :624-629) and ``data = {"y": [T, batch]}`` (NaN = missing)."""
+    κ_prior: tuple = (1.0, 1.0)
+    ω_prior: tuple = (0.0, 1.0)
+    x0_prior: tuple = (0.0, 1.0)
+    z1_prior: tuple = (0.0, 1.0)
+    z_precision: float = 1.0
+    y_variance: float = 1.0
+
+
+def hgf_offline_arguments(model, initialization):
+    """The ``prior`` and ``init`` arrays of ``Context.hgf_vmp_learn`` for ``model`` and ``initialization``."""
+    init = initialization or {}
+    missing = [k for k in ("κ", "ω", "z", "x") if not isinstance(init.get(k), NormalMeanVariance)]
+    if missing:
+        raise ValueError(f"hgf_offline needs initialization = {{'κ', 'ω', 'z', 'x'}} as NormalMeanVariance; missing or not "
+                         f"Normal: {missing}")
+    scalar = lambda d: (float(np.asarray(d.m)), float(np.asarray(d.v)))
+    prior = [float(v) for p in (model.κ_prior, model.ω_prior, model.x0_prior, model.z1_prior) for v in p]
+    return dict(prior=prior, init=[v for k in ("κ", "ω", "z", "x") for v in scalar(init[k])],
+                z_precision=float(model.z_precision), y_variance=float(model.y_variance))
+
+
 def vec_order(d):
     """perm with row_major = col_major[perm] (and col_major = row_major[perm]: a transpose is an involution) for vec(A)
     of a d x d matrix: Julia's vec is column-major, the C ABI's a[i * d + j] = A[i, j] row-major."""
@@ -371,6 +400,7 @@ class InferenceResult:
     error: object = None
     history: dict = field(default_factory=dict)
     predictions: dict = field(default_factory=dict)
+    status: object = None       # per-chain RXG_* codes of a family that returns flagged chains instead of raising
 
 
 _UNSUPPORTED = ("constraints", "meta", "callbacks", "annotations", "events", "uselock",
@@ -495,6 +525,52 @@ def _infer_hmm(model, data, constraints, initialization, iterations, free_energy
         raise
 
 
+def _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
+                       datastream, context, catch_exception):
+    """``infer`` of ``hgf_offline``: one ``rxg_hgf_vmp_learn_f32`` launch.  ``returnvars``: KeepLast() for x, z (and x_0),
+    KeepEach() or KeepLast() for κ, ω.  A chain whose GH products collapse (DESIGN 3.19) is flagged RXG_ERR_NAN in
+    ``result.status[batch]`` and its posteriors are not meaningful; the call does not raise for it, since at large batches
+    a few such chains are expected and the others' results stand."""
+    if not isinstance(constraints, MeanField):
+        raise ValueError(f"hgf_offline runs the naive mean-field factorisation only; pass constraints = MeanField() "
+                         f"(got {constraints!r})")
+    if predictvars is not None:
+        raise NotImplementedError("predictvars: predictions of the HGF are outside the batched hot path")
+    if datastream is not None or data is None:
+        raise NotImplementedError("hgf_offline runs over whole series: pass data = {'y': [T, batch]} (no datastream)")
+    if "y" not in data:
+        raise KeyError("hgf_offline needs data = {'y': observations}")
+    if isinstance(returnvars, dict):
+        bad = set(returnvars) - {"x", "z", "x_0", "κ", "ω"}
+        if bad or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
+            raise NotImplementedError(f"returnvars={returnvars!r}: KeepLast() of x, z, x_0 and KeepEach() / KeepLast() of κ, ω")
+        each = {k for k, v in returnvars.items() if isinstance(v, KeepEach)}
+        if each - {"κ", "ω"}:
+            raise NotImplementedError("returnvars: q(x), q(z), q(x_0) are kept for the last iteration only (KeepLast)")
+    elif returnvars is None or isinstance(returnvars, KeepLast):
+        each = set()
+    else:
+        raise NotImplementedError(f"returnvars={returnvars!r}: pass KeepLast() or a dict with KeepEach() for κ, ω only")
+    args = hgf_offline_arguments(model, initialization)
+    try:
+        ctx = context or default_context()
+        y = torch.as_tensor(data["y"]).to(device=f"cuda:{ctx.device}", dtype=torch.float32).contiguous()
+        if y.dim() != 2:
+            raise ValueError(f"data['y'] must be [T, batch], got {tuple(y.shape)}")
+        r = ctx.hgf_vmp_learn(y, **args, iterations=iterations or 1, want_free_energy=bool(free_energy),
+                              keep_each=bool(each))
+        post = {"x": NormalMeanVariance(r["xz"][:, 0], r["xz"][:, 1]), "z": NormalMeanVariance(r["xz"][:, 2], r["xz"][:, 3]),
+                "x_0": NormalMeanVariance(r["x0"][0], r["x0"][1])}
+        for i, name in enumerate(("κ", "ω")):
+            q = r["hist_kw"] if name in each else r["kw"]     # KeepEach: a leading iteration axis
+            post[name] = NormalMeanVariance(q[..., i, 0, :], q[..., i, 1, :])
+        return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"], status=r["status"])
+    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
+        if catch_exception:
+            return InferenceResult(posteriors={}, model=model, error=e)
+        raise
+
+
 def infer(*, model, iterations=None, free_energy=False, returnvars=None, options=None,
           initialization=None, autoupdates=None, keephistory=None, historyvars=None,
           catch_exception=False, showprogress=False, session=None, warn=True, allow_node_contraction=False,
@@ -506,7 +582,8 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
     With ``datastream=`` (an iterable of time-chunks, or ``None`` + ``autoupdates`` for a push-driven
     engine) the call returns an ``RxInferenceEngine`` (streaming.py), as the reference does when
     ``autoupdates`` is given (/root/reference/src/inference/inference.jl:577-733 dispatch)."""
-    constraints = kwargs.pop("constraints", None) if isinstance(model, (gaussian_mixture, hidden_markov_model)) else None
+    constraints = (kwargs.pop("constraints", None) if isinstance(model, (gaussian_mixture, hidden_markov_model, hgf_offline))
+                   else None)
     for k in kwargs:
         if k in _UNSUPPORTED:
             raise NotImplementedError(
@@ -519,6 +596,9 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             raise NotImplementedError(f"options {sorted(bad)} are outside the batched hot path")
     if data is not None and datastream is not None:
         raise ValueError("`data` and `datastream` are mutually exclusive")    # reference: inference.jl argument check
+    if isinstance(model, hgf_offline):
+        return _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
+                                  datastream, context, catch_exception)
     if isinstance(model, hidden_markov_model):
         return _infer_hmm(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
                           context, catch_exception)

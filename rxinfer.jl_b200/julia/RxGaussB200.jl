@@ -249,6 +249,11 @@ gmm_vmp(ctx, d, K, N, batch, its, a0, mu0, V0, nu0, S0, ai, mi, Vi, nui, Si, y, 
         ctx.handle, d, K, N, batch, its, a0, mu0, V0, nu0, S0, ai, mi, Vi, nui, Si, y, al, mm, mc, df, iS, fe, z, hal, hmm, hmc, hdf,
         hiS, st, fl))
 
+hgf_vmp_learn(ctx, T, batch, its, prior, zp, yv, init, y, x0, xz, kw, hkw, fe, st, fl) =
+    check(ctx, ccall((:rxg_hgf_vmp_learn_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Int64, Cint, F32P, Cfloat, Cfloat, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Float64}, Ptr{Int32}, Cuint),
+        ctx.handle, T, batch, its, prior, zp, yv, init, y, x0, xz, kw, hkw, fe, st, fl))
+
 hmm_vmp(ctx, K, M, T, batch, its, p0, Ap, Ai, Ak, Bp, Bi, Bk, x, sp, s0, Aa, Ba, fe, hs, hA, hB, st, fl) =
     check(ctx, ccall((:rxg_hmm_vmp_f32, LIB), Cint,
         (Ptr{Cvoid}, Cint, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{UInt8}, F32P, F32P, F32P, F32P,
@@ -679,6 +684,46 @@ function hgf_filter(ctx::Context, p::HGFPattern, y::Matrix{Float32}; iterations:
     return download(out), fe === nothing ? nothing : download(fe)
 end
 
+"""`hgf_1` of test/inference/inference_tests.jl:609-622 with numeric hyper-parameters: (mean, variance) priors of κ, ω, x_0,
+z[1], the z transition precision and the y variance; κ, ω are learned per series (`rxg_hgf_vmp_learn_f32`)."""
+struct HGFLearnPattern
+    prior::NTuple{8, Float64}         # (m, v) of κ, ω, x_0, z[1]
+    z_precision::Float64
+    y_variance::Float64
+end
+
+"""Mean-field VMP of `HGFLearnPattern` on host data `y[batch, T]` (NaN = missing); `init` = (m, v) of the initial q(κ), q(ω),
+q(z), q(x).  Returns `xz[batch, (m_x, v_x, m_z, v_z), T]`, `kw[batch, (m, v), (κ, ω)]` (KeepLast: the ABI's [2][2][batch] read
+column-major, so the second index is mean / variance and the third the variable), the KeepEach history
+`[batch, (m, v), (κ, ω), iterations]`, the free energy `[batch, iterations]` (or `nothing`) and the per-chain status
+(`RXG_ERR_NAN` for a chain whose GH products collapsed; its results are not meaningful)."""
+function hgf_vmp_learn(ctx::Context, p::HGFLearnPattern, y::Matrix{Float32}, init::NTuple{8, Float64};
+                       iterations::Integer = 1, free_energy::Bool = true)
+    batch, T = size(y)
+    dy = upload(ctx, y)
+    x0, xz, kw = DeviceArray(ctx, batch, 2), DeviceArray(ctx, batch, 4, T), DeviceArray(ctx, batch, 2, 2)
+    hkw = DeviceArray(ctx, batch, 2, 2, Int(iterations))
+    fe = free_energy ? Lib.device_alloc(ctx, 8 * batch * iterations) : C_NULL
+    st = Lib.device_alloc(ctx, 4 * batch)
+    pr, ini = Float32[p.prior...], Float32[init...]
+    try
+        GC.@preserve pr ini Lib.hgf_vmp_learn(ctx, T, batch, iterations, pointer(pr), p.z_precision, p.y_variance, pointer(ini),
+                                              dy.ptr, x0.ptr, xz.ptr, kw.ptr, hkw.ptr, Ptr{Float64}(fe), Ptr{Int32}(st),
+                                              RXG_PTR_DEVICE)
+        status = Vector{Int32}(undef, batch)
+        GC.@preserve status Lib.memcpy_d2h(ctx, Ptr{Cvoid}(pointer(status)), st, 4 * batch)
+        F = nothing
+        if free_energy
+            F = Matrix{Float64}(undef, batch, iterations)
+            GC.@preserve F Lib.memcpy_d2h(ctx, Ptr{Cvoid}(pointer(F)), fe, 8 * batch * iterations)
+        end
+        return download(xz), download(kw), download(hkw), F, status
+    finally
+        free_energy && Lib.device_free(ctx, fe)
+        Lib.device_free(ctx, st)
+    end
+end
+
 """Gamma-precision VMP around the scalar smoother (`rxg_lgssm_vmp_gamma_f32`), host data `y[batch, T]`."""
 function vmp_gamma(ctx::Context, y::Matrix{Float32}; iterations = 10, a = 1f0, v_proc = 1f0, prior = (0f0, 100f0),
                    gamma_prior = (1f0, 1f0), init_E_tau = 1f0)
@@ -1040,6 +1085,61 @@ function recognise(generator, one_series; inputs = nothing)
                         isempty(us) ? nothing : Vector{Float64}(first(us)), transition_first, true, ndata > 0)
 end
 
+# the `q(v) = ...` entries of an @initialization by variable name (src/model/plugins/initialization_plugin.jl:22-71)
+function init_marginals(init)
+    q = Dict{Symbol, Any}()
+    for o in RxInfer.getinitobjects(init)
+        o.var_descriptor isa RxInfer.InitDescriptor{RxInfer.InitMarginal} || continue
+        q[o.var_descriptor.var_descriptor.name] = o.init_info
+    end
+    return q
+end
+
+"""
+    recognise_hgf_offline(generator, one_series) -> HGFLearnPattern | nothing
+
+Matches the graph of `hgf_1` (test/inference/inference_tests.jl:609-622): four `NormalMeanVariance` nodes with constant mean
+and variance on κ, ω, x_0 and z[1], `NormalMeanPrecision` z transitions with one constant precision, a five-interface node
+`(y, x, z, κ, ω)` per step (the reference's `gcv` submodel, contracted with `allow_node_contraction = true`), and
+`NormalMeanVariance` observations with one constant variance.  Anything else returns `nothing`.
+"""
+function recognise_hgf_offline(generator, one_series)
+    model = RxInfer.getmodel(RxInfer.create_model(generator | (y = one_series,); allow_node_contraction = true))
+    T = length(one_series)
+    priors = Dict{Symbol, Tuple{Float64, Float64}}()
+    obs, trans, gcvs = Float64[], Float64[], Any[]
+    ok = Ref(true)
+    GraphPPL.factor_nodes(model) do label, node
+        props = GraphPPL.getproperties(node)
+        f = GraphPPL.fform(props)
+        names = Set(GraphPPL.getname(e) for (_, e, _) in GraphPPL.neighbors(props))
+        if names == Set((:y, :x, :z, :κ, :ω))
+            push!(gcvs, props)
+        elseif f === NormalMeanVariance
+            out = GraphPPL.getproperties(model[variable_on(props, :out)])
+            μ, v = constant_on(model, props, :μ), constant_on(model, props, :v)
+            if GraphPPL.is_data(out) && v !== nothing && μ === nothing
+                push!(obs, v)
+            elseif μ !== nothing && v !== nothing
+                priors[GraphPPL.getname(out)] = (μ, v)
+            else
+                ok[] = false
+            end
+        elseif f === NormalMeanPrecision
+            τ = constant_on(model, props, :τ)
+            τ === nothing ? (ok[] = false) : push!(trans, τ)
+        else
+            ok[] = false
+        end
+    end
+    ok[] || return nothing
+    (length(gcvs) == T && length(obs) == T && length(trans) == T - 1) || return nothing
+    all(==(first(obs)), obs) && (isempty(trans) || all(==(first(trans)), trans)) || return nothing
+    all(k -> haskey(priors, k), (:κ, :ω, :x_0, :z)) || return nothing
+    pr = (priors[:κ]..., priors[:ω]..., priors[:x_0]..., priors[:z]...)
+    return HGFLearnPattern(Float64.(pr), isempty(trans) ? 1.0 : Float64(first(trans)), Float64(first(obs)))
+end
+
 """
     infer_batched(; model, data, iterations = nothing, free_energy = false, context = default_context(), kwargs...)
 
@@ -1058,6 +1158,36 @@ function infer_batched(; model, data, iterations = nothing, free_energy = false,
     stock() = map(b -> RxInfer.infer(; model, data = series(b), iterations, free_energy, constraints, initialization, returnvars, kwargs...),
                   collect(eachindex(ys)))
     keys(data) ⊆ (:y, :u) || return stock()
+    # `hgf_1` under MeanField() with an @initialization of q(κ), q(ω), q(z), q(x): one rxg_hgf_vmp_learn_f32 launch
+    if constraints isa RxInfer.MeanField && initialization !== nothing && !haskey(data, :u) &&
+       !any(k -> haskey(kwargs, k) && k !== :allow_node_contraction, FALLBACK_KEYWORDS) &&
+       (returnvars === nothing || returnvars isa RxInfer.KeepLast) && !any(s -> any(ismissing, s), ys)
+        hp = recognise_hgf_offline(model, first(ys))
+        q = init_marginals(initialization)                     # the @initialization's q(κ), q(ω), q(z), q(x)
+        if hp !== nothing && all(k -> haskey(q, k), (:κ, :ω, :z, :x))
+            mv(k) = (BayesBase.mean(q[k]), BayesBase.var(q[k]))
+            init = Float64.((mv(:κ)..., mv(:ω)..., mv(:z)..., mv(:x)...))
+            y = Float32[ys[b][t] for b in eachindex(ys), t in 1:length(first(ys))]
+            its = iterations === nothing ? 1 : iterations
+            xz, kw, _, F, status = hgf_vmp_learn(context, hp, y, init; iterations = its, free_energy = free_energy !== false)
+            batch, _, T = size(xz)
+            # kw[b, (m, v), (κ, ω)]: mean kw[b, 1, j], variance kw[b, 2, j] of variable j = 1 (κ), 2 (ω)
+            posteriors = Dict(:x => [NormalMeanVariance(Float64(xz[b, 1, t]), Float64(xz[b, 2, t])) for t in 1:T, b in 1:batch],
+                              :z => [NormalMeanVariance(Float64(xz[b, 3, t]), Float64(xz[b, 4, t])) for t in 1:T, b in 1:batch],
+                              :κ => [NormalMeanVariance(Float64(kw[b, 1, 1]), Float64(kw[b, 2, 1])) for b in 1:batch],
+                              :ω => [NormalMeanVariance(Float64(kw[b, 1, 2]), Float64(kw[b, 2, 2])) for b in 1:batch])
+            # a chain flagged RXG_ERR_NAN (collapsed GH products, DESIGN 3.19) is rerun through stock RxInfer; the others keep
+            # the batched result
+            for b in findall(!=(RXG_OK), status)
+                r = RxInfer.infer(; model, data = series(b), iterations, free_energy, constraints, initialization, returnvars, kwargs...)
+                posteriors[:x][:, b] = r.posteriors[:x]
+                posteriors[:z][:, b] = r.posteriors[:z]
+                posteriors[:κ][b], posteriors[:ω][b] = r.posteriors[:κ], r.posteriors[:ω]
+                F === nothing || (F[b, :] = r.free_energy)
+            end
+            return RxInfer.InferenceResult(posteriors, Dict{Symbol, Any}(), F, model, nothing)
+        end
+    end
     us = haskey(data, :u) ? data.u : nothing
     # `predictvars = (y = KeepLast(),)` is the one prediction request of the fused path; any other form (forecast nodes, KeepEach,
     # other variables) stays in the fallback list
