@@ -10,6 +10,7 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
   python bench_extra.py --which vmp_transition (opt-in: learned transition matrix, alone and with the noise precisions)
   python bench_extra.py --which gmm          (opt-in: Gaussian-mixture VMP, d = 2 / K = 3 and d = 4 / K = 8)
   python bench_extra.py --which hmm          (opt-in: hidden Markov model VMP, K = M = 3 and K = 8 / M = 16)
+  python bench_extra.py --which hmm_gauss    (opt-in: Gaussian-emission HMM VMP, K = 3 / d = 2 and K = 8 / d = 4)
   python bench_extra.py --which hgf_learn    (opt-in: HGF with learned kappa, omega, T = 1000, 20 iterations)
 """
 from __future__ import annotations
@@ -442,6 +443,37 @@ def bench_hgf_learn(ctx, peak):
     torch.cuda.empty_cache()
 
 
+def bench_hmm_gauss(ctx, peak):
+    """Hidden Markov model with Gaussian emissions (rxg_hmm_gauss_vmp_f32), T = 1000 steps, 20 iterations, 65 536 chains,
+    A learned, free energy on; time from CUDA events around the call (host validation and the constant upload included).
+    Algorithmic bytes per (chain, step): (8 d + 8 K) per iteration (y read twice, the forward stash written and read once)
+    plus 4 K for q(s) written at the end.  The fp64 bound: the backward pass adds gamma into K (1 + d + d(d+1)/2) fp64
+    shared-memory accumulators per step (2 flops each), at the H100's 33.5 TFLOP/s fp64 (non-tensor) rate."""
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(23)
+    T, nb, its = 1000, 65536, 20
+    for K, d in ((3, 2), (8, 4)):
+        y = 3.0 * torch.randn(T, d, nb, device="cuda", generator=g)
+        rng = np.random.default_rng(K)
+        kw = dict(p0=np.full(K, 1.0 / K), A_prior=np.ones((K, K)) + 4 * np.eye(K), A_init=rng.uniform(0.5, 2.0, (K, K)),
+                  mu0=np.zeros((K, d)), V0=np.stack([100.0 * np.eye(d)] * K), nu0=np.full(K, d + 2.0),
+                  S0=np.stack([np.eye(d) / (d + 2.0)] * K), m_init=3.0 * rng.standard_normal((K, d)),
+                  Vm_init=np.stack([np.eye(d)] * K), nu_init=np.full(K, d + 2.0), S_init=np.stack([np.eye(d) / (d + 2.0)] * K))
+        runs = [timed(lambda: ctx.hmm_gauss_vmp(y, **kw, iterations=its), warm=2, reps=3) for _ in range(3)]
+        ms = float(np.median(runs))
+        by = ((8 * d + 8 * K) * its + 4 * K) * T * nb
+        fl64 = 2 * K * (1 + d + d * (d + 1) // 2) * its * T * nb
+        t = {"hbm": by / (peak * 1e9), "fp64_accumulators": fl64 / 33.5e12}
+        bound = max(t, key=t.get)
+        print(json.dumps({"what": "Gaussian-emission HMM VMP (hmm_gauss_vmp_kernel), A learned, free energy on", "K": K,
+                          "d": d, "T": T, "batch": nb, "iterations": its, "ms": ms, "ms_runs": runs,
+                          "ms_per_iteration": ms / its, "bytes_per_chain_step": by / (T * nb), "achieved_GBs": by / ms / 1e6,
+                          "bound": bound, "bound_ms": {k: v * 1e3 for k, v in t.items()}, "frac_of_bound": t[bound] * 1e3 / ms,
+                          "peak_hbm_gbs": peak, "gpu": gname, "power_limit": plim}), flush=True)
+        del y
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -465,6 +497,8 @@ def main():
         bench_hmm(ctx, peak)
     if "hgf_learn" in which:
         bench_hgf_learn(ctx, peak)
+    if "hmm_gauss" in which:
+        bench_hmm_gauss(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

@@ -294,6 +294,36 @@ int rxg_hmm_vmp_f32(rxg_ctx*, int K, int M, int T, int64_t batch, int iterations
                     const float* A_init, const float* A_known, const float* B_prior, const float* B_init,
                     const float* B_known, const uint8_t* x, float* s_prob, float* s0_prob, float* A_alpha, float* B_alpha,
                     double* free_energy, float* hist_s, float* hist_A, float* hist_B, int32_t* status, unsigned flags);
+/* Fused structured VMP of the hidden Markov model with Gaussian emissions, `batch` independent chains, all iterations in one
+ *   launch: A ~ DirichletCollection(A_prior) (K x K, column j = p(s_t | s_{t-1} = j)) or a known probability matrix,
+ *   m[k] ~ MvNormal(mu0[k], V0[k]), W[k] ~ Wishart(nu0[k], S0[k]) (precision; S0 the scale), s_0 ~ Categorical(p0),
+ *   s[t] ~ DiscreteTransition(s[t-1], A), y[t] ~ NormalMixture(switch = s[t], m, W), q(s_0, s) q(A) prod q(m[k]) q(W[k]),
+ *   initialised to DirichletCollection(A_init), MvNormal(m_init[k], Vm_init[k]), Wishart(nu_init[k], S_init[k])
+ *   [ref: test/models/statespace/hmm_tests.jl:8-45 (the chain, DiscreteTransition and its structured factorisation) with
+ *   the NormalMixture emission of test/models/mixtures/gmm_multivariate_tests.jl:4-24; no reference test runs this model,
+ *   so nothing pins it (DESIGN 3.20)].  A is learned (A_prior and A_init non-NULL, A_known NULL) or known (A_known, the
+ *   other two NULL).  Host arrays shared by every chain, row-major: p0[K], A_*[K][K] (row = next state), mu0[K][d],
+ *   V0[K][d][d] (covariance), nu0[K], S0[K][d][d], likewise m_init, Vm_init, nu_init, S_init.  y[T][d][batch]; a step whose
+ *   d components are all NaN is missing (a pure transition).  Outputs: s_prob[T][K][batch] (q(s_t) of the last iteration;
+ *   also the forward stash), and optional (NULL = not wanted): s0_prob[K][batch], A_alpha[K][K][batch] (A learned),
+ *   m_mean[K][d][batch], m_cov[K][d][d][batch], w_df[K][batch], w_inv_scale[K][d][d][batch] (q(W[k]) = Wishart(w_df,
+ *   inv(w_inv_scale))), free_energy[iterations][batch] (fp64, Bethe free energy after every iteration), the KeepEach
+ *   histories hist_s[iterations][T][K][batch], hist_A[iterations][K][K][batch], hist_m_mean[iterations][K][d][batch],
+ *   hist_m_cov[iterations][K][d][d][batch], hist_w_df[iterations][K][batch], hist_w_inv_scale[iterations][K][d][d][batch],
+ *   status[batch] (RXG_ERR_BAD_ARG for a chain with a non-finite datum other than an all-NaN step, read as missing;
+ *   RXG_ERR_NAN for a chain whose normaliser vanished; RXG_ERR_NOT_SPD for a chain whose update met a non-SPD matrix).
+ *   Per iteration: forward-backward with the previous q(A), q(m), q(W), then q(A), q(m[k]) with the previous E[W[k]],
+ *   q(W[k]) with the new q(m[k]).  1 <= d <= 4 and 2 <= K <= 8, else RXG_ERR_UNSUPPORTED; T, batch, iterations >= 1,
+ *   Dirichlet parameters > 0, p0 and the columns of A_known probability vectors (within 1e-5), nu0 and nu_init > d - 1,
+ *   V0, S0, Vm_init, S_init symmetric positive definite, else RXG_ERR_BAD_ARG.  Device pointers (RXG_ERR_UNSUPPORTED
+ *   otherwise).                                                                                                        */
+int rxg_hmm_gauss_vmp_f32(rxg_ctx*, int d, int K, int T, int64_t batch, int iterations, const float* p0,
+                          const float* A_prior, const float* A_init, const float* A_known, const float* mu0, const float* V0,
+                          const float* nu0, const float* S0, const float* m_init, const float* Vm_init, const float* nu_init,
+                          const float* S_init, const float* y, float* s_prob, float* s0_prob, float* A_alpha, float* m_mean,
+                          float* m_cov, float* w_df, float* w_inv_scale, double* free_energy, float* hist_s, float* hist_A,
+                          float* hist_m_mean, float* hist_m_cov, float* hist_w_df, float* hist_w_inv_scale,
+                          int32_t* status, unsigned flags);
 /* prod(GammaShapeRate, GammaShapeRate) = (a1 + a2 - 1, b1 + b2)                                 */
 int rxg_prod_gamma_f32(rxg_ctx*, int64_t n, const float* a1, const float* b1, const float* a2,
                        const float* b2, float* a, float* b, unsigned flags);

@@ -20,7 +20,8 @@ def __getattr__(name):   # lazy: these import torch
                 "hgf", "univariate_lgssm_gamma_precision", "kalman_gamma_streaming", "latent_autoregressive",
                 "linear_gaussian_ssm_wishart_precision", "linear_gaussian_ssm_wishart_noise",
                 "linear_gaussian_ssm_continuous_transition", "gaussian_mixture", "MeanField", "BetheFactorization",
-                "hidden_markov_model", "HMMConstraints", "hgf_offline",
+                "hidden_markov_model", "HMMConstraints", "hgf_offline", "gaussian_hidden_markov_model",
+                "GaussianHMMConstraints",
                 "default_context",
                 "KeepLast", "KeepEach"):
         from . import inference

@@ -802,6 +802,53 @@ class Context:
         out.update(h)
         return out
 
+    def hmm_gauss_vmp(self, y, p0, mu0, V0, nu0, S0, m_init, Vm_init, nu_init, S_init, A_prior=None, A_init=None,
+                      A_known=None, iterations=1, want_free_energy=True, keep_each=False):
+        """Fused structured VMP of the hidden Markov model with Gaussian emissions (``rxg_hmm_gauss_vmp_f32``); y[T, d, batch]
+        on the device (an all-NaN step is missing).  p0[K], A (learned: ``A_prior`` and ``A_init``, Dirichlet parameters
+        [K, K]; known: ``A_known``, a probability matrix; columns = conditionals) and the emission priors and initial
+        marginals (mu0[K, d], V0[K, d, d] covariance, nu0[K], S0[K, d, d] Wishart scale; likewise m_init, Vm_init, nu_init,
+        S_init) are host arrays shared by every chain.  Returns ``s_prob[T, K, batch]``, ``s0_prob[K, batch]``,
+        ``A_alpha[K, K, batch]`` (None when known), ``m_mean[K, d, batch]``, ``m_cov[K, d, d, batch]``, ``w_df[K, batch]``,
+        ``w_inv_scale[K, d, d, batch]``, ``free_energy[iterations, batch]`` (fp64), ``status[batch]`` and, with
+        ``keep_each``, ``hist_*`` with a leading iteration axis."""
+        self._dev(y)
+        if y.dim() != 3:
+            raise ValueError("hmm_gauss_vmp: y must be [T, d, batch]")
+        T, d, batch = y.shape
+        K = int(np.asarray(p0).reshape(-1).shape[0])
+        vals = dict(p0=(p0, (K,)), A_prior=(A_prior, (K, K)), A_init=(A_init, (K, K)), A_known=(A_known, (K, K)),
+                    mu0=(mu0, (K, d)), V0=(V0, (K, d, d)), nu0=(nu0, (K,)), S0=(S0, (K, d, d)), m_init=(m_init, (K, d)),
+                    Vm_init=(Vm_init, (K, d, d)), nu_init=(nu_init, (K,)), S_init=(S_init, (K, d, d)))
+        keep = {}
+        for k, (v, shp) in vals.items():
+            if v is None:
+                keep[k] = (None, L.as_fp(0))
+                continue
+            a = np.asarray(v, dtype=np.float64)
+            if a.shape != shp:
+                raise ValueError(f"hmm_gauss_vmp: {k} must have shape {shp} (K = {K}, d = {d}), got {a.shape}")
+            keep[k] = _model32(a)
+        learn_A = A_known is None
+        its = int(iterations)
+        sp, s0 = self.empty(T, K, batch), self.empty(K, batch)
+        Aa = self.empty(K, K, batch) if learn_A else None
+        mm, mc, df, iS = self.empty(K, d, batch), self.empty(K, d, d, batch), self.empty(K, batch), self.empty(K, d, d, batch)
+        fe = self.empty(its, batch, dtype=torch.float64) if want_free_energy else None
+        h = dict(hist_s=self.empty(its, T, K, batch), hist_A=self.empty(its, K, K, batch) if learn_A else None,
+                 hist_m_mean=self.empty(its, K, d, batch), hist_m_cov=self.empty(its, K, d, d, batch),
+                 hist_w_df=self.empty(its, K, batch), hist_w_inv_scale=self.empty(its, K, d, d, batch)) if keep_each else {}
+        st = self.empty(batch, dtype=torch.int32)
+        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
+        self._check(self.lib.rxg_hmm_gauss_vmp_f32(self.h, d, K, T, batch, its, *(keep[k][1] for k in vals), _fp(y), _fp(sp),
+                                                   _fp(s0), _fp(Aa), _fp(mm), _fp(mc), _fp(df), _fp(iS), fe_p,
+                                                   *(_fp(h.get(k)) for k in ("hist_s", "hist_A", "hist_m_mean", "hist_m_cov",
+                                                                               "hist_w_df", "hist_w_inv_scale")),
+                                                   ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+        out = dict(s_prob=sp, s0_prob=s0, A_alpha=Aa, m_mean=mm, m_cov=mc, w_df=df, w_inv_scale=iS, free_energy=fe, status=st)
+        out.update(h)
+        return out
+
     def prod_gamma(self, a1, b1, a2, b2):
         return self._six(self.lib.rxg_prod_gamma_f32, a1, b1, a2, b2)
 

@@ -331,6 +331,71 @@ def hmm_arguments(model, initialization):
 
 
 @dataclass
+class gaussian_hidden_markov_model:
+    """Hidden Markov model with Gaussian emissions: ``A ~ DirichletCollection(A_prior)`` (or a ``PointMass`` probability
+    matrix, known), ``m[k] ~ m_prior[k]``, ``w[k] ~ w_prior[k]`` (precision), ``s_0 ~ Categorical(p0)``,
+    ``s[t] ~ DiscreteTransition(s[t-1], A)``, ``y[t] ~ NormalMixture(switch = s[t], m = m, p = w)``; column j of A is
+    p(s_t | s_{t-1} = j), as in ``hidden_markov_model``.  Multivariate spelling: ``MvNormalMeanCovariance`` means and
+    ``Wishart(df, scale)`` precisions; at d = 1 also ``NormalMeanVariance`` and ``GammaShapeRate(shape, rate)``
+    (= Wishart(2 shape, 1 / (2 rate))).  Run with ``constraints = GaussianHMMConstraints()``, ``initialization =
+    {"A": q(A) (A learned), "m": [q(m[k])], "w": [q(w[k])]}`` (an ``"s"`` entry is accepted and not needed) and
+    ``data = {"y": [T, d, batch]}`` ([T, batch] at d = 1; an all-NaN step is missing)."""
+    p0: object
+    A: object
+    m_prior: list
+    w_prior: list
+
+
+class GaussianHMMConstraints:
+    """``q(s_0, s, A, m, w) = q(s_0, s) q(A) q(m[1]) ... q(m[K]) q(w[1]) ... q(w[K])``: the chain kept structured, the
+    transition matrix and every state's mean and precision apart."""
+
+    def __eq__(self, other):
+        return isinstance(other, GaussianHMMConstraints)
+
+    def __hash__(self):
+        return hash(GaussianHMMConstraints)
+
+
+def gaussian_hmm_arguments(model, initialization):
+    """The keyword arguments of ``Context.hmm_gauss_vmp`` for ``model`` and ``initialization``: p0[K], the A arguments of
+    ``hmm_arguments`` and the emission arrays of ``gaussian_mixture_arrays`` (mu0[K, d], V0[K, d, d], nu0[K], S0[K, d, d]
+    and the same for the initial q(m), q(w))."""
+    p0 = np.asarray(model.p0.p if isinstance(model.p0, Categorical) else model.p0, np.float64).reshape(-1)
+    K = p0.shape[0]
+    init = initialization or {}
+    if not {"m", "w"} <= set(init):
+        raise ValueError("gaussian_hidden_markov_model needs initialization = {'m': [q(m[k])], 'w': [q(w[k])]} (and 'A' "
+                         "when A is learned)")
+    out = {"p0": p0}
+    if isinstance(model.A, PointMass):
+        out["A_known"] = np.asarray(model.A.value, np.float64)
+        shape = out["A_known"].shape
+    elif isinstance(model.A, DirichletCollection):
+        if not isinstance(init.get("A"), DirichletCollection):
+            raise ValueError(f"A is learned: pass initialization = {{'A': DirichletCollection(...)}}, e.g. "
+                             f"vague(DirichletCollection, {np.asarray(model.A.alpha).shape})")
+        out["A_prior"] = np.asarray(model.A.alpha, np.float64)
+        out["A_init"] = np.asarray(init["A"].alpha, np.float64)
+        shape = out["A_prior"].shape
+        if out["A_init"].shape != shape:
+            raise ValueError(f"initialization['A'] has shape {out['A_init'].shape}, the prior {shape}")
+    else:
+        raise TypeError(f"model.A: expected DirichletCollection or PointMass, got {type(model.A).__name__}")
+    if shape != (K, K):
+        raise ValueError(f"model.A has shape {shape}; with K = {K} states A is K x K")
+    out["mu0"], out["V0"] = _gaussians(model.m_prior, K, "m_prior")
+    out["m_init"], out["Vm_init"] = _gaussians(init["m"], K, "initialization['m']")
+    out["nu0"], out["S0"] = _precisions(model.w_prior, K, "w_prior")
+    out["nu_init"], out["S_init"] = _precisions(init["w"], K, "initialization['w']")
+    d = out["mu0"].shape[1]
+    for k in ("m_init", "V0", "Vm_init", "S0", "S_init"):
+        if out[k].shape[1] != d:
+            raise ValueError(f"{k}: dimension {out[k].shape[1]}, the means have d = {d}")
+    return out
+
+
+@dataclass
 class hgf_offline:
     """``@model hgf_1`` (/root/reference/test/inference/inference_tests.jl:609-622) with every hyper-parameter a number:
     ``ω ~ N(ω_prior)``, ``κ ~ N(κ_prior)``, ``x_0 ~ N(x0_prior)``, ``z[1] ~ N(z1_prior)`` ((mean, variance) each),
@@ -525,6 +590,69 @@ def _infer_hmm(model, data, constraints, initialization, iterations, free_energy
         raise
 
 
+def _infer_hmm_gauss(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars, datastream,
+                     context, catch_exception):
+    """``infer`` of ``gaussian_hidden_markov_model``: one ``rxg_hmm_gauss_vmp_f32`` launch.  ``returnvars`` is KeepLast() /
+    KeepEach() for every variable or a dict over ``s``, ``A``, ``m``, ``w`` (and KeepLast() of ``s_0``)."""
+    if not isinstance(constraints, GaussianHMMConstraints):
+        raise ValueError("gaussian_hidden_markov_model runs the structured factorisation q(s_0, s) q(A) q(m[1]) ... q(m[K]) "
+                         f"q(w[1]) ... q(w[K]) only; pass constraints = GaussianHMMConstraints() (got {constraints!r})")
+    if predictvars is not None:
+        raise NotImplementedError("predictvars: predictions of the Gaussian hidden Markov model are outside the batched "
+                                  "hot path")
+    if datastream is not None or data is None:
+        raise NotImplementedError("gaussian_hidden_markov_model runs over whole series: pass data = {'y': [T, d, batch]} "
+                                  "(no datastream)")
+    if "y" not in data:
+        raise KeyError("gaussian_hidden_markov_model needs data = {'y': observations}")
+    if isinstance(returnvars, dict):
+        bad = set(returnvars) - {"s", "A", "m", "w", "s_0"}
+        if bad or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
+            raise NotImplementedError(f"returnvars={returnvars!r}: KeepEach() / KeepLast() of s, A, m, w (and KeepLast() "
+                                      "of s_0)")
+        each = {k for k, v in returnvars.items() if isinstance(v, KeepEach)}
+        if "s_0" in each:
+            raise NotImplementedError("returnvars: q(s_0) is kept for the last iteration only (KeepLast)")
+    elif returnvars is None or isinstance(returnvars, (KeepEach, KeepLast)):
+        each = {"s", "A", "m", "w"} if isinstance(returnvars, KeepEach) else set()
+    else:
+        raise NotImplementedError(f"returnvars={returnvars!r}: the Gaussian hidden Markov model returns KeepEach() or "
+                                  "KeepLast()")
+    args = gaussian_hmm_arguments(model, initialization)
+    d = args["mu0"].shape[1]
+    y = torch.as_tensor(data["y"])
+    y = y[:, None] if y.dim() == 2 and d == 1 else y            # univariate data may come as [T, batch]
+    if y.dim() != 3 or y.shape[1] != d:
+        raise ValueError(f"data['y'] must be [T, d = {d}, batch] (or [T, batch] at d = 1), got {tuple(y.shape)}")
+    univariate = isinstance(model.m_prior[0], NormalMeanVariance) and isinstance(model.w_prior[0], GammaShapeRate)
+    try:
+        ctx = context or default_context()
+        y = y.to(device=f"cuda:{ctx.device}", dtype=torch.float32).contiguous()
+        r = ctx.hmm_gauss_vmp(y, **args, iterations=iterations or 1, want_free_energy=bool(free_energy),
+                              keep_each=bool(each))
+        _raise_flagged(r["status"], "gaussian_hidden_markov_model: ",
+                       " (BAD_ARG: a non-finite datum other than an all-NaN step; NAN: a vanished normaliser; NOT_SPD: "
+                       "an update met a non-SPD matrix)")
+        post = {"s": Categorical(r["hist_s"] if "s" in each else r["s_prob"]), "s_0": Categorical(r["s0_prob"])}
+        if r["A_alpha"] is not None:
+            post["A"] = DirichletCollection(r["hist_A"] if "A" in each else r["A_alpha"])
+        mp = "hist_" if "m" in each else ""                      # KeepEach: a leading iteration axis
+        wp = "hist_" if "w" in each else ""
+        mm, mc, df, iS = r[mp + "m_mean"], r[mp + "m_cov"], r[wp + "w_df"], r[wp + "w_inv_scale"]
+        K = mm.shape[-3]
+        if univariate:
+            post["m"] = [NormalMeanVariance(mm[..., k, 0, :], mc[..., k, 0, 0, :]) for k in range(K)]
+            post["w"] = [GammaShapeRate(df[..., k, :] / 2, iS[..., k, 0, 0, :] / 2) for k in range(K)]
+        else:
+            post["m"] = [MvNormalMeanCovariance(mm[..., k, :, :], mc[..., k, :, :, :]) for k in range(K)]
+            post["w"] = [WishartFast(df[..., k, :], iS[..., k, :, :, :]) for k in range(K)]
+        return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
+    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
+        if catch_exception:
+            return InferenceResult(posteriors={}, model=model, error=e)
+        raise
+
+
 def _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
                        datastream, context, catch_exception):
     """``infer`` of ``hgf_offline``: one ``rxg_hgf_vmp_learn_f32`` launch.  ``returnvars``: KeepLast() for x, z (and x_0),
@@ -582,7 +710,8 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
     With ``datastream=`` (an iterable of time-chunks, or ``None`` + ``autoupdates`` for a push-driven
     engine) the call returns an ``RxInferenceEngine`` (streaming.py), as the reference does when
     ``autoupdates`` is given (/root/reference/src/inference/inference.jl:577-733 dispatch)."""
-    constraints = (kwargs.pop("constraints", None) if isinstance(model, (gaussian_mixture, hidden_markov_model, hgf_offline))
+    constraints = (kwargs.pop("constraints", None) if isinstance(model, (gaussian_mixture, hidden_markov_model, hgf_offline,
+                                                                         gaussian_hidden_markov_model))
                    else None)
     for k in kwargs:
         if k in _UNSUPPORTED:
@@ -599,6 +728,9 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
     if isinstance(model, hgf_offline):
         return _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
                                   datastream, context, catch_exception)
+    if isinstance(model, gaussian_hidden_markov_model):
+        return _infer_hmm_gauss(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
+                                datastream, context, catch_exception)
     if isinstance(model, hidden_markov_model):
         return _infer_hmm(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
                           context, catch_exception)

@@ -260,6 +260,14 @@ hmm_vmp(ctx, K, M, T, batch, its, p0, Ap, Ai, Ak, Bp, Bi, Bk, x, sp, s0, Aa, Ba,
          Ptr{Float64}, F32P, F32P, F32P, Ptr{Int32}, Cuint),
         ctx.handle, K, M, T, batch, its, p0, Ap, Ai, Ak, Bp, Bi, Bk, x, sp, s0, Aa, Ba, fe, hs, hA, hB, st, fl))
 
+hmm_gauss_vmp(ctx, d, K, T, batch, its, p0, Ap, Ai, Ak, mu0, V0, nu0, S0, mi, Vi, nui, Si, y, sp, s0, Aa, mm, mc, df, iS, fe, hs, hA,
+              hmm, hmc, hdf, hiS, st, fl) =
+    check(ctx, ccall((:rxg_hmm_gauss_vmp_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P,
+         F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Float64}, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Int32}, Cuint),
+        ctx.handle, d, K, T, batch, its, p0, Ap, Ai, Ak, mu0, V0, nu0, S0, mi, Vi, nui, Si, y, sp, s0, Aa, mm, mc, df, iS, fe, hs,
+        hA, hmm, hmc, hdf, hiS, st, fl))
+
 # ---- diagnostics
 selftest_umma(ctx, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_f32, LIB), Cint, (Ptr{Cvoid}, F32P, F32P, F32P, Cuint), ctx.handle, A, B, D, fl))
 selftest_umma_shape(ctx, n, k, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_shape_f32, LIB), Cint, (Ptr{Cvoid}, Cint, Cint, F32P, F32P, F32P, Cuint), ctx.handle, n, k, A, B, D, fl))
@@ -919,6 +927,59 @@ function gaussian_mixture(ctx::Context, y::Array{Float32, 3}; alpha0, mu0, V0, n
     Lib.device_free(ctx, fe)
     return (s = download(hal), m_mean = download(hmm), m_cov = download(hmc), w_df = download(hdf), w_inv_scale = download(hiS),
             z = download(z), free_energy = fe_host, status = reinterpret(Int32, download(st)))
+end
+
+"""Fused structured VMP of the hidden Markov model with Gaussian emissions (`rxg_hmm_gauss_vmp_f32`); `y[batch, d, T]`, a step
+whose d components are all NaN is missing.  The model, in RxInfer's spelling (no reference test runs it; DESIGN 3.20):
+
+    @model function gaussian_hmm(y, p0, A_prior, m_priors, w_priors)
+        A ~ DirichletCollection(A_prior)                       # or A passed as data (known)
+        for k in 1:K
+            m[k] ~ MvNormal(μ = μ0[k], Σ = V0[k])
+            w[k] ~ Wishart(ν0[k], S0[k])                       # precision
+        end
+        s_0 ~ Categorical(p0)
+        s_prev = s_0
+        for t in eachindex(y)
+            s[t] ~ DiscreteTransition(s_prev, A)
+            y[t] ~ NormalMixture(switch = s[t], m = m, p = w)
+            s_prev = s[t]
+        end
+    end
+    # q(s_0, s, A, m, w) = q(s_0, s) q(A) q(m[1]) … q(m[K]) q(w[1]) … q(w[K])
+
+`p0` is a `K` vector; `A` is learned, `(prior = alpha0, init = alpha_init)` with K x K Dirichlet parameter matrices, or
+known, a probability matrix; column j is the distribution conditioned on state j, as in `hidden_markov_model`.  `mu0` is a
+`d x K` matrix (one column per state), `V0`, `S0` `d x d x K` arrays (covariance, Wishart scale), `nu0` a `K` vector; the
+`init` NamedTuple `(m, Vm, nu, S)` holds the initial q(m), q(w) in the same shapes (the layout of `gaussian_mixture`).
+Returns the KeepEach posteriors (trailing iteration axis): q(s) `[batch, K, T, its]`, the Dirichlet parameters of a learned
+A `[batch, K, K, its]` with entry `[b, i, j, n]` = alpha[i, j] (`nothing` when known), m mean `[batch, d, K, its]`, m cov
+`[batch, d, d, K, its]`, W df `[batch, K, its]`, W inverse scale `[batch, d, d, K, its]`, q(s_0) `[batch, K]`, the Bethe
+free energy `[batch, its]` (Float64) and the per-chain status."""
+function gaussian_hidden_markov_model(ctx::Context, y::Array{Float32, 3}; p0, A, mu0, V0, nu0, S0, init, iterations = 20)
+    batch, d, T = size(y)
+    K = length(p0)
+    dy = upload(ctx, y)
+    sp, s0 = DeviceArray(ctx, batch, K, T), DeviceArray(ctx, batch, K)
+    hs = DeviceArray(ctx, batch, K, T, iterations)
+    hA = A isa NamedTuple ? DeviceArray(ctx, batch, K, K, iterations) : nothing
+    hmm, hmc = DeviceArray(ctx, batch, d, K, iterations), DeviceArray(ctx, batch, d, d, K, iterations)
+    hdf, hiS = DeviceArray(ctx, batch, K, iterations), DeviceArray(ctx, batch, d, d, K, iterations)
+    st = DeviceArray(ctx, batch)
+    fe = Lib.device_alloc(ctx, 8 * batch * iterations)
+    side = A isa NamedTuple ? (rowmajor32(A.prior), rowmajor32(A.init), nothing) : (nothing, nothing, rowmajor32(A))
+    em = [Float32.(collect(x)) for x in (mu0, V0, nu0, S0, init.m, init.Vm, init.nu, init.S)]
+    h = (Float32.(collect(p0)), side..., em...)
+    ptr(v) = v === nothing ? NULLF : pointer(v)
+    GC.@preserve h Lib.hmm_gauss_vmp(ctx, d, K, T, batch, iterations, (ptr(v) for v in h)..., dy.ptr, sp.ptr, s0.ptr, NULLF,
+                                     NULLF, NULLF, NULLF, NULLF, Ptr{Float64}(fe), hs.ptr, hA === nothing ? NULLF : hA.ptr,
+                                     hmm.ptr, hmc.ptr, hdf.ptr, hiS.ptr, Ptr{Int32}(st.ptr), RXG_PTR_DEVICE)
+    fe_host = Array{Float64}(undef, batch, iterations)
+    GC.@preserve fe_host Lib.memcpy_d2h(ctx, pointer(fe_host), fe, 8 * batch * iterations)
+    Lib.device_free(ctx, fe)
+    rowcol(x) = x === nothing ? nothing : permutedims(download(x), (1, 3, 2, 4))
+    return (s = download(hs), A = rowcol(hA), m_mean = download(hmm), m_cov = download(hmc), w_df = download(hdf),
+            w_inv_scale = download(hiS), s_0 = download(s0), free_energy = fe_host, status = reinterpret(Int32, download(st)))
 end
 
 """Fused structured VMP of the hidden Markov model (hmm_tests.jl:8-45, `rxg_hmm_vmp_f32`); `x[batch, T]` UInt8 symbols 0..M-1
