@@ -40,6 +40,10 @@ int launch(rxg_ctx* ctx, const rxg::hmm::Args& a, int32_t* status) {
     return RXG_OK;
 }
 
+}  // namespace
+
+namespace rxg {
+
 // columns of a [rows][K] matrix each a probability vector (non-negative, finite, sum 1 within 1e-5)
 bool stochastic_columns(const float* p, int rows, int K) {
     for (int j = 0; j < K; ++j) {
@@ -60,7 +64,7 @@ bool positive(const float* p, int n) {
     return true;
 }
 
-}  // namespace
+}  // namespace rxg
 
 extern "C" int rxg_hmm_vmp_f32(rxg_ctx* ctx, int K, int M, int T, int64_t batch, int iterations, const float* p0,
                                const float* A_prior, const float* A_init, const float* A_known, const float* B_prior,
@@ -79,11 +83,11 @@ extern "C" int rxg_hmm_vmp_f32(rxg_ctx* ctx, int K, int M, int T, int64_t batch,
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_vmp: pass either A_prior and A_init (A learned) or A_known");
     if (learn_B == (B_known != nullptr) || (learn_B && !(B_prior && B_init)))
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_vmp: pass either B_prior and B_init (B learned) or B_known");
-    if (!stochastic_columns(p0, K, 1)) return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_vmp: p0 is not a probability vector");
-    if (learn_A ? !(positive(A_prior, K * K) && positive(A_init, K * K)) : !stochastic_columns(A_known, K, K))
+    if (!rxg::stochastic_columns(p0, K, 1)) return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_vmp: p0 is not a probability vector");
+    if (learn_A ? !(rxg::positive(A_prior, K * K) && rxg::positive(A_init, K * K)) : !rxg::stochastic_columns(A_known, K, K))
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, learn_A ? "hmm_vmp: A_prior and A_init must be positive"
                                                         : "hmm_vmp: the columns of A_known must be probability vectors");
-    if (learn_B ? !(positive(B_prior, M * K) && positive(B_init, M * K)) : !stochastic_columns(B_known, M, K))
+    if (learn_B ? !(rxg::positive(B_prior, M * K) && rxg::positive(B_init, M * K)) : !rxg::stochastic_columns(B_known, M, K))
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, learn_B ? "hmm_vmp: B_prior and B_init must be positive"
                                                         : "hmm_vmp: the columns of B_known must be probability vectors");
     double hp[8 + 2 * 64 + 2 * MAX_M * 8];

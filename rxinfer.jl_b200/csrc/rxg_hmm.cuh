@@ -94,6 +94,44 @@ RXG_HD double log_beta_terms(const double* a0, N n, int R, int C) {
     return f;
 }
 
+// q(A) of the chains here and in rxg_hmm_gauss.cuh, whose Args both carry prm (p0 [K], alpha_A0 [K][K], A_init [K][K] at
+// its head), batch, hist_A and A_alpha; xi: the fp64 transition counts [K][K], slot q at xi[q * ss].
+// A~ = exp(E[log A]) into At, alpha = A_init in the first iteration, else alpha_A0 + the counts of the previous sweep;
+// xi is the scratch (it holds E[log A] on return)
+template <int K, typename ArgsT>
+RXG_HD void a_tilde(const ArgsT& a, int it, double* xi, int ss, float (&At)[K][K]) {
+    const double *pA = a.prm + off_A(K), *ai = a.prm + off_Ai(K);
+    for (int q = 0; q < K * K; ++q) xi[q * ss] = it == 0 ? ai[q] : pA[q] + xi[q * ss];   // alpha, in place
+    for (int j = 0; j < K; ++j)
+        elog_column([&](int r, int c) { return xi[(r * K + c) * ss]; }, K, j,
+                    [&](int r, double e) { xi[(r * K + j) * ss] = e; });
+#pragma unroll
+    for (int i = 0; i < K; ++i)
+#pragma unroll
+        for (int j = 0; j < K; ++j) At[i][j] = (float)exp(xi[(i * K + j) * ss]);
+}
+
+// The free-energy terms of q(A) after the sweep that ran with At and counted xi, added to F; alpha_A0 + xi into hist_A
+// (every iteration) and A_alpha (the last)
+template <int K, typename ArgsT>
+RXG_HD void a_terms(const ArgsT& a, int it, bool last, int64_t b, const double* xi, int ss, const float (&At)[K][K],
+                    double& F) {
+    const double* pA = a.prm + off_A(K);
+    F += log_beta_terms(pA, [&](int r, int c) { return xi[(r * K + c) * ss]; }, K, K);
+#pragma unroll
+    for (int i = 0; i < K; ++i)
+#pragma unroll
+        for (int j = 0; j < K; ++j) {                // At > 0 wherever the count is (it is proportional to At)
+            const double n = xi[(i * K + j) * ss];
+            if (n > 0.0) F += n * log((double)At[i][j]);
+        }
+    for (int q = 0; q < K * K; ++q) {
+        const float v = (float)(pA[q] + xi[q * ss]);
+        if (a.hist_A) a.hist_A[((int64_t)it * K * K + q) * a.batch + b] = v;
+        if (last && a.A_alpha) a.A_alpha[(int64_t)q * a.batch + b] = v;
+    }
+}
+
 // One chain.  fsh / dsh: this thread's shared memory, slot q at [q * ss]; fsh holds B~ [M][K] (fp32), dsh the transition
 // counts [K][K] then the emission counts [M][K] (fp64).  Returns the status code (0, ST_BAD_SYMBOL or ST_NAN).
 template <int K>
@@ -122,17 +160,7 @@ RXG_HD int chain(int64_t b, const Args& a, float* fsh, double* dsh, int ss) {
     for (int it = 0; it < a.iters; ++it) {
         const bool last = it == a.iters - 1;
         // ---- A~, B~ from q(A), q(B): the initial marginals, then prior + counts of the previous sweep
-        if (a.learn_A) {
-            const double* ai = prm + off_Ai(K);
-            for (int q = 0; q < K * K; ++q) xi64[q * ss] = it == 0 ? ai[q] : pA[q] + xi64[q * ss];   // alpha, in place
-            for (int j = 0; j < K; ++j)
-                elog_column([&](int r, int c) { return xi64[(r * K + c) * ss]; }, K, j,
-                            [&](int r, double e) { xi64[(r * K + j) * ss] = e; });
-#pragma unroll
-            for (int i = 0; i < K; ++i)
-#pragma unroll
-                for (int j = 0; j < K; ++j) At[i][j] = (float)exp(xi64[(i * K + j) * ss]);
-        }
+        if (a.learn_A) a_tilde<K>(a, it, xi64, ss, At);
         if (a.learn_B) {
             const double* bi = prm + off_Bi(K, M);
             for (int q = 0; q < M * K; ++q) nB64[q * ss] = it == 0 ? bi[q] : pB[q] + nB64[q * ss];
@@ -234,21 +262,7 @@ RXG_HD int chain(int64_t b, const Args& a, float* fsh, double* dsh, int ss) {
 
         // ---- conjugate updates (alpha = alpha0 + counts, kept as counts in shared memory) and the free energy
         double F = -logZ;
-        if (a.learn_A) {
-            F += log_beta_terms(pA, [&](int r, int c) { return xi64[(r * K + c) * ss]; }, K, K);
-#pragma unroll
-            for (int i = 0; i < K; ++i)
-#pragma unroll
-                for (int j = 0; j < K; ++j) {                // At > 0 wherever the count is (it is proportional to At)
-                    const double n = xi64[(i * K + j) * ss];
-                    if (n > 0.0) F += n * log((double)At[i][j]);
-                }
-            for (int q = 0; q < K * K; ++q) {
-                const float v = (float)(pA[q] + xi64[q * ss]);
-                if (a.hist_A) a.hist_A[((int64_t)it * K * K + q) * nb + b] = v;
-                if (last && a.A_alpha) a.A_alpha[(int64_t)q * nb + b] = v;
-            }
-        }
+        if (a.learn_A) a_terms<K>(a, it, last, b, xi64, ss, At, F);
         if (a.learn_B) {
             F += log_beta_terms(pB, [&](int r, int c) { return nB64[(r * K + c) * ss]; }, M, K);
             for (int q = 0; q < M * K; ++q) {

@@ -56,26 +56,6 @@ int launch_k(rxg_ctx* ctx, int K, const rxg::hmmg::Args& a, int32_t* status) {
     }
 }
 
-// columns of a [rows][K] matrix each a probability vector (non-negative, finite, sum 1 within 1e-5), as rxg_hmm.cu checks
-bool stochastic_columns(const float* p, int rows, int K) {
-    for (int j = 0; j < K; ++j) {
-        double s = 0.0;
-        for (int i = 0; i < rows; ++i) {
-            const float v = p[i * K + j];
-            if (!(v >= 0.f) || !std::isfinite(v)) return false;
-            s += v;
-        }
-        if (std::fabs(s - 1.0) > 1e-5) return false;
-    }
-    return true;
-}
-
-bool positive(const float* p, int n) {
-    for (int i = 0; i < n; ++i)
-        if (!(p[i] > 0.f) || !std::isfinite(p[i])) return false;
-    return true;
-}
-
 }  // namespace
 
 extern "C" int rxg_hmm_gauss_vmp_f32(rxg_ctx* ctx, int d, int K, int T, int64_t batch, int iterations, const float* p0,
@@ -97,53 +77,22 @@ extern "C" int rxg_hmm_gauss_vmp_f32(rxg_ctx* ctx, int d, int K, int T, int64_t 
     const bool learn_A = A_prior || A_init;
     if (learn_A == (A_known != nullptr) || (learn_A && !(A_prior && A_init)))
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_gauss_vmp: pass either A_prior and A_init (A learned) or A_known");
-    if (!stochastic_columns(p0, K, 1))
+    if (!rxg::stochastic_columns(p0, K, 1))
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_gauss_vmp: p0 is not a probability vector");
-    if (learn_A ? !(positive(A_prior, K * K) && positive(A_init, K * K)) : !stochastic_columns(A_known, K, K))
+    if (learn_A ? !(rxg::positive(A_prior, K * K) && rxg::positive(A_init, K * K)) : !rxg::stochastic_columns(A_known, K, K))
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, learn_A ? "hmm_gauss_vmp: A_prior and A_init must be positive"
                                                         : "hmm_gauss_vmp: the columns of A_known must be probability vectors");
-    const Layout LY = layout(d);
-    const int dd = d * d;
+    const int blk = layout(d).blk;
     double hp[8 + 2 * 64 + 8 * (3 * 4 + 4 * 16 + 5)];
     for (int i = 0; i < K; ++i) hp[i] = p0[i];
     for (int q = 0; q < K * K; ++q) {
         hp[K + q] = learn_A ? A_prior[q] : A_known[q];
         hp[K + K * K + q] = learn_A ? A_init[q] : 0.0;
     }
-    for (int k = 0; k < K; ++k) {          // the emission constants in the layout of rxg_gmm_vmp_f32's blocks
-        double* pk = hp + off_states(K) + k * LY.blk;
-        if (!(nu0[k] > (float)(d - 1)) || !(nu_init[k] > (float)(d - 1)) || !std::isfinite(nu0[k]) || !std::isfinite(nu_init[k]))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_gauss_vmp: nu0 and nu_init must exceed d - 1 (state %d)", k);
-        for (int i = 0; i < d; ++i)
-            if (!std::isfinite(mu0[k * d + i]) || !std::isfinite(m_init[k * d + i]))
-                return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_gauss_vmp: mu0 and m_init must be finite (state %d)", k);
-        double ld, tmp[16];
-        if (!rxg::host_spd_inv(V0 + k * dd, d, pk + LY.V0i, &ld))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_gauss_vmp: V0[%d] is not SPD", k);
-        pk[LY.ldV0] = ld;
-        if (!rxg::host_spd_inv(S0 + k * dd, d, pk + LY.S0i, &ld))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_gauss_vmp: S0[%d] is not SPD", k);
-        pk[LY.ldS0] = ld;
-        if (!rxg::host_spd_inv(Vm_init + k * dd, d, tmp, &ld))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_gauss_vmp: Vm_init[%d] is not SPD", k);
-        for (int i = 0; i < d; ++i)
-            for (int j = 0; j < d; ++j)
-                pk[LY.Vi + i * d + j] = 0.5 * ((double)Vm_init[k * dd + i * d + j] + (double)Vm_init[k * dd + j * d + i]);
-        if (!rxg::host_spd_inv(S_init + k * dd, d, pk + LY.iSi, &ld))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "hmm_gauss_vmp: S_init[%d] is not SPD", k);
-        for (int i = 0; i < d; ++i) {
-            pk[LY.mu0 + i] = mu0[k * d + i];
-            pk[LY.mi + i] = m_init[k * d + i];
-            double s = 0.0;
-            for (int j = 0; j < d; ++j) s += pk[LY.V0i + i * d + j] * (double)mu0[k * d + j];
-            pk[LY.xi0 + i] = s;
-        }
-        pk[LY.nu0] = nu0[k];
-        pk[LY.nui] = nu_init[k];
-        double lgd = 0.25 * d * (d - 1) * LOGPI;
-        for (int i = 0; i < d; ++i) lgd += std::lgamma(0.5 * ((double)nu0[k] - i));
-        pk[LY.lgd0] = lgd;
-    }
+    for (int k = 0; k < K; ++k)
+        if (int rc = pack(ctx, "hmm_gauss_vmp", "state", k, d, mu0, V0, nu0, S0, m_init, Vm_init, nu_init, S_init,
+                          hp + off_states(K) + k * blk))
+            return rc;
     RXG_CUDA(ctx, cudaSetDevice(ctx->device));
     const size_t nbytes = (size_t)n_params(K, d) * sizeof(double);
     double* dp = (double*)rxg::workspace(ctx, nbytes);

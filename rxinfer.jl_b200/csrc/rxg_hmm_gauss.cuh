@@ -15,8 +15,8 @@
 //   backward: as rxg_hmm.cuh (the transition counts in fp32 registers flushed into fp64), the emission weights recomputed
 //             from y; the Gaussian statistics N_k = sum gamma, b_k = sum gamma (y - c_k), C_k = sum gamma (y - c_k)(y - c_k)'
 //             around the centre the sweep used, and S = sum_t sum_k gamma_tk (l_k(y_t) - max), all fp64;
-//   updates:  q(A) = Dirichlet(alpha_A0 + sum xi); q(m_k) with the sweep's E[W_k]; q(W_k) with the new q(m_k) (the
-//             order of rxg_mixture.cu, in fp64, C_k moved to the new mean through delta = E[m_k]new - c_k);
+//   updates:  q(A) = Dirichlet(alpha_A0 + sum xi) (rxg_hmm.cuh); q(m_k) with the sweep's E[W_k]; q(W_k) with the new
+//             q(m_k) (the component of rxg_mixture.cu, rxg_normal_wishart.cuh);
 //   free energy, fp64: F = -sum_t log c_t + S + [A terms of rxg_hmm.cuh] + sum_k [KL(q(m_k)||p) + KL(q(W_k)||p) +
 //             N_k (d/2 log 2 pi - 1/2 E_new log|W_k|) + 1/2 tr(E_new[W_k] (R_k + N_k V_k))].  -sum log c_t + S is
 //             -log Z~ + sum gamma l_used with the per-step shifts cancelled exactly (they are never added), so the fp32
@@ -28,34 +28,21 @@
 #include <math.h>
 #include <stdint.h>
 
-#include "rxg_hmm.cuh"      // RXG_HD, hmm::digamma, hmm::elog_column, hmm::log_beta_terms
+#include "rxg_hmm.cuh"              // RXG_HD, hmm::FLUSH, hmm::a_tilde, hmm::a_terms
+#include "rxg_normal_wishart.cuh"
 
 namespace rxg {
 namespace hmmg {
 
-constexpr double LOG2PI = 1.8378770664093453;
-constexpr double LOGPI = 1.1447298858494002;
-constexpr double LOG2 = 0.6931471805599453;
+using namespace nw;                                        // the component: layout, derive, update, store
 constexpr int ST_BAD_ARG = 1, ST_NOT_SPD = 4, ST_NAN = 5;    // RXG_ERR_BAD_ARG, RXG_ERR_NOT_SPD, RXG_ERR_NAN
 
-RXG_HD constexpr int packed(int d) { return d * (d + 1) / 2; }
-RXG_HD constexpr int acc_slots(int d) { return 1 + d + packed(d); }      // N_k, b_k, C_k (lower), fp64
-RXG_HD constexpr int st_slots(int d) { return d + packed(d) + 1; }       // c_k, E[W_k] (lower, doubled), offset, fp32
 // Where the fp32 transition partials live: registers up to K = 4; from K = 5 on, K x K fp32 shared-memory slots after the
 // sweep constants, since in registers they spill at K >= 5 for d >= 3 and K >= 6 for d = 2 (DESIGN 3.20)
 RXG_HD constexpr bool u_shared(int /*d*/, int K) { return K >= 5; }
 RXG_HD constexpr int f_slots(int d, int K) { return K * st_slots(d) + (u_shared(d, K) ? K * K : 0); }
 
-// fp64 host constants: p0[K], A (prior alpha or known matrix) [K][K], A_init [K][K], then one block of blk doubles per state:
-// mu0, inv(V0), inv(V0) mu0, log|V0|, inv(S0), log|S0|, nu0, log Gamma_d(nu0 / 2), m_init, Vm_init, nu_init, inv(S_init)
-struct Layout {
-    int mu0, V0i, xi0, ldV0, S0i, ldS0, nu0, lgd0, mi, Vi, nui, iSi, blk;
-};
-RXG_HD constexpr Layout layout(int d) {
-    const int dd = d * d;
-    return Layout{0, d, d + dd, 2 * d + dd, 2 * d + dd + 1, 2 * d + 2 * dd + 1, 2 * d + 2 * dd + 2, 2 * d + 2 * dd + 3,
-                  2 * d + 2 * dd + 4, 3 * d + 2 * dd + 4, 3 * d + 3 * dd + 4, 3 * d + 3 * dd + 5, 3 * d + 4 * dd + 5};
-}
+// fp64 host constants: p0[K], A (prior alpha or known matrix) [K][K], A_init [K][K], then one nw::Layout block per state
 RXG_HD int off_states(int K) { return K + 2 * K * K; }
 RXG_HD int n_params(int K, int d) { return off_states(K) + K * layout(d).blk; }
 
@@ -72,87 +59,6 @@ struct Args {
     double* fe;                              // [iters][batch]
     float *hist_s, *hist_A, *hist_m_mean, *hist_m_cov, *hist_w_df, *hist_w_inv_scale;
 };
-
-// inv(A) and log|A| of a D x D SPD matrix (row-major, fp64) from one Cholesky factorisation; false at a non-positive (or
-// NaN) pivot.  rxg_linalg.cuh's cholesky and the mixture's inv_logdet are device-only, and this body is also compiled for
-// the host (tests/c/hmm_gauss_host_harness.cu), so the d <= 4 factorisation is written here once for both.
-template <int D>
-RXG_HD bool spd_inv(const double* A, double* Ai, double& logdet) {
-    double L[D][D], Li[D][D];
-    logdet = 0.0;
-#pragma unroll
-    for (int j = 0; j < D; ++j) {
-        double s = A[j * D + j];
-#pragma unroll
-        for (int k = 0; k < j; ++k) s -= L[j][k] * L[j][k];
-        if (!(s > 0.0)) {
-            for (int i = 0; i < D * D; ++i) Ai[i] = NAN;
-            return false;
-        }
-        L[j][j] = sqrt(s);
-        logdet += 2.0 * log(L[j][j]);
-        const double r = 1.0 / L[j][j];
-#pragma unroll
-        for (int i = j + 1; i < D; ++i) {
-            double t = A[i * D + j];
-#pragma unroll
-            for (int k = 0; k < j; ++k) t -= L[i][k] * L[j][k];
-            L[i][j] = t * r;
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < D; ++j) {                          // L^-1 (lower), column by column
-        Li[j][j] = 1.0 / L[j][j];
-#pragma unroll
-        for (int i = j + 1; i < D; ++i) {
-            double s = 0.0;
-#pragma unroll
-            for (int k = j; k < i; ++k) s += L[i][k] * Li[k][j];
-            Li[i][j] = -s / L[i][i];
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < D; ++i)                            // L^-T L^-1
-#pragma unroll
-        for (int j = 0; j <= i; ++j) {
-            double s = 0.0;
-#pragma unroll
-            for (int k = i; k < D; ++k) s += Li[k][i] * Li[k][j];
-            Ai[i * D + j] = s;
-            Ai[j * D + i] = s;
-        }
-    return true;
-}
-
-template <int D>
-RXG_HD double lgamma_mv(double a) {                       // log Gamma_D(a)
-    double s = 0.25 * D * (D - 1) * LOGPI;
-    for (int i = 0; i < D; ++i) s += lgamma(a - 0.5 * i);
-    return s;
-}
-
-// From q(m_k) = N(m, Vm) and q(W_k) = Wishart(nu, inv(iS)): the fp32 constants of the sweep into st (slot q at st[q * ss])
-// and E[W_k] into EW; returns E[log|W_k|].
-template <int D>
-RXG_HD double derive(const double* m, const double* Vm, double nu, const double* iS, float* st, int ss, bool& bad,
-                     double* EW) {
-    double S[D * D], ldiS;
-    if (!spd_inv<D>(iS, S, ldiS)) bad = true;
-    double elog = D * LOG2 - ldiS;                                              // log|S| = -log|iS|
-    for (int i = 0; i < D; ++i) elog += hmm::digamma(0.5 * (nu - i));
-    double tr = 0.0;
-#pragma unroll
-    for (int i = 0; i < D * D; ++i) { EW[i] = nu * S[i]; tr += EW[i] * Vm[i]; }
-#pragma unroll
-    for (int i = 0; i < D; ++i) st[i * ss] = (float)m[i];
-    int p = D;
-#pragma unroll
-    for (int i = 0; i < D; ++i)
-#pragma unroll
-        for (int j = 0; j <= i; ++j, ++p) st[p * ss] = (float)((i == j ? 1.0 : 2.0) * EW[i * D + j]);
-    st[p * ss] = (float)(0.5 * elog - 0.5 * D * LOG2PI - 0.5 * tr);
-    return elog;
-}
 
 // y_t of chain b into v; false for a missing step (all d components NaN, or any non-finite one, which also flags the chain)
 template <int D>
@@ -234,15 +140,7 @@ RXG_HD int chain(int64_t b, const Args& a, float* fsh, double* dsh, int ss) {
 #pragma unroll
                 for (int j = 0; j < K; ++j) At[i][j] = (float)pA[i * K + j];
         } else {
-            const double* ai = prm + K + K * K;
-            for (int q = 0; q < K * K; ++q) xi64[q * ss] = it == 0 ? ai[q] : pA[q] + xi64[q * ss];   // alpha, in place
-            for (int j = 0; j < K; ++j)
-                hmm::elog_column([&](int r, int c) { return xi64[(r * K + c) * ss]; }, K, j,
-                                 [&](int r, double e) { xi64[(r * K + j) * ss] = e; });
-#pragma unroll
-            for (int i = 0; i < K; ++i)
-#pragma unroll
-                for (int j = 0; j < K; ++j) At[i][j] = (float)exp(xi64[(i * K + j) * ss]);
+            hmm::a_tilde<K>(a, it, xi64, ss, At);
         }
         for (int q = 0; q < K * K; ++q) xi64[q * ss] = 0.0;
         for (int q = 0; q < K * SA; ++q) acc[q * ss] = 0.0;
@@ -360,119 +258,15 @@ RXG_HD int chain(int64_t b, const Args& a, float* fsh, double* dsh, int ss) {
             for (int j = 0; j < K; ++j) a.s0_prob[(int64_t)j * nb + b] = p0[j] * be[j];
         }
 
-        // ---- q(A); the A terms of the free energy as in rxg_hmm.cuh
+        // ---- q(A) and its free-energy terms; q(m_k) with the sweep's E[W_k], q(W_k) with the new q(m_k), and theirs
         double F = Sl - logc;
-        if (a.learn_A) {
-            F += hmm::log_beta_terms(pA, [&](int r, int c) { return xi64[(r * K + c) * ss]; }, K, K);
-#pragma unroll
-            for (int i = 0; i < K; ++i)
-#pragma unroll
-                for (int j = 0; j < K; ++j) {
-                    const double n = xi64[(i * K + j) * ss];
-                    if (n > 0.0) F += n * log((double)At[i][j]);
-                }
-            for (int q = 0; q < K * K; ++q) {
-                const float v = (float)(pA[q] + xi64[q * ss]);
-                if (a.hist_A) a.hist_A[((int64_t)it * K * K + q) * nb + b] = v;
-                if (last && a.A_alpha) a.A_alpha[(int64_t)q * nb + b] = v;
-            }
-        }
-        // ---- q(m_k) with the sweep's E[W_k], q(W_k) with the new q(m_k); their free-energy terms (rxg_mixture.cu)
+        if (a.learn_A) hmm::a_terms<K>(a, it, last, b, xi64, ss, At, F);
 #pragma unroll 1
         for (int k = 0; k < K; ++k) {
-            const double* pk = ps + k * LY.blk;
-            const double* ak = acc + k * SA * ss;
-            float* sk = fsh + k * SS * ss;
-            const double Nk = ak[0];
-            double c[D], bk[D], EW[D * D], Ck[D * D];
-#pragma unroll
-            for (int i = 0; i < D; ++i) { c[i] = (double)sk[i * ss]; bk[i] = ak[(1 + i) * ss]; }
-            int p = D, pc = 1 + D;
-#pragma unroll
-            for (int i = 0; i < D; ++i)
-#pragma unroll
-                for (int j = 0; j <= i; ++j, ++p, ++pc) {
-                    const double w = (double)sk[p * ss] * (i == j ? 1.0 : 0.5);
-                    EW[i * D + j] = w; EW[j * D + i] = w;
-                    Ck[i * D + j] = ak[pc * ss]; Ck[j * D + i] = Ck[i * D + j];
-                }
-            // q(m_k): precision inv(V0) + N_k E[W_k], weighted mean inv(V0) mu0 + E[W_k] sum_t gamma_tk y_t
-            double Lm[D * D], Vm[D * D], sy[D], xi[D], m[D], ldL;
-#pragma unroll
-            for (int i = 0; i < D * D; ++i) Lm[i] = pk[LY.V0i + i] + Nk * EW[i];
-#pragma unroll
-            for (int i = 0; i < D; ++i) sy[i] = bk[i] + Nk * c[i];
-            if (!spd_inv<D>(Lm, Vm, ldL)) bad = true;                       // ldL = log|Lm| = -log|Vm|
-#pragma unroll
-            for (int i = 0; i < D; ++i) {
-                double s = pk[LY.xi0 + i];
-#pragma unroll
-                for (int j = 0; j < D; ++j) s += EW[i * D + j] * sy[j];
-                xi[i] = s;
-            }
-#pragma unroll
-            for (int i = 0; i < D; ++i) {
-                double s = 0.0;
-#pragma unroll
-                for (int j = 0; j < D; ++j) s += Vm[i * D + j] * xi[j];
-                m[i] = s;
-            }
-            // q(W_k): nu0 + N_k, inverse scale inv(S0) + R_k + N_k Vm, R_k = sum_t gamma_tk (y_t - m)(y_t - m)'
-            double dm[D], R[D * D], iS[D * D];
-#pragma unroll
-            for (int i = 0; i < D; ++i) dm[i] = m[i] - c[i];
-#pragma unroll
-            for (int i = 0; i < D; ++i)
-#pragma unroll
-                for (int j = 0; j < D; ++j) {
-                    R[i * D + j] = Ck[i * D + j] - bk[i] * dm[j] - dm[i] * bk[j] + Nk * dm[i] * dm[j];
-                    iS[i * D + j] = pk[LY.S0i + i * D + j] + R[i * D + j] + Nk * Vm[i * D + j];
-                }
-            const double nu = pk[LY.nu0] + Nk;
-            double EWn[D * D];
-            const double elog = derive<D>(m, Vm, nu, iS, sk, ss, bad, EWn);
-            double trV = 0.0, quad = 0.0, trS = 0.0, trR = 0.0, e[D];
-#pragma unroll
-            for (int i = 0; i < D; ++i) e[i] = m[i] - pk[LY.mu0 + i];
-#pragma unroll
-            for (int i = 0; i < D; ++i)
-#pragma unroll
-                for (int j = 0; j < D; ++j) {
-                    const double v0i = pk[LY.V0i + i * D + j];
-                    trV += v0i * Vm[j * D + i];
-                    quad += e[i] * v0i * e[j];
-                    trS += pk[LY.S0i + i * D + j] * EWn[j * D + i];             // nu tr(inv(S0) S)
-                    trR += EWn[i * D + j] * (R[j * D + i] + Nk * Vm[j * D + i]);
-                }
-            const double nu0 = pk[LY.nu0];
-            double psum = 0.0;
-            for (int i = 0; i < D; ++i) psum += hmm::digamma(0.5 * (nu - i));
-            const double logdetS = elog - D * LOG2 - psum;                        // log|S| of the new q(W_k)
-            const double kl_m = 0.5 * (trV + quad - D + pk[LY.ldV0] + ldL);
-            const double kl_w = 0.5 * (nu - nu0) * elog - 0.5 * nu * D + 0.5 * trS - 0.5 * (nu - nu0) * D * LOG2
-                                - 0.5 * nu * logdetS + 0.5 * nu0 * pk[LY.ldS0] - lgamma_mv<D>(0.5 * nu) + pk[LY.lgd0];
-            F += kl_m + kl_w + Nk * (0.5 * D * LOG2PI - 0.5 * elog) + 0.5 * trR;
-            // outputs
-            if (a.hist_w_df) a.hist_w_df[((int64_t)it * K + k) * nb + b] = (float)nu;
-#pragma unroll
-            for (int i = 0; i < D; ++i)
-                if (a.hist_m_mean) a.hist_m_mean[(((int64_t)it * K + k) * D + i) * nb + b] = (float)m[i];
-#pragma unroll
-            for (int i = 0; i < D * D; ++i) {
-                if (a.hist_m_cov) a.hist_m_cov[(((int64_t)it * K + k) * D * D + i) * nb + b] = (float)Vm[i];
-                if (a.hist_w_inv_scale) a.hist_w_inv_scale[(((int64_t)it * K + k) * D * D + i) * nb + b] = (float)iS[i];
-            }
-            if (last) {
-                if (a.w_df) a.w_df[(int64_t)k * nb + b] = (float)nu;
-#pragma unroll
-                for (int i = 0; i < D; ++i)
-                    if (a.m_mean) a.m_mean[((int64_t)k * D + i) * nb + b] = (float)m[i];
-#pragma unroll
-                for (int i = 0; i < D * D; ++i) {
-                    if (a.m_cov) a.m_cov[((int64_t)k * D * D + i) * nb + b] = (float)Vm[i];
-                    if (a.w_inv_scale) a.w_inv_scale[((int64_t)k * D * D + i) * nb + b] = (float)iS[i];
-                }
-            }
+            double m[D], Vm[D * D], nu, iS[D * D];
+            F += update<D>(ps + k * LY.blk, acc + k * SA * ss, fsh + k * SS * ss, ss, bad, m, Vm, nu, iS);
+            store<D>((int64_t)it * K + k, nb, b, m, Vm, nu, iS, a.hist_m_mean, a.hist_m_cov, a.hist_w_df, a.hist_w_inv_scale);
+            if (last) store<D>(k, nb, b, m, Vm, nu, iS, a.m_mean, a.m_cov, a.w_df, a.w_inv_scale);
         }
         if (bad && !status) status = ST_NOT_SPD;
         if (a.fe) a.fe[(int64_t)it * nb + b] = F;

@@ -72,6 +72,9 @@ void* workspace(rxg_ctx* ctx, size_t bytes);
 // host: fp64 Cholesky of the symmetrised (A + A')/2 of an n x n matrix (n <= 16), then its inverse; false if it is not
 // symmetric positive definite (or not finite); log det on success
 bool host_spd_inv(const float* a, int n, double* inv, double* logdet);
+// rxg_hmm.cu: host checks of the HMM entries' probability arrays and Dirichlet parameters
+bool stochastic_columns(const float* p, int rows, int K);
+bool positive(const float* p, int n);
 void* staging(rxg_ctx* ctx, size_t bytes);
 // rxg_hgf.cu: the 31 Gauss-Hermite nodes and weights (physicists' convention), fp64
 void gauss_hermite_31(double* t, double* w);

@@ -7,50 +7,25 @@
 // responsibilities r[i][k] from the previous q(s), q(m), q(W), then the per-component statistics N_k, sum r (y - c_k),
 // sum r (y - c_k)(y - c_k)' accumulated in fp64 around c_k = the previous E[m_k] (the points sit near their cluster's
 // mean, so nothing cancels when the data are far from the origin), then the O(K d^3) conjugate updates in fp64 in the
-// order q(m) (previous E[W]), q(W) (new q(m)), q(s) (DESIGN 3.17), then the Bethe free energy in fp64.
+// order q(m) (previous E[W]), q(W) (new q(m)) (rxg_normal_wishart.cuh), q(s) (DESIGN 3.17), then the Bethe free energy
+// in fp64.
 // Shared memory per thread, laid out [slot][thread]: the fp64 accumulators and the fp32 per-component constants the
 // data pass reads (centre, packed E[W], log-weight offset).  At K = 8, d = 4 that is 120 + 120 slots.
 #include <cfloat>
 #include <cmath>
 
 #include "rxg_internal.h"
-#include "rxg_linalg.cuh"
+#include "rxg_normal_wishart.cuh"
 
 namespace rxg {
 namespace gmm {
 
 constexpr int TPB = 64;                       // threads (chains) per block
-constexpr double LOG2PI = 1.8378770664093453;
-constexpr double LOGPI = 1.1447298858494002;
+using namespace nw;                           // the component: layout, derive, update, store, digamma
 
-__host__ __device__ constexpr int packed(int d) { return d * (d + 1) / 2; }
-__host__ __device__ constexpr int acc_slots(int d) { return 1 + d + packed(d); }      // N_k, b_k, C_k (lower)
-__host__ __device__ constexpr int st_slots(int d) { return d + packed(d) + 1; }       // c_k, E[W_k] (lower), cst_k
-
-// fp64 host constants, per component k (block of blk(d) doubles), then two global values
-struct Layout {
-    int mu0, V0i, xi0, ldV0, S0i, ldS0, nu0, a0, lgd0, ai, mi, Vi, nui, iSi, blk;
-};
-__host__ __device__ constexpr Layout layout(int d) {
-    const int dd = d * d;
-    return Layout{0, d, d + dd, 2 * d + dd, 2 * d + dd + 1, 2 * d + 2 * dd + 1, 2 * d + 2 * dd + 2, 2 * d + 2 * dd + 3,
-                  2 * d + 2 * dd + 4, 2 * d + 2 * dd + 5, 2 * d + 2 * dd + 6, 3 * d + 2 * dd + 6, 3 * d + 3 * dd + 6,
-                  3 * d + 3 * dd + 7, 3 * d + 4 * dd + 7};
-}
-// after the K blocks: sum(alpha0), lgamma(sum alpha0) - sum lgamma(alpha0)
-
-__device__ __forceinline__ double digamma(double x) {      // psi(x), x > 0: recurrence up to x >= 10, asymptotic series
-    double r = 0.0;
-    while (x < 10.0) { r -= 1.0 / x; x += 1.0; }
-    const double i = 1.0 / x, i2 = i * i;
-    return r + log(x) - 0.5 * i - i2 * (1.0 / 12 - i2 * (1.0 / 120 - i2 * (1.0 / 252 - i2 * (1.0 / 240 - i2 * (1.0 / 132)))));
-}
-template <int D>
-__host__ __device__ inline double lgamma_mv(double a) {   // log Gamma_D(a)
-    double s = 0.25 * D * (D - 1) * LOGPI;
-    for (int i = 0; i < D; ++i) s += lgamma(a - 0.5 * i);
-    return s;
-}
+// fp64 host constants: one nw::Layout block per component, then alpha0[K], alpha_init[K], sum(alpha0),
+// lgamma(sum alpha0) - sum lgamma(alpha0)
+inline int n_params(int K, int d) { return K * layout(d).blk + 2 * K + 2; }
 
 struct Out {
     float *alpha, *m_mean, *m_cov, *w_df, *w_inv_scale;
@@ -59,63 +34,6 @@ struct Out {
     float *h_alpha, *h_m_mean, *h_m_cov, *h_w_df, *h_w_inv_scale;
     int32_t* status;
 };
-
-// inv(A) and log|A| of an SPD matrix from one Cholesky factorisation (cholinv's inverse, rxg_linalg.cuh)
-template <int D>
-__device__ __forceinline__ Mat<double, D, D> inv_logdet(const Mat<double, D, D>& A, double& logdet, bool& bad) {
-    const Chol<double, D> c = cholesky<double, D, true>(A, bad);
-    logdet = -2.0 * c.neg_half_logdet;
-    Mat<double, D, D> Li;                                   // L^-1 (lower), column by column
-#pragma unroll
-    for (int i = 0; i < D * D; ++i) Li.a[i] = 0.0;
-#pragma unroll
-    for (int j = 0; j < D; ++j) {
-        Li(j, j) = c.L(j, j);
-#pragma unroll
-        for (int i = j + 1; i < D; ++i) {
-            double s = 0.0;
-#pragma unroll
-            for (int k = j; k < i; ++k) s = fma(-c.L(i, k), Li(k, j), s);
-            Li(i, j) = s * c.L(i, i);
-        }
-    }
-    Mat<double, D, D> o;                                    // L^-T L^-1
-#pragma unroll
-    for (int i = 0; i < D; ++i)
-#pragma unroll
-        for (int j = 0; j <= i; ++j) {
-            double s = 0.0;
-#pragma unroll
-            for (int k = i; k < D; ++k) s = fma(Li(k, i), Li(k, j), s);
-            o(i, j) = s;
-            o(j, i) = s;
-        }
-    return o;
-}
-
-// From q(m_k) = N(m, Vm) and q(W_k) = Wishart(nu, inv(iS)): the fp32 constants of the data pass (without the
-// E[log s_k] term, added once every alpha is known); returns E[log|W_k|].
-template <int D>
-__device__ __forceinline__ double derive(const Vec<double, D>& m, const Mat<double, D, D>& Vm, double nu,
-                                         const Mat<double, D, D>& iS, float* st, int tid, bool& bad,
-                                         Mat<double, D, D>& EW) {
-    double ldiS;
-    const Mat<double, D, D> S = inv_logdet(iS, ldiS, bad);
-    double elog = D * 0.6931471805599453 - ldiS;                              // log|S| = -log|iS|
-    for (int i = 0; i < D; ++i) elog += digamma(0.5 * (nu - i));
-    double tr = 0.0;
-#pragma unroll
-    for (int i = 0; i < D * D; ++i) { EW.a[i] = nu * S.a[i]; tr += EW.a[i] * Vm.a[i]; }
-#pragma unroll
-    for (int i = 0; i < D; ++i) st[i * TPB + tid] = (float)m(i);
-    int p = D;
-#pragma unroll
-    for (int i = 0; i < D; ++i)
-#pragma unroll
-        for (int j = 0; j <= i; ++j, ++p) st[p * TPB + tid] = (float)((i == j ? 1.0 : 2.0) * EW(i, j));   // off-diagonal doubled
-    st[p * TPB + tid] = (float)(0.5 * elog - 0.5 * D * LOG2PI - 0.5 * tr);
-    return elog;
-}
 
 template <int D, int K>
 __global__ void __launch_bounds__(TPB)
@@ -128,8 +46,13 @@ gmm_vmp_kernel(const float* __restrict__ y, int N, int64_t batch, int iters, con
     const int tid = threadIdx.x;
     const int64_t b = (int64_t)blockIdx.x * TPB + tid;
     if (b >= batch) return;
-    bool bad = false;
-    const double sum_a0 = prm[K * LY.blk], lg_dir0 = prm[K * LY.blk + 1];
+    // Status: RXG_ERR_NOT_SPD from the first non-positive pivot on, else RXG_OK.  At d = 1 it is written when a pivot
+    // fails, since a flag kept through the kernel is spilled there around the fp64 slow-path calls of the updates; the
+    // other sizes keep the flag, which at d = 4, K = 8 keeps the data pass faster (82 against 90 ms, DESIGN 3.17).
+    constexpr bool EAGER = D == 1;
+    bool bad = false, bk = false;
+    if (EAGER && o.status) o.status[b] = RXG_OK;
+    const double* a0 = prm + K * LY.blk;                       // alpha0[K], alpha_init[K], sum(alpha0), normaliser
 
     // initial q(s), q(m), q(W) -> constants of the first data pass
     {
@@ -137,17 +60,14 @@ gmm_vmp_kernel(const float* __restrict__ y, int N, int64_t batch, int iters, con
 #pragma unroll 1
         for (int k = 0; k < K; ++k) {
             const double* pk = prm + k * LY.blk;
-            Vec<double, D> m;
-            Mat<double, D, D> Vm, iS, EW;
-            for (int i = 0; i < D; ++i) m(i) = pk[LY.mi + i];
-            for (int i = 0; i < D * D; ++i) { Vm.a[i] = pk[LY.Vi + i]; iS.a[i] = pk[LY.iSi + i]; }
-            derive<D>(m, Vm, pk[LY.nui], iS, st + k * SS * TPB, tid, bad, EW);
-            sa += pk[LY.ai];
+            double EW[D * D];
+            derive<D>(pk + LY.mi, pk + LY.Vi, pk[LY.nui], pk + LY.iSi, st + k * SS * TPB + tid, TPB, EAGER ? bk : bad, EW);
+            if (EAGER && bk && o.status) o.status[b] = RXG_ERR_NOT_SPD;
+            sa += a0[K + k];
         }
         const double psa = digamma(sa);
 #pragma unroll 1
-        for (int k = 0; k < K; ++k)
-            st[(k * SS + SS - 1) * TPB + tid] += (float)(digamma(prm[k * LY.blk + LY.ai]) - psa);
+        for (int k = 0; k < K; ++k) st[(k * SS + SS - 1) * TPB + tid] += (float)(digamma(a0[K + k]) - psa);
     }
 
     for (int it = 0; it < iters; ++it) {
@@ -202,119 +122,38 @@ gmm_vmp_kernel(const float* __restrict__ y, int N, int64_t batch, int iters, con
             }
         }
         // ---- q(m_k), q(W_k) per component, then q(s); the free energy with the new marginals
-        double fe = -Hz, sa = sum_a0;
+        double fe = -Hz, sa = a0[2 * K];
 #pragma unroll 1
         for (int k = 0; k < K; ++k) {
-            const double* pk = prm + k * LY.blk;
-            const double* ak = acc + k * SA * TPB + tid;
-            float* sk = st + k * SS * TPB;
-            const double Nk = ak[0];
+            const double Nk = acc[k * SA * TPB + tid];
             sa += Nk;
-            Vec<double, D> c, bk;
-            Mat<double, D, D> EW, Ck;
-#pragma unroll
-            for (int i = 0; i < D; ++i) { c(i) = (double)sk[i * TPB + tid]; bk(i) = ak[(1 + i) * TPB]; }
-            int p = D, pc = 1 + D;
-#pragma unroll
-            for (int i = 0; i < D; ++i)
-#pragma unroll
-                for (int j = 0; j <= i; ++j, ++p, ++pc) {
-                    const double w = (double)sk[p * TPB + tid] * (i == j ? 1.0 : 0.5);
-                    EW(i, j) = w; EW(j, i) = w;
-                    Ck(i, j) = ak[pc * TPB]; Ck(j, i) = Ck(i, j);
-                }
-            // q(m_k): precision V0^-1 + N_k E[W_k], weighted mean V0^-1 mu0 + E[W_k] sum_i r_ik y_i.  E[W_k] and the centre
-            // c_k are the fp32 constants the data pass used: c_k exactly (the statistics are taken around it), E[W_k]
-            // rounded to fp32 (relative 6e-8, DESIGN 3.17)
-            Mat<double, D, D> Lm;
-            Vec<double, D> sy;
-#pragma unroll
-            for (int i = 0; i < D * D; ++i) Lm.a[i] = pk[LY.V0i + i] + Nk * EW.a[i];
-#pragma unroll
-            for (int i = 0; i < D; ++i) sy(i) = bk(i) + Nk * c(i);
-            double ldL;
-            const Mat<double, D, D> Vm = inv_logdet(Lm, ldL, bad);
-            Vec<double, D> xi = mulv(EW, sy);
-#pragma unroll
-            for (int i = 0; i < D; ++i) xi(i) += pk[LY.xi0 + i];
-            const Vec<double, D> m = mulv(Vm, xi);
-            // q(W_k): nu0 + N_k, inverse scale inv(S0) + R_k + N_k V_m, R_k = sum_i r_ik (y_i - m)(y_i - m)'
-            Vec<double, D> dm;
-#pragma unroll
-            for (int i = 0; i < D; ++i) dm(i) = m(i) - c(i);
-            Mat<double, D, D> R, iS;
-#pragma unroll
-            for (int i = 0; i < D; ++i)
-#pragma unroll
-                for (int j = 0; j < D; ++j) {
-                    R(i, j) = Ck(i, j) - bk(i) * dm(j) - dm(i) * bk(j) + Nk * dm(i) * dm(j);
-                    iS(i, j) = pk[LY.S0i + i * D + j] + R(i, j) + Nk * Vm(i, j);
-                }
-            const double nu = pk[LY.nu0] + Nk;
-            Mat<double, D, D> EWn;
-            const double elog = derive<D>(m, Vm, nu, iS, sk, tid, bad, EWn);
-            // free energy: KL(q(m_k) || prior), KL(q(W_k) || prior), the NormalMixture's average energy on component k
-            double trV = 0.0, quad = 0.0, trS = 0.0, trR = 0.0;
-            Vec<double, D> e;
-#pragma unroll
-            for (int i = 0; i < D; ++i) e(i) = m(i) - pk[LY.mu0 + i];
-#pragma unroll
-            for (int i = 0; i < D; ++i)
-#pragma unroll
-                for (int j = 0; j < D; ++j) {
-                    const double v0i = pk[LY.V0i + i * D + j];
-                    trV += v0i * Vm(j, i);
-                    quad += e(i) * v0i * e(j);
-                    trS += pk[LY.S0i + i * D + j] * EWn(j, i);                 // nu tr(inv(S0) S)
-                    trR += EWn(i, j) * (R(j, i) + Nk * Vm(j, i));
-                }
-            const double nu0 = pk[LY.nu0];
-            double psum = 0.0;
-            for (int i = 0; i < D; ++i) psum += digamma(0.5 * (nu - i));
-            const double logdetS = elog - D * 0.6931471805599453 - psum;            // log|S| of the new q(W_k)
-            const double kl_m = 0.5 * (trV + quad - D + pk[LY.ldV0] + ldL);
-            const double kl_w = 0.5 * (nu - nu0) * elog - 0.5 * nu * D + 0.5 * trS - 0.5 * (nu - nu0) * D * 0.6931471805599453
-                                - 0.5 * nu * logdetS + 0.5 * nu0 * pk[LY.ldS0] - lgamma_mv<D>(0.5 * nu) + pk[LY.lgd0];
-            fe += kl_m + kl_w + Nk * (0.5 * D * LOG2PI - 0.5 * elog) + 0.5 * trR;
-            // outputs
-            const double ak_new = pk[LY.a0] + Nk;
+            double m[D], Vm[D * D], nu, iS[D * D];
+            fe += update<D>(prm + k * LY.blk, acc + k * SA * TPB + tid, st + k * SS * TPB + tid, TPB, EAGER ? bk : bad, m, Vm,
+                            nu, iS);
+            if (EAGER && bk && o.status) o.status[b] = RXG_ERR_NOT_SPD;
+            const double ak_new = a0[k] + Nk;
             if (o.h_alpha) o.h_alpha[((int64_t)it * K + k) * batch + b] = (float)ak_new;
-            if (o.h_w_df) o.h_w_df[((int64_t)it * K + k) * batch + b] = (float)nu;
-#pragma unroll
-            for (int i = 0; i < D; ++i)
-                if (o.h_m_mean) o.h_m_mean[(((int64_t)it * K + k) * D + i) * batch + b] = (float)m(i);
-#pragma unroll
-            for (int i = 0; i < D * D; ++i) {
-                if (o.h_m_cov) o.h_m_cov[(((int64_t)it * K + k) * D * D + i) * batch + b] = (float)Vm.a[i];
-                if (o.h_w_inv_scale) o.h_w_inv_scale[(((int64_t)it * K + k) * D * D + i) * batch + b] = (float)iS.a[i];
-            }
+            store<D>((int64_t)it * K + k, batch, b, m, Vm, nu, iS, o.h_m_mean, o.h_m_cov, o.h_w_df, o.h_w_inv_scale);
             if (last) {
                 o.alpha[(int64_t)k * batch + b] = (float)ak_new;
-                o.w_df[(int64_t)k * batch + b] = (float)nu;
-#pragma unroll
-                for (int i = 0; i < D; ++i) o.m_mean[((int64_t)k * D + i) * batch + b] = (float)m(i);
-#pragma unroll
-                for (int i = 0; i < D * D; ++i) {
-                    o.m_cov[((int64_t)k * D * D + i) * batch + b] = (float)Vm.a[i];
-                    o.w_inv_scale[((int64_t)k * D * D + i) * batch + b] = (float)iS.a[i];
-                }
+                store<D>(k, batch, b, m, Vm, nu, iS, o.m_mean, o.m_cov, o.w_df, o.w_inv_scale);
             }
         }
         // q(s) = Dirichlet(alpha0 + N); E[log s_k] into the next pass's constants.  KL(q(s) || prior) carries
         // sum_k (alpha_k - alpha0_k) E[log s_k] = sum_k N_k E[log s_k], which cancels the Categorical nodes' average
         // energy -sum_k N_k E[log s_k]: the two add up to the log-normaliser difference alone.
         const double psa = digamma(sa);
-        double lg = lgamma(sa) - lg_dir0;
+        double lg = lgamma(sa) - a0[2 * K + 1];
 #pragma unroll 1
         for (int k = 0; k < K; ++k) {
-            const double a = prm[k * LY.blk + LY.a0] + acc[k * SA * TPB + tid];
+            const double a = a0[k] + acc[k * SA * TPB + tid];
             st[(k * SS + SS - 1) * TPB + tid] += (float)(digamma(a) - psa);
             lg -= lgamma(a);
         }
         fe += lg;
         if (o.free_energy) o.free_energy[(int64_t)it * batch + b] = fe;
     }
-    if (o.status) o.status[b] = bad ? RXG_ERR_NOT_SPD : RXG_OK;
+    if (!EAGER && o.status) o.status[b] = bad ? RXG_ERR_NOT_SPD : RXG_OK;
 }
 
 }  // namespace gmm
@@ -362,55 +201,25 @@ extern "C" int rxg_gmm_vmp_f32(rxg_ctx* ctx, int d, int K, int N, int64_t batch,
     if (N < 1 || batch < 1 || iterations < 1 || !alpha0 || !mu0 || !V0 || !nu0 || !S0 || !alpha_init || !m_init ||
         !Vm_init || !nu_init || !S_init || !y || !alpha || !m_mean || !m_cov || !w_df || !w_inv_scale)
         return rxg::fail(ctx, RXG_ERR_BAD_ARG, "gmm_vmp: bad argument");
-    const rxg::gmm::Layout LY = rxg::gmm::layout(d);
-    const int dd = d * d;
-    double hp[8 * (3 * 4 + 4 * 16 + 7) + 2];
+    const int blk = rxg::nw::layout(d).blk;
+    double hp[8 * (3 * 4 + 4 * 16 + 5) + 2 * 8 + 2];
+    double *a0 = hp + K * blk, *ai = a0 + K;
     double sa0 = 0.0, slg0 = 0.0;
     for (int k = 0; k < K; ++k) {
-        double* pk = hp + k * LY.blk;
         if (!(alpha0[k] > 0.f) || !(alpha_init[k] > 0.f) || !std::isfinite(alpha0[k]) || !std::isfinite(alpha_init[k]))
             return rxg::fail(ctx, RXG_ERR_BAD_ARG, "gmm_vmp: alpha0 and alpha_init must be positive (component %d)", k);
-        if (!(nu0[k] > (float)(d - 1)) || !(nu_init[k] > (float)(d - 1)) || !std::isfinite(nu0[k]) || !std::isfinite(nu_init[k]))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "gmm_vmp: nu0 and nu_init must exceed d - 1 (component %d)", k);
-        for (int i = 0; i < d; ++i)
-            if (!std::isfinite(mu0[k * d + i]) || !std::isfinite(m_init[k * d + i]))
-                return rxg::fail(ctx, RXG_ERR_BAD_ARG, "gmm_vmp: mu0 and m_init must be finite (component %d)", k);
-        double ld, tmp[16];
-        if (!rxg::host_spd_inv(V0 + k * dd, d, pk + LY.V0i, &ld))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "gmm_vmp: V0[%d] is not SPD", k);
-        pk[LY.ldV0] = ld;
-        if (!rxg::host_spd_inv(S0 + k * dd, d, pk + LY.S0i, &ld))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "gmm_vmp: S0[%d] is not SPD", k);
-        pk[LY.ldS0] = ld;
-        if (!rxg::host_spd_inv(Vm_init + k * dd, d, tmp, &ld))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "gmm_vmp: Vm_init[%d] is not SPD", k);
-        for (int i = 0; i < d; ++i)              // symmetrised, as every host matrix is validated
-            for (int j = 0; j < d; ++j) pk[LY.Vi + i * d + j] = 0.5 * ((double)Vm_init[k * dd + i * d + j] + (double)Vm_init[k * dd + j * d + i]);
-        if (!rxg::host_spd_inv(S_init + k * dd, d, pk + LY.iSi, &ld))
-            return rxg::fail(ctx, RXG_ERR_BAD_ARG, "gmm_vmp: S_init[%d] is not SPD", k);
-        for (int i = 0; i < d; ++i) {
-            pk[LY.mu0 + i] = mu0[k * d + i];
-            pk[LY.mi + i] = m_init[k * d + i];
-        }
-        for (int i = 0; i < d; ++i) {
-            double s = 0.0;
-            for (int j = 0; j < d; ++j) s += pk[LY.V0i + i * d + j] * (double)mu0[k * d + j];
-            pk[LY.xi0 + i] = s;
-        }
-        pk[LY.nu0] = nu0[k];
-        pk[LY.a0] = alpha0[k];
-        pk[LY.ai] = alpha_init[k];
-        pk[LY.nui] = nu_init[k];
-        double lgd = 0.25 * d * (d - 1) * rxg::gmm::LOGPI;
-        for (int i = 0; i < d; ++i) lgd += std::lgamma(0.5 * ((double)nu0[k] - i));
-        pk[LY.lgd0] = lgd;
+        if (int rc = rxg::nw::pack(ctx, "gmm_vmp", "component", k, d, mu0, V0, nu0, S0, m_init, Vm_init, nu_init, S_init,
+                                   hp + k * blk))
+            return rc;
+        a0[k] = alpha0[k];
+        ai[k] = alpha_init[k];
         sa0 += alpha0[k];
         slg0 += std::lgamma((double)alpha0[k]);
     }
-    hp[K * LY.blk] = sa0;
-    hp[K * LY.blk + 1] = std::lgamma(sa0) - slg0;
+    a0[2 * K] = sa0;
+    a0[2 * K + 1] = std::lgamma(sa0) - slg0;
     RXG_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t nbytes = (size_t)(K * LY.blk + 2) * sizeof(double);
+    const size_t nbytes = (size_t)rxg::gmm::n_params(K, d) * sizeof(double);
     double* dp = (double*)rxg::workspace(ctx, nbytes);
     if (!dp) return RXG_ERR_CUDA;
     RXG_CUDA(ctx, cudaMemcpyAsync(dp, hp, nbytes, cudaMemcpyHostToDevice, ctx->stream));
