@@ -11,6 +11,8 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
   python bench_extra.py --which gmm          (opt-in: Gaussian-mixture VMP, d = 2 / K = 3 and d = 4 / K = 8)
   python bench_extra.py --which hmm          (opt-in: hidden Markov model VMP, K = M = 3 and K = 8 / M = 16)
   python bench_extra.py --which hmm_gauss    (opt-in: Gaussian-emission HMM VMP, K = 3 / d = 2 and K = 8 / d = 4)
+  python bench_extra.py --which binomial     (opt-in: binomial regression VMP, both kernels, and the grid that places the
+                                             automatic choice between them)
   python bench_extra.py --which hgf_learn    (opt-in: HGF with learned kappa, omega, T = 1000, 20 iterations)
 """
 from __future__ import annotations
@@ -474,6 +476,45 @@ def bench_hmm_gauss(ctx, peak):
         torch.cuda.empty_cache()
 
 
+def bench_binomial(ctx):
+    """Bayesian binomial regression (rxg_binomial_polya_vmp_f32) on both kernels, forced through RXG_OPT_POLYA_PATH
+    (1 = one thread per chain, 2 = chain groups), on the same inputs: the reference test's workload (20 chains, N = 1000,
+    p = 2, 100 iterations), large batches (65 536 chains, N = 1000, p = 2 and 8, 20 iterations), then a batch x N grid at
+    p = 2, 20 iterations, that places the automatic choice.  Free energy on.  Time from CUDA events around the call.
+    Algorithmic bytes: every pass reads x, y and n once, (4 p + 8) per sample and chain, over iterations + 1 passes; the
+    fraction is of the 3.35 TB/s data-sheet HBM3 bandwidth of the H100 SXM."""
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(31)
+
+    def one(what, nb, N, p, its, reps):
+        X = torch.randn(N, p, nb, device="cuda", generator=g)
+        n = torch.randint(5, 21, (N, nb), device="cuda", generator=g, dtype=torch.int32)
+        beta = torch.randn(p, nb, device="cuda", generator=g)
+        prob = torch.sigmoid(torch.einsum("ijb,jb->ib", X, beta))
+        y = torch.binomial(n.float(), prob).to(torch.int32)
+        by = (its + 1) * N * nb * (4 * p + 8)
+        row = {"what": what, "batch": nb, "N": N, "p": p, "iterations": its, "algorithmic_bytes": by}
+        for path in (1, 2):
+            ctx.set_option("polya_path", path)
+            f = lambda: ctx.binomial_polya_vmp(X, y, np.zeros(p), np.eye(p), ntrials=n, iterations=its)
+            runs = [timed(f, warm=1, reps=reps) for _ in range(3)]
+            ms = float(np.median(runs))
+            row[f"ms_path{path}"] = ms
+            row[f"frac_of_3350GBs_path{path}"] = by / (ms * 1e-3) / 3.35e12
+        ctx.set_option("polya_path", 0)
+        row.update(gpu=gname, power_limit=plim)
+        print(json.dumps(row), flush=True)
+        del X, y, n
+        torch.cuda.empty_cache()
+
+    one("reference workload", 20, 1000, 2, 100, 5)
+    for p in (2, 8):
+        one("large batch", 65536, 1000, p, 20, 2)
+    for nb in (20, 1024, 4096, 8448, 16384, 65536):
+        for N in (100, 1000, 10000):
+            one("grid", nb, N, 2, 20, 2)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -483,6 +524,8 @@ def main():
     peak, _ = peaks()
     if "predict" in which:
         bench_predict(ctx, peak)
+    if "binomial" in which:
+        bench_binomial(ctx)
     if "inputs" in which:
         bench_inputs(ctx, peak)
     if "vmp_wishart" in which:

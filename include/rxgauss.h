@@ -88,7 +88,8 @@ typedef enum rxg_option {
     RXG_OPT_HOST_BCAST_MIN_MB = 7, /* below this covariance size the host broadcast is not used (default 64)        */
     RXG_OPT_HOST_SLICES = 8,       /* batch slices of the host-pointer pipeline (0 = auto)                          */
     RXG_OPT_GATHER_MODE = 9,       /* rxg_lgssm_smooth_gather_f32: 0/1 peer stores fused into the sweep, 2 push after it  */
-    RXG_OPT_COUNT_ = 10
+    RXG_OPT_POLYA_PATH = 10,       /* rxg_binomial_polya_vmp_f32: 0 auto, 1 one thread per chain, 2 chain groups (cross-check) */
+    RXG_OPT_COUNT_ = 11
 } rxg_option;
 
 #define RXG_MAX_PEERS 8            /* ranks of one peer group (one NVSwitch domain)                                 */
@@ -324,6 +325,22 @@ int rxg_hmm_gauss_vmp_f32(rxg_ctx*, int d, int K, int T, int64_t batch, int iter
                           float* m_cov, float* w_df, float* w_inv_scale, double* free_energy, float* hist_s, float* hist_A,
                           float* hist_m_mean, float* hist_m_cov, float* hist_w_df, float* hist_w_inv_scale,
                           int32_t* status, unsigned flags);
+/* Bayesian binomial / logistic regression, mean-field Polya-Gamma VMP, `batch` independent chains, all iterations in one
+ *   launch: beta ~ MvNormalWeightedMeanPrecision(xi0, W0), y[i] ~ BinomialPolya(x[i], n[i], beta) (y[i] ~ Binomial(n[i],
+ *   sigmoid(x[i]' beta))), i = 1..N, q(beta) Gaussian [ref: test/models/regression/binomialreg_tests.jl:32-43; the rule
+ *   reads q(beta) where the reference may read the cavity, and the reference pins no free energy (DESIGN 3.21)].  Host
+ *   arrays shared by every chain: xi0[p], W0[p][p] (symmetric positive definite).  X[N][p][batch] fp32, y[N][batch] int32,
+ *   ntrials[N][batch] int32 or NULL (every n = 1: logistic regression); a sample with n = 0 contributes nothing (padding
+ *   of ragged batches).  Outputs: beta_mean[p][batch], and optional (NULL = not wanted): beta_cov[p][p][batch],
+ *   free_energy[iterations][batch] (fp64, the collapsed Polya-Gamma bound of the posterior each iteration returns), the
+ *   KeepEach histories hist_mean[iterations][p][batch], hist_cov[iterations][p][p][batch], status[batch] (RXG_ERR_BAD_ARG
+ *   for a chain with a sample with a non-finite x, y < 0, n < 0 or y > n, read as n = 0; RXG_ERR_NOT_SPD for a
+ *   non-positive pivot; RXG_ERR_NAN for a non-finite result; the last two take precedence).  1 <= p <= 8, else
+ *   RXG_ERR_UNSUPPORTED; N, batch, iterations >= 1, finite xi0 and W0 symmetric positive definite, else RXG_ERR_BAD_ARG.
+ *   Device pointers (RXG_ERR_UNSUPPORTED otherwise).  RXG_OPT_POLYA_PATH selects the kernel.                           */
+int rxg_binomial_polya_vmp_f32(rxg_ctx*, int p, int N, int64_t batch, int iterations, const float* xi0, const float* W0,
+                               const float* X, const int32_t* y, const int32_t* ntrials, float* beta_mean, float* beta_cov,
+                               double* free_energy, float* hist_mean, float* hist_cov, int32_t* status, unsigned flags);
 /* prod(GammaShapeRate, GammaShapeRate) = (a1 + a2 - 1, b1 + b2)                                 */
 int rxg_prod_gamma_f32(rxg_ctx*, int64_t n, const float* a1, const float* b1, const float* a2,
                        const float* b2, float* a, float* b, unsigned flags);

@@ -66,7 +66,7 @@ class Context:
         return int(self.lib.rxg_host_fill_threads())
 
     OPTIONS = {"gain_seq": 0, "large_seq": 1, "no_umma": 2, "sweep_variant": 3, "force_cpt": 4, "host_threads": 5,
-               "host_cov_d2h": 6, "host_bcast_min_mb": 7, "host_slices": 8, "gather_mode": 9}
+               "host_cov_d2h": 6, "host_bcast_min_mb": 7, "host_slices": 8, "gather_mode": 9, "polya_path": 10}
 
     def set_option(self, name: str, value: int):
         """``rxg_set_option``: per-context dispatch switches (cross-check kernels, host-pipeline tuning)."""
@@ -846,6 +846,45 @@ class Context:
                                                                                "hist_w_df", "hist_w_inv_scale")),
                                                    ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
         out = dict(s_prob=sp, s0_prob=s0, A_alpha=Aa, m_mean=mm, m_cov=mc, w_df=df, w_inv_scale=iS, free_energy=fe, status=st)
+        out.update(h)
+        return out
+
+    def binomial_polya_vmp(self, X, y, xi0, W0, ntrials=None, iterations=1, want_free_energy=True, keep_each=False):
+        """Bayesian binomial / logistic regression by mean-field Polya-Gamma VMP (``rxg_binomial_polya_vmp_f32``), one chain
+        per batch column: X[N, p, batch] float32, y[N, batch] and ntrials[N, batch] (None: every n = 1) int32 on the
+        device; xi0[p] and W0[p, p] (the prior's weighted mean and precision) are host arrays shared by every chain.  A
+        sample with n = 0 contributes nothing.  Returns ``beta_mean[p, batch]``, ``beta_cov[p, p, batch]``,
+        ``free_energy[iterations, batch]`` (fp64), ``status[batch]`` and, with ``keep_each``, ``hist_mean`` / ``hist_cov``
+        with a leading iteration axis."""
+        self._dev(X)
+        if X.dim() != 3:
+            raise ValueError("binomial_polya_vmp: X must be [N, p, batch]")
+        N, p, batch = X.shape
+        for name, t in (("y", y), ("ntrials", ntrials)):
+            if t is None and name == "ntrials":
+                continue
+            if not (t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and tuple(t.shape) == (N, batch)):
+                raise ValueError(f"binomial_polya_vmp: {name} must be a contiguous int32 CUDA tensor [N, batch] = {(N, batch)}")
+            if t.device.index != self.device:
+                raise ValueError(f"binomial_polya_vmp: {name} lives on cuda:{t.device.index}, this context is bound to "
+                                 f"cuda:{self.device}")
+        keep = {}
+        for k, (v, shp) in dict(xi0=(xi0, (p,)), W0=(W0, (p, p))).items():
+            a = np.asarray(v, dtype=np.float64)
+            if a.shape != shp:
+                raise ValueError(f"binomial_polya_vmp: {k} must have shape {shp} (p = {p}), got {a.shape}")
+            keep[k] = _model32(a)
+        its = int(iterations)
+        mean, cov = self.empty(p, batch), self.empty(p, p, batch)
+        fe = self.empty(its, batch, dtype=torch.float64) if want_free_energy else None
+        h = dict(hist_mean=self.empty(its, p, batch), hist_cov=self.empty(its, p, p, batch)) if keep_each else {}
+        st = self.empty(batch, dtype=torch.int32)
+        i32 = lambda t: ctypes.cast(c_void_p(t.data_ptr() if t is not None else None), L.i32p)
+        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
+        self._check(self.lib.rxg_binomial_polya_vmp_f32(self.h, p, N, batch, its, keep["xi0"][1], keep["W0"][1], _fp(X), i32(y),
+                                                        i32(ntrials), _fp(mean), _fp(cov), fe_p, _fp(h.get("hist_mean")),
+                                                        _fp(h.get("hist_cov")), i32(st), L.PTR_DEVICE))
+        out = dict(beta_mean=mean, beta_cov=cov, free_energy=fe, status=st)
         out.update(h)
         return out
 

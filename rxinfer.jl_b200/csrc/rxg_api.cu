@@ -183,7 +183,7 @@ int rxg_create(rxg_ctx** out, int device, unsigned flags) {
         {RXG_OPT_SWEEP_VARIANT, "RXG_SWEEP_VARIANT"}, {RXG_OPT_FORCE_CPT, "RXG_FORCE_CPT"},
         {RXG_OPT_HOST_THREADS, "RXG_HOST_THREADS"}, {RXG_OPT_HOST_COV_D2H, "RXG_HOST_COV_D2H"},
         {RXG_OPT_HOST_BCAST_MIN_MB, "RXG_HOST_BCAST_MIN_MB"}, {RXG_OPT_HOST_SLICES, "RXG_HOST_SLICES"},
-        {RXG_OPT_GATHER_MODE, "RXG_GATHER_MODE"}};
+        {RXG_OPT_GATHER_MODE, "RXG_GATHER_MODE"}, {RXG_OPT_POLYA_PATH, "RXG_POLYA_PATH"}};
     for (const auto& e : kEnv)
         if (const char* v = getenv(e.env)) ctx->opt[e.id] = atoll(v);
     *out = ctx;

@@ -653,6 +653,79 @@ def _infer_hmm_gauss(model, data, constraints, initialization, iterations, free_
         raise
 
 
+@dataclass
+class binomial_regression:
+    """Bayesian binomial / logistic regression (RxInfer test/models/regression/binomialreg_tests.jl:32-43):
+    ``β ~ MvNormalWeightedMeanPrecision(prior_xi, prior_precision)``, ``y[i] ~ BinomialPolya(X[i], n_trials[i], β)``, i.e.
+    y_i ~ Binomial(n_i, σ(X_iᵀβ)), fitted by mean-field Pólya-Gamma VMP (DESIGN 3.21).  Run with ``data = {"X": [batch, N,
+    p], "y": [batch, N], "n_trials": [batch, N]}`` (no ``n_trials``: every n = 1, logistic regression; one series may
+    come without the batch axis); a sample with n = 0 contributes nothing."""
+    prior_xi: object
+    prior_precision: object
+
+
+def _infer_binomial(model, data, initialization, iterations, free_energy, returnvars, predictvars, datastream, context,
+                    catch_exception):
+    """``infer`` of ``binomial_regression``: one ``rxg_binomial_polya_vmp_f32`` launch.  ``returnvars`` is KeepLast() /
+    KeepEach() of ``β``; ``free_energy=True`` gives F after every iteration."""
+    if predictvars is not None:
+        raise NotImplementedError("predictvars: predictions of y are outside the batched hot path")
+    if datastream is not None or data is None:
+        raise NotImplementedError("binomial_regression runs over whole data sets: pass data = {'X', 'y', 'n_trials'} "
+                                  "(no datastream)")
+    if initialization is not None:
+        raise NotImplementedError("binomial_regression starts from the prior: initialization is not used")
+    if "X" not in data or "y" not in data:
+        raise KeyError("binomial_regression needs data = {'X': [batch, N, p], 'y': [batch, N]} (and 'n_trials')")
+    bad = set(data) - {"X", "y", "n_trials"}
+    if bad:
+        raise ValueError(f"binomial_regression: unknown data {sorted(bad)} (X, y, n_trials)")
+    if isinstance(returnvars, dict):
+        if set(returnvars) - {"β"} or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
+            raise NotImplementedError(f"returnvars={returnvars!r}: KeepEach() / KeepLast() of β")
+        each = isinstance(returnvars.get("β"), KeepEach)
+    elif returnvars is None or isinstance(returnvars, (KeepEach, KeepLast)):
+        each = isinstance(returnvars, KeepEach)
+    else:
+        raise NotImplementedError(f"returnvars={returnvars!r}: binomial_regression returns KeepEach() or KeepLast() of β")
+    X = torch.as_tensor(data["X"])
+    single = X.dim() == 2
+    X = X[None] if single else X
+    if X.dim() != 3:
+        raise ValueError(f"data['X'] must be [batch, N, p] (or [N, p]), got {tuple(X.shape)}")
+    nb, N, p = X.shape
+
+    def counts(name):
+        v = torch.as_tensor(data[name])
+        v = v[None] if single else v
+        if tuple(v.shape) != (nb, N):
+            raise ValueError(f"data['{name}'] must be [batch, N] = {(nb, N)} (or [N]), got {tuple(v.shape)}")
+        if v.is_floating_point() and not bool((v == torch.round(v)).all()):
+            raise ValueError(f"data['{name}'] must hold whole numbers")
+        return v.to(torch.int32)
+
+    y = counts("y")
+    n = counts("n_trials") if data.get("n_trials") is not None else None
+    try:
+        ctx = context or default_context()
+        dev = f"cuda:{ctx.device}"
+        r = ctx.binomial_polya_vmp(X.to(device=dev, dtype=torch.float32).permute(1, 2, 0).contiguous(),
+                                   y.to(dev).T.contiguous(), model.prior_xi, model.prior_precision,
+                                   ntrials=None if n is None else n.to(dev).T.contiguous(), iterations=iterations or 1,
+                                   want_free_energy=bool(free_energy), keep_each=each)
+        _raise_flagged(r["status"], "binomial_regression: ", " (BAD_ARG: a non-finite x, y < 0, n < 0 or y > n; NOT_SPD: "
+                       "a non-positive pivot; NAN: a non-finite result)")
+        mean, cov = (r["hist_mean"], r["hist_cov"]) if each else (r["beta_mean"], r["beta_cov"])
+        fe = r["free_energy"]
+        if single:
+            mean, cov, fe = mean[..., 0], cov[..., 0], (fe[:, 0] if fe is not None else None)
+        return InferenceResult(posteriors={"β": MvNormalMeanCovariance(mean, cov)}, model=model, free_energy=fe)
+    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
+        if catch_exception:
+            return InferenceResult(posteriors={}, model=model, error=e)
+        raise
+
+
 def _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
                        datastream, context, catch_exception):
     """``infer`` of ``hgf_offline``: one ``rxg_hgf_vmp_learn_f32`` launch.  ``returnvars``: KeepLast() for x, z (and x_0),
@@ -725,6 +798,12 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             raise NotImplementedError(f"options {sorted(bad)} are outside the batched hot path")
     if data is not None and datastream is not None:
         raise ValueError("`data` and `datastream` are mutually exclusive")    # reference: inference.jl argument check
+    if isinstance(model, binomial_regression):
+        if autoupdates is not None or keephistory is not None or historyvars is not None or batch is not None or cov_shared_out:
+            raise NotImplementedError("binomial_regression: autoupdates, keephistory, historyvars, batch and cov_shared_out "
+                                      "are outside the batched hot path")
+        return _infer_binomial(model, data, initialization, iterations, free_energy, returnvars, predictvars, datastream,
+                               context, catch_exception)
     if isinstance(model, hgf_offline):
         return _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
                                   datastream, context, catch_exception)

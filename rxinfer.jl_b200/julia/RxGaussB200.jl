@@ -268,6 +268,12 @@ hmm_gauss_vmp(ctx, d, K, T, batch, its, p0, Ap, Ai, Ak, mu0, V0, nu0, S0, mi, Vi
         ctx.handle, d, K, T, batch, its, p0, Ap, Ai, Ak, mu0, V0, nu0, S0, mi, Vi, nui, Si, y, sp, s0, Aa, mm, mc, df, iS, fe, hs,
         hA, hmm, hmc, hdf, hiS, st, fl))
 
+binomial_polya_vmp(ctx, p, N, batch, its, xi0, W0, X, y, nt, bm, bc, fe, hm, hc, st, fl) =
+    check(ctx, ccall((:rxg_binomial_polya_vmp_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Int64, Cint, F32P, F32P, F32P, Ptr{Int32}, Ptr{Int32}, F32P, F32P, Ptr{Float64}, F32P, F32P,
+         Ptr{Int32}, Cuint),
+        ctx.handle, p, N, batch, its, xi0, W0, X, y, nt, bm, bc, fe, hm, hc, st, fl))
+
 # ---- diagnostics
 selftest_umma(ctx, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_f32, LIB), Cint, (Ptr{Cvoid}, F32P, F32P, F32P, Cuint), ctx.handle, A, B, D, fl))
 selftest_umma_shape(ctx, n, k, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_shape_f32, LIB), Cint, (Ptr{Cvoid}, Cint, Cint, F32P, F32P, F32P, Cuint), ctx.handle, n, k, A, B, D, fl))
@@ -927,6 +933,48 @@ function gaussian_mixture(ctx::Context, y::Array{Float32, 3}; alpha0, mu0, V0, n
     Lib.device_free(ctx, fe)
     return (s = download(hal), m_mean = download(hmm), m_cov = download(hmc), w_df = download(hdf), w_inv_scale = download(hiS),
             z = download(z), free_energy = fe_host, status = reinterpret(Int32, download(st)))
+end
+
+"""Bayesian binomial / logistic regression by mean-field Pólya-Gamma VMP (`rxg_binomial_polya_vmp_f32`, DESIGN 3.21), one
+regression per batch row; the model of binomialreg_tests.jl:32-43:
+
+    @model function binomial_model(prior_xi, prior_precision, n_trials, X, y)
+        β ~ MvNormalWeightedMeanPrecision(prior_xi, prior_precision)
+        for i in eachindex(y)
+            y[i] ~ BinomialPolya(X[i], n_trials[i], β)
+        end
+    end
+
+`X[batch, p, N]` (Float32), `y[batch, N]` and `ntrials[batch, N]` (Int32; `nothing`: every n = 1, logistic regression; a
+sample with n = 0 contributes nothing).  `xi0` (p vector) and `W0` (p x p, SPD) are shared by every regression.  Returns
+the KeepEach posteriors (trailing iteration axis): mean `[batch, p, its]`, covariance `[batch, p, p, its]`, the free energy
+`[batch, its]` (Float64) and the per-regression status.  No GraphPPL pattern routes this model here: the reference test
+passes `options`, which is on the fallback list."""
+function binomial_polya_vmp(ctx::Context, X::Array{Float32, 3}, y::Matrix{Int32}, ntrials::Union{Nothing, Matrix{Int32}};
+                            xi0, W0, iterations = 100)
+    batch, p, N = size(X)
+    dX = upload(ctx, X)
+    dy = Lib.device_alloc(ctx, sizeof(y))
+    GC.@preserve y Lib.memcpy_h2d(ctx, dy, Ptr{Cvoid}(pointer(y)), sizeof(y))
+    dn = C_NULL
+    if ntrials !== nothing
+        dn = Lib.device_alloc(ctx, sizeof(ntrials))
+        GC.@preserve ntrials Lib.memcpy_h2d(ctx, dn, Ptr{Cvoid}(pointer(ntrials)), sizeof(ntrials))
+    end
+    bm, bc = DeviceArray(ctx, batch, p), DeviceArray(ctx, batch, p, p)
+    hm, hc = DeviceArray(ctx, batch, p, iterations), DeviceArray(ctx, batch, p, p, iterations)
+    st = DeviceArray(ctx, batch)
+    fe = Lib.device_alloc(ctx, 8 * batch * iterations)
+    h = (Float32.(collect(xi0)), rowmajor32(W0))
+    GC.@preserve h Lib.binomial_polya_vmp(ctx, p, N, batch, iterations, pointer(h[1]), pointer(h[2]), dX.ptr, Ptr{Int32}(dy),
+                                          Ptr{Int32}(dn), bm.ptr, bc.ptr, Ptr{Float64}(fe), hm.ptr, hc.ptr,
+                                          Ptr{Int32}(st.ptr), RXG_PTR_DEVICE)
+    fe_host = Array{Float64}(undef, batch, iterations)
+    GC.@preserve fe_host Lib.memcpy_d2h(ctx, pointer(fe_host), fe, 8 * batch * iterations)
+    Lib.device_free(ctx, fe)
+    Lib.device_free(ctx, dy)
+    ntrials !== nothing && Lib.device_free(ctx, dn)
+    return (mean = download(hm), cov = download(hc), free_energy = fe_host, status = reinterpret(Int32, download(st)))
 end
 
 """Fused structured VMP of the hidden Markov model with Gaussian emissions (`rxg_hmm_gauss_vmp_f32`); `y[batch, d, T]`, a step
