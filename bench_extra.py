@@ -13,6 +13,8 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
   python bench_extra.py --which hmm_gauss    (opt-in: Gaussian-emission HMM VMP, K = 3 / d = 2 and K = 8 / d = 4)
   python bench_extra.py --which binomial     (opt-in: binomial regression VMP, both kernels, and the grid that places the
                                              automatic choice between them)
+  python bench_extra.py --which multinomial  (opt-in: multinomial regression VMP, whole data sets and online, per-kernel
+                                             times, data-pass bandwidth and fp64 FMA rate)
   python bench_extra.py --which hgf_learn    (opt-in: HGF with learned kappa, omega, T = 1000, 20 iterations)
 """
 from __future__ import annotations
@@ -515,6 +517,68 @@ def bench_binomial(ctx):
             one("grid", nb, N, 2, 20, 2)
 
 
+def bench_multinomial(ctx):
+    """Bayesian multinomial regression (rxg_multinomial_polya_vmp_f32 / _online_f32): the reference test's workloads
+    (offline: 1 chain, n = 1000, K = 10, 100 iterations; online: 1 chain, T = 5000, K = 40) and large batches (offline
+    65 536 chains at K = 10 and 4096 at K = 40, n = 1000, 100 iterations; online 4096 chains, T = 1000, K = 10 and 40, no
+    covariance history).  Free energy on.  Call time from CUDA events around the call; per-kernel times from
+    torch.profiler in a separate pass.  The data pass reads y once, 4 n K bytes per chain (fraction of the 3.35 TB/s
+    data-sheet HBM3 bandwidth of the H100 SXM); a step does D^3 + D^2 fp64 FMAs (D Sherman-Morrison updates of D^2
+    entries, then the mean)."""
+    from torch.profiler import ProfilerActivity, profile
+    gname, plim = gpu_name_and_power_limit()
+    g = torch.Generator(device="cuda").manual_seed(41)
+
+    def counts(n, K, nb, N):
+        p = torch.softmax(torch.randn(K, nb, device="cuda", generator=g), 0)
+        c = torch.distributions.Multinomial(N, probs=p.T).sample((n,))          # [n, nb, K]
+        return c.permute(0, 2, 1).contiguous().to(torch.int32)
+
+    def kernel_ms(f):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            f()
+            torch.cuda.synchronize()
+        out = {}
+        for e in prof.key_averages():
+            if "mnp_" in e.key:
+                name = e.key.split("mnp_")[1].split("_kernel")[0]
+                out[name] = out.get(name, 0.0) + e.device_time_total / 1e3
+        return out
+
+    def one(what, mode, nb, n, K, N, its, reps):
+        D = K - 1
+        y = counts(n, K, nb, N)
+        xi0, W0 = np.zeros(D), float(K) * np.eye(D)
+        if mode == "offline":
+            f = lambda: ctx.multinomial_polya_vmp(y, xi0, W0, iterations=its)
+            steps = its * nb
+        else:
+            f = lambda: ctx.multinomial_polya_online(y, xi0, W0, keep_cov=nb == 1)
+            steps = n * nb
+        ms = float(np.median([timed(f, warm=1, reps=reps) for _ in range(3)]))
+        k = kernel_ms(f)
+        row = {"what": what, "mode": mode, "batch": nb, "n" if mode == "offline" else "T": n, "K": K, "trials": N,
+               "iterations": its, "ms_call": ms, "kernel_ms": k}
+        fma = steps * (D ** 3 + D ** 2)
+        step_ms = k.get("vmp" if mode == "offline" else "online", float("nan"))
+        row["fp64_fma_per_s"] = fma / (step_ms * 1e-3)
+        if mode == "offline":
+            by = 4 * n * K * nb
+            row["data_bytes"] = by
+            row["data_frac_of_3350GBs"] = by / (k.get("data", float("nan")) * 1e-3) / 3.35e12
+        row.update(gpu=gname, power_limit=plim)
+        print(json.dumps(row), flush=True)
+        del y
+        torch.cuda.empty_cache()
+
+    one("reference workload", "offline", 1, 1000, 10, 20, 100, 5)
+    one("large batch", "offline", 65536, 1000, 10, 20, 100, 2)
+    one("large batch", "offline", 4096, 1000, 40, 50, 100, 2)
+    one("reference workload", "online", 1, 5000, 40, 50, 1, 2)
+    one("large batch", "online", 4096, 1000, 10, 20, 1, 2)
+    one("large batch", "online", 4096, 1000, 40, 50, 1, 2)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--which", default="per_chain,filter,hgf,rules,vmp,scaling_T,large,stream,round2")
@@ -526,6 +590,8 @@ def main():
         bench_predict(ctx, peak)
     if "binomial" in which:
         bench_binomial(ctx)
+    if "multinomial" in which:
+        bench_multinomial(ctx)
     if "inputs" in which:
         bench_inputs(ctx, peak)
     if "vmp_wishart" in which:

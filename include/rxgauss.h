@@ -341,6 +341,31 @@ int rxg_hmm_gauss_vmp_f32(rxg_ctx*, int d, int K, int T, int64_t batch, int iter
 int rxg_binomial_polya_vmp_f32(rxg_ctx*, int p, int N, int64_t batch, int iterations, const float* xi0, const float* W0,
                                const float* X, const int32_t* y, const int32_t* ntrials, float* beta_mean, float* beta_cov,
                                double* free_energy, float* hist_mean, float* hist_cov, int32_t* status, unsigned flags);
+/* Bayesian multinomial regression, mean-field Polya-Gamma VMP, `batch` independent chains, all iterations in one call:
+ *   psi ~ MvNormalWeightedMeanPrecision(xi0, W0), y[i] ~ MultinomialPolya(N_i, psi), i = 1..n, N_i = sum_k y[i][k], read
+ *   through stick-breaking (y_ik ~ Binomial(N_ik, sigmoid(psi_k)), N_ik = sum_{j >= k} y_ij), D = K - 1, q(psi) Gaussian
+ *   [ref: test/models/regression/multinomialreg_tests.jl; the rule reads q(psi) where the reference may read the cavity
+ *   (DESIGN 3.22)].  Host arrays shared by every chain: xi0[D], W0[D][D] (symmetric positive definite).  y[n][K][batch]
+ *   int32 counts; an all-zero sample contributes nothing (padding of ragged batches).  Outputs: psi_mean[D][batch], and
+ *   optional (NULL = not wanted): psi_cov[D][D][batch], free_energy[iterations][batch] (fp64, the collapsed Polya-Gamma
+ *   bound of the posterior each iteration returns), the KeepEach histories hist_mean[iterations][D][batch],
+ *   hist_cov[iterations][D][D][batch], status[batch] (RXG_ERR_BAD_ARG for a chain with a negative count, that sample read
+ *   as all-zero; RXG_ERR_NOT_SPD for a non-positive pivot; RXG_ERR_NAN for a non-finite result; the last two take
+ *   precedence).  2 <= K <= 64, else RXG_ERR_UNSUPPORTED; n, batch, iterations >= 1, finite xi0 and W0 symmetric
+ *   positive definite, else RXG_ERR_BAD_ARG.  Device pointers (RXG_ERR_UNSUPPORTED otherwise).  Two kernel launches.   */
+int rxg_multinomial_polya_vmp_f32(rxg_ctx*, int K, int n, int64_t batch, int iterations, const float* xi0, const float* W0,
+                                  const int32_t* y, float* psi_mean, float* psi_cov, double* free_energy, float* hist_mean,
+                                  float* hist_cov, int32_t* status, unsigned flags);
+/* The same model online (@autoupdates of q(psi), one datum at a time): datum t of y[T][K][batch] runs `iterations` steps
+ *   from the base q_{t-1}, then q_t is the next base.  The carry is fp64: m_in[D][batch], S_in[D][D][batch] (both NULL:
+ *   every chain starts at N(W0^-1 xi0, W0^-1)), m_out, S_out the same shapes (may be m_in, S_in: updated in place), so a
+ *   stream split into chunks gives the bits of one call.  Optional per datum: hist_mean[T][D][batch],
+ *   hist_cov[T][D][D][batch], free_energy[T][batch] (fp64, KL(q_t || q_{t-1}) minus the bound of datum t's evidence:
+ *   free_energy_final_only_history), status[batch] as above.  Limits and errors as rxg_multinomial_polya_vmp_f32.     */
+int rxg_multinomial_polya_online_f32(rxg_ctx*, int K, int T, int64_t batch, int iterations, const float* xi0, const float* W0,
+                                     const double* m_in, const double* S_in, const int32_t* y, double* m_out, double* S_out,
+                                     float* hist_mean, float* hist_cov, double* free_energy, int32_t* status,
+                                     unsigned flags);
 /* prod(GammaShapeRate, GammaShapeRate) = (a1 + a2 - 1, b1 + b2)                                 */
 int rxg_prod_gamma_f32(rxg_ctx*, int64_t n, const float* a1, const float* b1, const float* a2,
                        const float* b2, float* a, float* b, unsigned flags);

@@ -21,7 +21,8 @@ def __getattr__(name):   # lazy: these import torch
                 "linear_gaussian_ssm_wishart_precision", "linear_gaussian_ssm_wishart_noise",
                 "linear_gaussian_ssm_continuous_transition", "gaussian_mixture", "MeanField", "BetheFactorization",
                 "hidden_markov_model", "HMMConstraints", "hgf_offline", "gaussian_hidden_markov_model",
-                "GaussianHMMConstraints", "binomial_regression",
+                "GaussianHMMConstraints", "binomial_regression", "multinomial_regression",
+                "multinomial_regression_online",
                 "default_context",
                 "KeepLast", "KeepEach"):
         from . import inference

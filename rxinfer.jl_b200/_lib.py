@@ -78,6 +78,11 @@ SIGNATURES = {
                                       fp, fp, fp, fp, fp, fp, fp, fp, POINTER(c_double), fp, fp, fp, fp, fp, fp, i32p, c_uint]),
     "rxg_binomial_polya_vmp_f32": (c_int, [c_void_p, c_int, c_int, c_int64, c_int, fp, fp, fp, i32p, i32p, fp, fp, POINTER(c_double),
                                            fp, fp, i32p, c_uint]),
+    "rxg_multinomial_polya_vmp_f32": (c_int, [c_void_p, c_int, c_int, c_int64, c_int, fp, fp, i32p, fp, fp, POINTER(c_double),
+                                              fp, fp, i32p, c_uint]),
+    "rxg_multinomial_polya_online_f32": (c_int, [c_void_p, c_int, c_int, c_int64, c_int, fp, fp, POINTER(c_double),
+                                                 POINTER(c_double), i32p, POINTER(c_double), POINTER(c_double), fp, fp,
+                                                 POINTER(c_double), i32p, c_uint]),
     "rxg_prod_gamma_f32": (c_int, [c_void_p, c_int64, fp, fp, fp, fp, fp, fp, c_uint]),
     "rxg_prod_normal_f32": (c_int, [c_void_p, c_int64, fp, fp, fp, fp, fp, fp, c_uint]),
     "rxg_rule_gcv_out_f32": (c_int, [c_void_p, c_int64, fp, fp, fp, fp, c_float, c_float, fp, fp, c_uint]),

@@ -21,6 +21,14 @@ def _fp(t):
     return L.as_fp(t.data_ptr())
 
 
+def _i32(t):
+    return ctypes.cast(c_void_p(t.data_ptr() if t is not None else None), L.i32p)
+
+
+def _f64(t):
+    return ctypes.cast(c_void_p(t.data_ptr() if t is not None else None), ctypes.POINTER(ctypes.c_double))
+
+
 def _model32(M):
     """Shared model matrices are small host arrays (row-major fp32)."""
     a = np.ascontiguousarray(np.asarray(M, dtype=np.float32))
@@ -887,6 +895,74 @@ class Context:
         out = dict(beta_mean=mean, beta_cov=cov, free_energy=fe, status=st)
         out.update(h)
         return out
+
+    def _multinomial_args(self, who, y, xi0, W0):
+        """y: a contiguous int32 CUDA tensor [n, K, batch] on this context's device; the prior (xi0 [D], W0 [D, D], D = K - 1)
+        as the fp32 host arrays the C entries take."""
+        if not (isinstance(y, torch.Tensor) and y.is_cuda and y.dtype == torch.int32 and y.is_contiguous() and y.dim() == 3):
+            raise ValueError(f"{who}: y must be a contiguous int32 CUDA tensor [n, K, batch]")
+        if y.device.index != self.device:
+            raise ValueError(f"{who}: y lives on cuda:{y.device.index}, this context is bound to cuda:{self.device}")
+        D = y.shape[1] - 1
+        keep = {}
+        for k, (v, shp) in dict(xi0=(xi0, (D,)), W0=(W0, (D, D))).items():
+            a = np.asarray(v, dtype=np.float64)
+            if a.shape != shp:
+                raise ValueError(f"{who}: {k} must have shape {shp} (K = {D + 1}), got {a.shape}")
+            keep[k] = _model32(a)
+        return D, keep
+
+    def multinomial_polya_vmp(self, y, xi0, W0, iterations=1, want_free_energy=True, keep_each=False):
+        """Bayesian multinomial regression by mean-field Polya-Gamma VMP over whole data sets
+        (``rxg_multinomial_polya_vmp_f32``), one chain per batch column: counts y[n, K, batch] int32 on the device (an
+        all-zero sample contributes nothing); xi0[D] and W0[D, D] (the prior's weighted mean and precision, D = K - 1) are
+        host arrays shared by every chain.  Returns ``psi_mean[D, batch]``, ``psi_cov[D, D, batch]``,
+        ``free_energy[iterations, batch]`` (fp64), ``status[batch]`` and, with ``keep_each``, ``hist_mean`` / ``hist_cov``
+        with a leading iteration axis."""
+        D, keep = self._multinomial_args("multinomial_polya_vmp", y, xi0, W0)
+        n, K, batch = y.shape
+        its = int(iterations)
+        mean, cov = self.empty(D, batch), self.empty(D, D, batch)
+        fe = self.empty(its, batch, dtype=torch.float64) if want_free_energy else None
+        h = dict(hist_mean=self.empty(its, D, batch), hist_cov=self.empty(its, D, D, batch)) if keep_each else {}
+        st = self.empty(batch, dtype=torch.int32)
+        self._check(self.lib.rxg_multinomial_polya_vmp_f32(self.h, K, n, batch, its, keep["xi0"][1], keep["W0"][1],
+                                                           _i32(y), _fp(mean), _fp(cov), _f64(fe), _fp(h.get("hist_mean")),
+                                                           _fp(h.get("hist_cov")), _i32(st), L.PTR_DEVICE))
+        out = dict(psi_mean=mean, psi_cov=cov, free_energy=fe, status=st)
+        out.update(h)
+        return out
+
+    def multinomial_polya_online(self, y, xi0, W0, m=None, S=None, iterations=1, want_free_energy=True,
+                                 keep_mean=True, keep_cov=True, in_place=False):
+        """The same model online (``rxg_multinomial_polya_online_f32``): datum t of y[T, K, batch] (int32, device) runs
+        ``iterations`` steps from q_{t-1}.  The carry is fp64 on the device, m[D, batch] and S[D, D, batch]; None starts
+        every chain at the prior (xi0, W0).  ``in_place`` updates the given carry.  Returns ``m``, ``S`` (the carry after
+        the last datum), ``hist_mean[T, D, batch]`` / ``hist_cov[T, D, D, batch]`` (None when not kept),
+        ``free_energy[T, batch]`` (fp64, per datum) and ``status[batch]``."""
+        D, keep = self._multinomial_args("multinomial_polya_online", y, xi0, W0)
+        T, K, batch = y.shape
+        if (m is None) != (S is None):
+            raise ValueError("multinomial_polya_online: pass the carry m and S together, or neither")
+        if m is not None:
+            for name, t, shp in (("m", m, (D, batch)), ("S", S, (D, D, batch))):
+                if not (t.is_cuda and t.dtype == torch.float64 and t.is_contiguous() and tuple(t.shape) == shp
+                        and t.device.index == self.device):
+                    raise ValueError(f"multinomial_polya_online: {name} must be a contiguous float64 tensor {shp} on "
+                                     f"cuda:{self.device}")
+        if in_place and m is None:
+            raise ValueError("multinomial_polya_online: in_place needs a carry")
+        m_out = m if in_place else self.empty(D, batch, dtype=torch.float64)
+        S_out = S if in_place else self.empty(D, D, batch, dtype=torch.float64)
+        hm = self.empty(T, D, batch) if keep_mean else None
+        hc = self.empty(T, D, D, batch) if keep_cov else None
+        fe = self.empty(T, batch, dtype=torch.float64) if want_free_energy else None
+        st = self.empty(batch, dtype=torch.int32)
+        self._check(self.lib.rxg_multinomial_polya_online_f32(self.h, K, T, batch, int(iterations), keep["xi0"][1],
+                                                              keep["W0"][1], _f64(m), _f64(S), _i32(y), _f64(m_out),
+                                                              _f64(S_out), _fp(hm), _fp(hc), _f64(fe), _i32(st),
+                                                              L.PTR_DEVICE))
+        return dict(m=m_out, S=S_out, hist_mean=hm, hist_cov=hc, free_energy=fe, status=st)
 
     def prod_gamma(self, a1, b1, a2, b2):
         return self._six(self.lib.rxg_prod_gamma_f32, a1, b1, a2, b2)

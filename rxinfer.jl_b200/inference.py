@@ -19,7 +19,7 @@ import torch
 from . import _lib as L
 from .context import Context
 from .distributions import (Beta, Categorical, Dirichlet, DirichletCollection, GammaShapeRate, MvNormalMeanCovariance,
-                            NormalMeanVariance, PointMass, Wishart, WishartFast)
+                            MvNormalWeightedMeanPrecision, NormalMeanVariance, PointMass, Wishart, WishartFast)
 
 
 # --------------------------------------------------------------------------- recognised models
@@ -726,6 +726,119 @@ def _infer_binomial(model, data, initialization, iterations, free_energy, return
         raise
 
 
+@dataclass
+class multinomial_regression:
+    """Bayesian multinomial regression (RxInfer test/models/regression/multinomialreg_tests.jl, offline item):
+    ``ψ ~ MvNormalWeightedMeanPrecision(prior_xi, prior_precision)``, ``y[i] ~ MultinomialPolya(N_i, ψ)`` with N_i the sum
+    of y[i]'s K counts and ψ of length K − 1 (stick-breaking), fitted by mean-field Pólya-Gamma VMP (DESIGN 3.22).  Run
+    with ``data = {"y": [batch, n, K]}`` (one data set may come as [n, K]); an all-zero sample contributes nothing."""
+    prior_xi: object
+    prior_precision: object
+
+
+@dataclass
+class multinomial_regression_online:
+    """The same model online (multinomialreg_tests.jl, online item): ``ψ ~ MvNormalWeightedMeanPrecision(ξ_ψ, W_ψ)``,
+    ``y ~ MultinomialPolya(N, ψ)`` with ``@autoupdates ξ_ψ, W_ψ = weightedmean_precision(q(ψ))`` and
+    ``initialization = {"ψ": MvNormalWeightedMeanPrecision(ξ, W)}``.  ``infer`` returns an ``RxInferenceEngine`` whose
+    chunks are int32 counts [Tc, K, batch]; ``data = {"y": [batch, T, K]}`` (or [T, K]) gives a completed engine."""
+
+
+def _returns_each(returnvars, name, who):
+    """KeepEach() / KeepLast() of one variable, bare or as {name: ...}: True for KeepEach."""
+    if isinstance(returnvars, dict):
+        if set(returnvars) - {name} or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
+            raise NotImplementedError(f"returnvars={returnvars!r}: KeepEach() / KeepLast() of {name}")
+        return isinstance(returnvars.get(name), KeepEach)
+    if returnvars is None or isinstance(returnvars, (KeepEach, KeepLast)):
+        return isinstance(returnvars, KeepEach)
+    raise NotImplementedError(f"returnvars={returnvars!r}: {who} returns KeepEach() or KeepLast() of {name}")
+
+
+def _counts(v, what):
+    """Whole-number counts as an int32 tensor; a float array must hold whole numbers."""
+    v = torch.as_tensor(v)
+    if v.is_floating_point():
+        if not bool((v == torch.round(v)).all()):
+            raise ValueError(f"{what} must hold whole numbers")
+    elif v.dtype == torch.bool or v.is_complex():
+        raise ValueError(f"{what} must hold whole numbers")
+    return v.to(torch.int32)
+
+
+def _infer_multinomial(model, data, initialization, iterations, free_energy, returnvars, predictvars, datastream,
+                       context, catch_exception):
+    """``infer`` of ``multinomial_regression``: one ``rxg_multinomial_polya_vmp_f32`` call.  ``returnvars`` is
+    KeepLast() / KeepEach() of ``ψ``; ``free_energy=True`` gives F after every iteration."""
+    if predictvars is not None:
+        raise NotImplementedError("predictvars: predictions of y are outside the batched hot path")
+    if datastream is not None or data is None:
+        raise NotImplementedError("multinomial_regression runs over whole data sets: pass data = {'y'} (the online form "
+                                  "is multinomial_regression_online)")
+    if initialization is not None:
+        raise NotImplementedError("multinomial_regression starts from the prior: initialization is not used")
+    if "y" not in data:
+        raise KeyError("multinomial_regression needs data = {'y': [batch, n, K]}")
+    bad = set(data) - {"y"}
+    if bad:
+        raise ValueError(f"multinomial_regression: unknown data {sorted(bad)} (y)")
+    each = _returns_each(returnvars, "ψ", "multinomial_regression")
+    y = _counts(data["y"], "data['y']")
+    single = y.dim() == 2
+    y = y[None] if single else y
+    if y.dim() != 3:
+        raise ValueError(f"data['y'] must be [batch, n, K] (or [n, K]), got {tuple(y.shape)}")
+    try:
+        ctx = context or default_context()
+        r = ctx.multinomial_polya_vmp(y.to(f"cuda:{ctx.device}").permute(1, 2, 0).contiguous(), model.prior_xi,
+                                      model.prior_precision, iterations=iterations or 1,
+                                      want_free_energy=bool(free_energy), keep_each=each)
+        _raise_flagged(r["status"], "multinomial_regression: ", " (BAD_ARG: a negative count; NOT_SPD: a non-positive "
+                       "pivot; NAN: a non-finite result)")
+        mean, cov = (r["hist_mean"], r["hist_cov"]) if each else (r["psi_mean"], r["psi_cov"])
+        fe = r["free_energy"]
+        if single:
+            mean, cov, fe = mean[..., 0], cov[..., 0], (fe[:, 0] if fe is not None else None)
+        return InferenceResult(posteriors={"ψ": MvNormalMeanCovariance(mean, cov)}, model=model, free_energy=fe)
+    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
+        if catch_exception:
+            return InferenceResult(posteriors={}, model=model, error=e)
+        raise
+
+
+def _infer_multinomial_online(model, data, initialization, autoupdates, iterations, free_energy, returnvars, predictvars,
+                              keephistory, historyvars, datastream, autostart, batch, context):
+    """``infer`` of ``multinomial_regression_online``: an ``RxInferenceEngine`` of kind "multinomial" (the carry q(ψ) in
+    fp64 on the device).  With ``data`` the whole stream is one chunk and the engine is returned completed."""
+    if predictvars is not None or returnvars is not None:
+        raise NotImplementedError("multinomial_regression_online keeps q(ψ) through keephistory; returnvars and "
+                                  "predictvars are outside the batched hot path")
+    if autoupdates is None:
+        raise ValueError("multinomial_regression_online needs autoupdates (ξ_ψ, W_ψ = weightedmean_precision(q(ψ)))")
+    init = initialization.get("ψ") if isinstance(initialization, dict) else None
+    if not isinstance(init, MvNormalWeightedMeanPrecision) or set(initialization) != {"ψ"}:
+        raise ValueError("multinomial_regression_online needs initialization = {'ψ': MvNormalWeightedMeanPrecision(ξ, W)}")
+    from .streaming import RxInferenceEngine
+    y = None
+    if data is not None:
+        if set(data) != {"y"}:
+            raise ValueError(f"multinomial_regression_online: data must be {{'y': [batch, T, K]}}, got {sorted(data)}")
+        y = _counts(data["y"], "data['y']")
+        y = y[None] if y.dim() == 2 else y
+        if y.dim() != 3:
+            raise ValueError(f"data['y'] must be [batch, T, K] (or [T, K]), got {tuple(y.shape)}")
+        if batch is not None and batch != y.shape[0]:
+            raise ValueError(f"batch = {batch}, data['y'] has {y.shape[0]} series")
+    elif batch is None:
+        raise ValueError("streaming inference needs `batch` (number of lock-step datastreams)")
+    ctx = context or default_context()
+    if y is not None:
+        datastream, batch, autostart = [y.to(f"cuda:{ctx.device}").permute(1, 2, 0).contiguous()], y.shape[0], True
+    return RxInferenceEngine(ctx, model, batch=batch, iterations=iterations, keephistory=keephistory,
+                             historyvars=historyvars, free_energy=free_energy, datastream=datastream, autostart=autostart,
+                             initialization=init)
+
+
 def _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
                        datastream, context, catch_exception):
     """``infer`` of ``hgf_offline``: one ``rxg_hgf_vmp_learn_f32`` launch.  ``returnvars``: KeepLast() for x, z (and x_0),
@@ -804,6 +917,18 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
                                       "are outside the batched hot path")
         return _infer_binomial(model, data, initialization, iterations, free_energy, returnvars, predictvars, datastream,
                                context, catch_exception)
+    if isinstance(model, multinomial_regression):
+        if autoupdates is not None or keephistory is not None or historyvars is not None or batch is not None or cov_shared_out:
+            raise NotImplementedError("multinomial_regression: autoupdates, keephistory, historyvars, batch and "
+                                      "cov_shared_out are outside the batched hot path (the online form is "
+                                      "multinomial_regression_online)")
+        return _infer_multinomial(model, data, initialization, iterations, free_energy, returnvars, predictvars,
+                                  datastream, context, catch_exception)
+    if isinstance(model, multinomial_regression_online):
+        if cov_shared_out:
+            raise NotImplementedError("multinomial_regression_online: cov_shared_out is outside the batched hot path")
+        return _infer_multinomial_online(model, data, initialization, autoupdates, iterations, free_energy, returnvars,
+                                         predictvars, keephistory, historyvars, datastream, autostart, batch, context)
     if isinstance(model, hgf_offline):
         return _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
                                   datastream, context, catch_exception)

@@ -274,6 +274,17 @@ binomial_polya_vmp(ctx, p, N, batch, its, xi0, W0, X, y, nt, bm, bc, fe, hm, hc,
          Ptr{Int32}, Cuint),
         ctx.handle, p, N, batch, its, xi0, W0, X, y, nt, bm, bc, fe, hm, hc, st, fl))
 
+multinomial_polya_vmp(ctx, K, n, batch, its, xi0, W0, y, pm, pc, fe, hm, hc, st, fl) =
+    check(ctx, ccall((:rxg_multinomial_polya_vmp_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Int64, Cint, F32P, F32P, Ptr{Int32}, F32P, F32P, Ptr{Float64}, F32P, F32P, Ptr{Int32}, Cuint),
+        ctx.handle, K, n, batch, its, xi0, W0, y, pm, pc, fe, hm, hc, st, fl))
+
+multinomial_polya_online(ctx, K, T, batch, its, xi0, W0, mi, Si, y, mo, So, hm, hc, fe, st, fl) =
+    check(ctx, ccall((:rxg_multinomial_polya_online_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Int64, Cint, F32P, F32P, Ptr{Float64}, Ptr{Float64}, Ptr{Int32}, Ptr{Float64}, Ptr{Float64},
+         F32P, F32P, Ptr{Float64}, Ptr{Int32}, Cuint),
+        ctx.handle, K, T, batch, its, xi0, W0, mi, Si, y, mo, So, hm, hc, fe, st, fl))
+
 # ---- diagnostics
 selftest_umma(ctx, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_f32, LIB), Cint, (Ptr{Cvoid}, F32P, F32P, F32P, Cuint), ctx.handle, A, B, D, fl))
 selftest_umma_shape(ctx, n, k, A, B, D, fl) = check(ctx, ccall((:rxg_selftest_umma_shape_f32, LIB), Cint, (Ptr{Cvoid}, Cint, Cint, F32P, F32P, F32P, Cuint), ctx.handle, n, k, A, B, D, fl))
@@ -974,6 +985,42 @@ function binomial_polya_vmp(ctx::Context, X::Array{Float32, 3}, y::Matrix{Int32}
     Lib.device_free(ctx, fe)
     Lib.device_free(ctx, dy)
     ntrials !== nothing && Lib.device_free(ctx, dn)
+    return (mean = download(hm), cov = download(hc), free_energy = fe_host, status = reinterpret(Int32, download(st)))
+end
+
+"""Bayesian multinomial regression by mean-field Pólya-Gamma VMP over whole data sets (`rxg_multinomial_polya_vmp_f32`,
+DESIGN 3.22), one regression per batch row; the offline model of multinomialreg_tests.jl:
+
+    @model function multinomial_model(y, N, ξ_ψ, W_ψ)
+        ψ ~ MvNormalWeightedMeanPrecision(ξ_ψ, W_ψ)
+        for i in eachindex(y)
+            y[i] ~ MultinomialPolya(N, ψ)
+        end
+    end
+
+`y[batch, K, n]` (Int32 counts; a sample's N is the sum of its counts, an all-zero sample contributes nothing).  `xi0`
+(K - 1 vector) and `W0` ((K - 1) x (K - 1), SPD) are shared by every regression.  Returns the KeepEach posteriors of ψ
+(trailing iteration axis): mean `[batch, K - 1, its]`, covariance `[batch, K - 1, K - 1, its]`, the free energy
+`[batch, its]` (Float64) and the per-regression status.  The online form is `Lib.multinomial_polya_online`, whose fp64
+carry stays on the device between calls.  No GraphPPL pattern routes this model here: the reference test passes
+`options`, which is on the fallback list."""
+function multinomial_polya_vmp(ctx::Context, y::Array{Int32, 3}; xi0, W0, iterations = 100)
+    batch, K, n = size(y)
+    D = K - 1
+    dy = Lib.device_alloc(ctx, sizeof(y))
+    GC.@preserve y Lib.memcpy_h2d(ctx, dy, Ptr{Cvoid}(pointer(y)), sizeof(y))
+    pm, pc = DeviceArray(ctx, batch, D), DeviceArray(ctx, batch, D, D)
+    hm, hc = DeviceArray(ctx, batch, D, iterations), DeviceArray(ctx, batch, D, D, iterations)
+    st = DeviceArray(ctx, batch)
+    fe = Lib.device_alloc(ctx, 8 * batch * iterations)
+    h = (Float32.(collect(xi0)), rowmajor32(W0))
+    GC.@preserve h Lib.multinomial_polya_vmp(ctx, K, n, batch, iterations, pointer(h[1]), pointer(h[2]), Ptr{Int32}(dy),
+                                             pm.ptr, pc.ptr, Ptr{Float64}(fe), hm.ptr, hc.ptr, Ptr{Int32}(st.ptr),
+                                             RXG_PTR_DEVICE)
+    fe_host = Array{Float64}(undef, batch, iterations)
+    GC.@preserve fe_host Lib.memcpy_d2h(ctx, pointer(fe_host), fe, 8 * batch * iterations)
+    Lib.device_free(ctx, fe)
+    Lib.device_free(ctx, dy)
     return (mean = download(hm), cov = download(hc), free_energy = fe_host, status = reinterpret(Int32, download(st)))
 end
 

@@ -25,7 +25,7 @@ class RxInferenceEngine:
     ``Subject``-style datastream).  ``autostart=True`` consumes an iterable datastream immediately."""
 
     def __init__(self, ctx, model, *, batch, iterations=1, keephistory=None, historyvars=None, free_energy=False,
-                 datastream=None, autostart=True, cov_shared_out=False):
+                 datastream=None, autostart=True, cov_shared_out=False, initialization=None):
         from . import inference as I
         self.ctx, self.model, self.batch = ctx, model, int(batch)
         self.iterations = int(iterations or 1)
@@ -54,6 +54,13 @@ class RxInferenceEngine:
             m0 = torch.as_tensor(np.asarray(model.x0[0], np.float32), device=f"cuda:{ctx.device}")
             self._prev_mean = m0[:, None].expand(-1, self.batch).contiguous()      # q(x_t) initialisation, broadcast
             self._carry_cov = np.ascontiguousarray(np.asarray(model.x0[1], np.float32)).copy()
+        elif isinstance(model, I.multinomial_regression_online):
+            self._kind = "multinomial"
+            names = ("ψ",)
+            # the prior of the first datum is the initialization, as the host arrays the C entry takes; the carry
+            # q(ψ) = (m, S) is fp64 on the device once the first chunk has run
+            self._prior = (np.asarray(initialization.xi, np.float64), np.asarray(initialization.W, np.float64))
+            self._carry = None
         else:
             raise NotImplementedError(f"model pattern {type(model).__name__} has no streaming path")
         hv = tuple(historyvars) if historyvars is not None else names
@@ -97,6 +104,8 @@ class RxInferenceEngine:
             if self._kind != "lgssm" and "u" in chunk:
                 raise NotImplementedError("input sequences belong to the LGSSM streaming engine")
             chunk, inputs = chunk["y"], chunk.get("u")
+        if self._kind == "multinomial":
+            return self._push_multinomial(chunk)
         if self._kind == "lgssm":
             mo = self.model
             r = self.ctx.lgssm_filter_chunk(chunk, mo.A, mo.B, mo.P, mo.Q, self._prev_mean, self._carry_cov, u=mo.u,
@@ -129,6 +138,28 @@ class RxInferenceEngine:
             self._carry = o[-1]
             out = {"xt": NormalMeanVariance(o[:, 0], o[:, 1]), "zt": NormalMeanVariance(o[:, 2], o[:, 3])}
         self.ticks += int(chunk.shape[0])
+        self._keep(out)
+        return out
+
+    def _push_multinomial(self, chunk):
+        """One chunk y[Tc, K, batch] (int32 counts on the device) of the multinomial regression: one
+        ``rxg_multinomial_polya_online_f32`` call, the fp64 carry updated in place.  A chunk that flags a chain raises."""
+        from .inference import _raise_flagged
+        m, S = self._carry if self._carry is not None else (None, None)
+        r = self.ctx.multinomial_polya_online(chunk, *self._prior, m=m, S=S, iterations=self.iterations,
+                                              want_free_energy=self.free_energy_enabled, keep_mean=bool(self.keephistory),
+                                              keep_cov=bool(self.keephistory), in_place=m is not None)
+        _raise_flagged(r["status"], "multinomial_regression_online: ", " (BAD_ARG: a negative count; NOT_SPD: a "
+                       "non-positive pivot; NAN: a non-finite result)")
+        self._carry = (r["m"], r["S"])
+        if self.free_energy_enabled:
+            self._fe.append(r["free_energy"])
+        self.ticks += int(chunk.shape[0])
+        out = {"ψ": MvNormalMeanCovariance(r["hist_mean"], r["hist_cov"])} if self.keephistory else {}
+        self._keep(out)
+        return out
+
+    def _keep(self, out):
         if self.keephistory:
             for name in self.historyvars:
                 parts = self._hist.setdefault(name, [])
@@ -138,7 +169,6 @@ class RxInferenceEngine:
                 total = sum(getattr(p, field).shape[0] for p in parts)
                 while len(parts) > 1 and total - getattr(parts[0], field).shape[0] >= self.keephistory:
                     total -= getattr(parts.pop(0), field).shape[0]
-        return out
 
     # -------------------------------------------------------------- results (streaming.jl:16-140)
     @property
@@ -146,6 +176,8 @@ class RxInferenceEngine:
         """Most recent marginals (the reference exposes observables; here: the last tick's values)."""
         if self._kind == "lgssm":
             return {"x_t": (self._prev_mean, self._carry_cov.copy())}
+        if self._kind == "multinomial":      # fp64 carry, [D, batch] / [D, D, batch]
+            return {"ψ": None if self._carry is None else MvNormalMeanCovariance(*self._carry)}
         if self._kind == "vmpgamma":
             c = self._carry
             return {"x_t": None if c is None else NormalMeanVariance(c[0], c[1]),
@@ -172,6 +204,19 @@ class RxInferenceEngine:
         evidence of the whole stream (on this tree BFE = -log evidence)."""
         if not self.free_energy_enabled:
             raise RuntimeError("Bethe Free Energy has not been computed: use `free_energy = true`")
+        if self._kind == "multinomial":
+            raise NotImplementedError("the multinomial regression keeps the free energy of each datum's final iteration "
+                                      "only: free_energy_final_only_history")
         if self._kind in ("vmpgamma", "hgf"):   # reference semantics (streaming.jl:12): per iteration, averaged over the observations
             return torch.cat(self._fe, dim=0).mean(dim=0)
         return torch.stack(self._fe)
+
+    @property
+    def free_energy_final_only_history(self):
+        """The free energy of each datum's final iteration, [ticks, batch] (fp64): KL(q_t || q_{t-1}) minus the bound of
+        datum t's evidence (multinomial regression)."""
+        if not self.free_energy_enabled:
+            raise RuntimeError("Bethe Free Energy has not been computed: use `free_energy = true`")
+        if self._kind != "multinomial":
+            raise NotImplementedError("free_energy_final_only_history is kept by the multinomial regression engine")
+        return torch.cat(self._fe, dim=0)
