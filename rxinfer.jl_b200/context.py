@@ -29,10 +29,29 @@ def _f64(t):
     return ctypes.cast(c_void_p(t.data_ptr() if t is not None else None), ctypes.POINTER(ctypes.c_double))
 
 
+def _u8(t):
+    return ctypes.cast(c_void_p(t.data_ptr() if t is not None else None), L.u8p)
+
+
 def _model32(M):
     """Shared model matrices are small host arrays (row-major fp32)."""
     a = np.ascontiguousarray(np.asarray(M, dtype=np.float32))
     return a, a.ctypes.data_as(L.fp)
+
+
+def _host_arrays(who, arrays, dims, nulls=False):
+    """The host model arrays of one C entry, shape-checked and packed to row-major fp32: ``arrays`` maps each name to
+    (value, expected shape); with ``nulls`` a None value is a null pointer.  ``dims`` names the sizes in the error text
+    (``"K = 3, d = 2"``).  Returns {name: (array, pointer)}; the arrays must outlive the call."""
+    keep = {}
+    for k, (v, shp) in arrays.items():
+        if v is None and nulls:
+            keep[k] = (None, L.as_fp(0))
+            continue
+        keep[k] = _model32(v)
+        if keep[k][0].shape != shp:
+            raise ValueError(f"{who}: {k}: expected shape {shp} ({dims}), got {keep[k][0].shape}")
+    return keep
 
 
 class Context:
@@ -113,20 +132,26 @@ class Context:
             if t.device.index != self.device:
                 raise ValueError(f"tensor lives on cuda:{t.device.index}, this context is bound to cuda:{self.device}")
 
-    def _io(self, t, name, on_dev, dtype=torch.float32, shape=None):
-        """Validate one I/O array of a fused sweep: dtype, contiguity, device (or host), shape."""
+    def _io(self, t, name, on_dev=True, dtype=torch.float32, shape=None, ndim=None):
+        """Validate one tensor an entry reads or writes (None passes): dtype, contiguity, on this context's device (or
+        on the host), then its shape or its number of dimensions.  Dtype, contiguity and host / device come first, so
+        that they are checked without ``self.device``."""
         if t is None:
             return
-        if t.dtype != dtype or not t.is_contiguous():
-            raise ValueError(f"{name}: expected a contiguous {dtype} tensor, got {t.dtype}, "
-                             f"contiguous={t.is_contiguous()} (call .contiguous() / .to({dtype}) explicitly)")
-        if on_dev:
-            if not t.is_cuda or t.device.index != self.device:
-                raise ValueError(f"{name}: expected a tensor on cuda:{self.device} (y is a device array), got {t.device}")
-        elif t.is_cuda:
+        if not isinstance(t, torch.Tensor) or t.dtype != dtype or not t.is_contiguous():
+            got = f"{t.dtype}, contiguous={t.is_contiguous()}" if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f"{name}: expected a contiguous {dtype} tensor, got {got} (call .contiguous() / "
+                             f".to({dtype}) explicitly)")
+        if on_dev and not t.is_cuda:
+            raise ValueError(f"{name}: expected a tensor on cuda (y is a device array), got {t.device}")
+        if on_dev and t.device.index != self.device:
+            raise ValueError(f"{name}: expected a tensor on cuda:{self.device} (y is a device array), got {t.device}")
+        if not on_dev and t.is_cuda:
             raise ValueError(f"{name}: y is a host array, so every data array must be on the host; got {t.device}")
         if shape is not None and tuple(t.shape) != tuple(shape):
             raise ValueError(f"{name}: expected shape {tuple(shape)}, got {tuple(t.shape)}")
+        if ndim is not None and t.dim() != ndim:
+            raise ValueError(f"{name}: expected {ndim} dimensions, got shape {tuple(t.shape)}")
 
     def empty(self, *shape, dtype=torch.float32):
         return torch.empty(*shape, dtype=dtype, device=f"cuda:{self.device}")
@@ -307,10 +332,7 @@ class Context:
         variance) of the initial q(kappa), q(omega), q(z[t]), q(x[t]).  Returns ``xz[T, 4, batch]`` = (m_x, v_x, m_z, v_z),
         ``x0[2, batch]``, ``kw[2, 2, batch]`` = (mean, variance) of q(kappa) then q(omega), ``free_energy[iterations,
         batch]`` (fp64) or None, ``status[batch]`` and, with ``keep_each``, ``hist_kw[iterations, 2, 2, batch]``."""
-        if not (y.is_cuda and y.dtype == torch.float32 and y.is_contiguous() and y.dim() == 2):
-            raise ValueError("hgf_vmp_learn: y must be a contiguous float32 CUDA tensor [T, batch]")
-        if y.device.index != self.device:
-            raise ValueError(f"hgf_vmp_learn: y lives on cuda:{y.device.index}, this context is bound to cuda:{self.device}")
+        self._io(y, "hgf_vmp_learn: y [T, batch]", ndim=2)
         T, batch = y.shape
         pr, ini = np.asarray(prior, np.float32).reshape(-1), np.asarray(init, np.float32).reshape(-1)
         if pr.shape != (8,) or ini.shape != (8,):
@@ -320,11 +342,9 @@ class Context:
         hist = self.empty(its, 2, 2, batch) if keep_each else None
         fe = self.empty(its, batch, dtype=torch.float64) if want_free_energy else None
         st = self.empty(batch, dtype=torch.int32)
-        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
         self._check(self.lib.rxg_hgf_vmp_learn_f32(self.h, T, batch, its, pr.ctypes.data_as(L.fp), float(z_precision),
                                                    float(y_variance), ini.ctypes.data_as(L.fp), _fp(y), _fp(x0), _fp(xz),
-                                                   _fp(kw), _fp(hist), fe_p, ctypes.cast(c_void_p(st.data_ptr()), L.i32p),
-                                                   L.PTR_DEVICE))
+                                                   _fp(kw), _fp(hist), _f64(fe), _i32(st), L.PTR_DEVICE))
         return dict(xz=xz, x0=x0, kw=kw, hist_kw=hist, free_energy=fe, status=st)
 
     def hgf_filter_chunk(self, y, prev, iters=20, kappa=1.0, omega=0.0, z_variance=0.04, y_variance=0.01, out=None,
@@ -385,8 +405,9 @@ class Context:
             w_prior = (m + 1.0, np.eye(m))
         if init_E_W is None:
             init_E_W = m * 1e12 * np.eye(m)                     # mean of vague(Wishart, m): df = m, scale 1e12 I
-        c = self._vmp_setup(y, d, dict(A=A), dict(A=(d, d)), B, m0, S0, P, None, None, None, w_prior, init_E_W, u, iterations,
-                            mask, transition_first, asynchronous, want_free_energy, q_keys=("inv_scale0", "init_E_W"))
+        c = self._vmp_setup("lgssm_vmp_wishart", y, d, dict(A=A), dict(A=(d, d)), B, m0, S0, P, None, None, None,
+                            w_prior, init_E_W, u, iterations, mask, transition_first, asynchronous, want_free_energy,
+                            q_keys=("inv_scale0", "init_E_W"))
         self._check(self.lib.rxg_lgssm_vmp_wishart_f32(       # this entry has no known Q and no outputs for P
             *c.head, c.hp("A"), c.hp("B"), c.hp("P"), c.hp("m0"), c.hp("S0"), c.hp("u"), *c.q[1:], *c.io, *c.w_out[2:],
             *c.tail))
@@ -397,7 +418,7 @@ class Context:
         """Mask pointer and flags of the Wishart VMP entries: a [T, batch] device mask per chain or a [T] pattern shared by
         every chain (staged from the host; kept alive in ``keep``)."""
         flags = L.PTR_DEVICE
-        mask_p = ctypes.cast(c_void_p(None), L.u8p)
+        mask_p = _u8(None)
         if mask is not None and getattr(mask, "ndim", 2) == 1:
             sm = np.ascontiguousarray(np.asarray(mask.cpu() if isinstance(mask, torch.Tensor) else mask, dtype=np.uint8))
             if sm.shape != (T,):
@@ -407,7 +428,7 @@ class Context:
             flags |= L.MASK_SHARED
         elif mask is not None:
             self._io(mask, "mask", True, dtype=torch.uint8, shape=(T, batch))
-            mask_p = ctypes.cast(c_void_p(mask.data_ptr()), L.u8p)
+            mask_p = _u8(mask)
         if transition_first:
             flags |= L.TRANSITION_FIRST
         if asynchronous:
@@ -428,8 +449,9 @@ class Context:
         after every iteration (None for a known noise), free_energy[iterations, batch] fp64 or None, status[batch])."""
         self._vmp_dims(y)
         d = np.asarray(A).shape[-1]
-        c = self._vmp_setup(y, d, dict(A=A), dict(A=(d, d)), B, m0, S0, P, p_prior, p_init, Q, q_prior, q_init, u, iterations,
-                            mask, transition_first, asynchronous, want_free_energy, both_known_ok=False)
+        c = self._vmp_setup("lgssm_vmp_noise", y, d, dict(A=A), dict(A=(d, d)), B, m0, S0, P, p_prior, p_init, Q,
+                            q_prior, q_init, u, iterations, mask, transition_first, asynchronous, want_free_energy,
+                            both_known_ok=False)
         self._check(self.lib.rxg_lgssm_vmp_noise_f32(
             *c.head, c.hp("A"), c.hp("B"), c.hp("m0"), c.hp("S0"), c.hp("u"), *c.p, *c.q, *c.io, *c.w_out, *c.tail))
         return dict(mean=c.mean, cov=c.cov, **c.out, free_energy=c.fe, status=c.st)
@@ -440,12 +462,13 @@ class Context:
             raise ValueError(f"y: expected [T, m, batch], got shape {tuple(y.shape)}")
         return y.shape
 
-    def _vmp_setup(self, y, d, mats, shapes, B, m0, S0, P, p_prior, p_init, Q, q_prior, q_init, u, iterations, mask,
-                   transition_first, asynchronous, want_free_energy, both_known_ok=True,
+    def _vmp_setup(self, who, y, d, mats, shapes, B, m0, S0, P, p_prior, p_init, Q, q_prior, q_init, u, iterations,
+                   mask, transition_first, asynchronous, want_free_energy, both_known_ok=True,
                    q_keys=("inv_scale_q0", "init_E_Wq")):
-        """Shared argument handling of the Wishart VMP entries: each noise known or (prior, init), its host arrays named
-        ``inv_scale_p0`` / ``init_E_Wp`` and ``q_keys`` in the error texts; host model arrays converted to row-major fp32
-        and shape-checked (kept alive in ``keep``); then y and the mask validated and the outputs allocated.  Returns the
+        """Shared argument handling of the Wishart VMP entries (``who`` in the error texts): each noise known or
+        (prior, init), its host arrays named ``inv_scale_p0`` / ``init_E_Wp`` and ``q_keys`` in the error texts; host
+        model arrays converted to row-major fp32 and shape-checked (kept alive in ``keep``); then y and the mask
+        validated and the outputs allocated.  Returns the
         pieces of the C call: ``head`` (context and sizes), ``hp(key)`` (a host array's pointer, null if absent), ``p`` /
         ``q`` (known, nu0, inv_scale0, init_E_W), ``io`` (y, mask, mean, cov), ``w_out`` (df_p, inv_scale_p, df_q,
         inv_scale_q; null for a known noise), ``tail`` (free energy, status, flags), next to the output tensors."""
@@ -473,12 +496,7 @@ class Context:
             raise ValueError("P and Q are both known: that is the plain smoother (Context.lgssm)")
         if u is not None:
             shapes["u"], mats["u"] = (d,), u
-        keep = {}
-        for k, v in mats.items():
-            a, p = _model32(v)
-            if a.shape != shapes[k]:
-                raise ValueError(f"{k}: expected shape {shapes[k]}, got {a.shape}")
-            keep[k] = (a, p)
+        keep = _host_arrays(who, {k: (v, shapes[k]) for k, v in mats.items()}, f"d = {d}, m = {m}")
         self._io(y, "y", True)
         mask_p, flags = self._vmp_mask_flags(mask, T, batch, keep, transition_first, asynchronous)
         c = SimpleNamespace(keep=keep, iterations=iterations, batch=batch, mean=self.empty(T, d, batch),
@@ -494,8 +512,7 @@ class Context:
         c.p, c.q = ((c.hp(name.upper()), nus.get(name, 0.0), *map(c.hp, keys[name])) for name in ("p", "q"))
         c.io = (_fp(y), mask_p, _fp(c.mean), _fp(c.cov))
         c.w_out = tuple(_fp(c.out[k]) for k in ("df_p", "inv_scale_p", "df_q", "inv_scale_q"))
-        c.tail = (ctypes.cast(c_void_p(c.fe.data_ptr() if c.fe is not None else None), ctypes.POINTER(ctypes.c_double)),
-                  ctypes.cast(c_void_p(c.st.data_ptr()), L.i32p), flags)
+        c.tail = (_f64(c.fe), _i32(c.st), flags)
         return c
 
     def lgssm_vmp_transition(self, y, B, m0, S0, *, a_prior, a_init, P=None, Q=None, p_prior=None, p_init=None,
@@ -518,8 +535,8 @@ class Context:
         mats = dict(a_mean0=np.asarray(a_prior[0]).reshape(-1), a_cov0=a_prior[1],
                     a_init_mean=np.asarray(a_init[0]).reshape(-1), a_init_cov=a_init[1])
         shapes = dict(a_mean0=(n,), a_cov0=(n, n), a_init_mean=(n,), a_init_cov=(n, n))
-        c = self._vmp_setup(y, d, mats, shapes, B, m0, S0, P, p_prior, p_init, Q, q_prior, q_init, u, iterations, mask,
-                            transition_first, asynchronous, want_free_energy)
+        c = self._vmp_setup("lgssm_vmp_transition", y, d, mats, shapes, B, m0, S0, P, p_prior, p_init, Q, q_prior,
+                            q_init, u, iterations, mask, transition_first, asynchronous, want_free_energy)
         a_mean, a_cov = self.empty(c.iterations, d, d, c.batch), self.empty(c.iterations, n, n, c.batch)
         self._check(self.lib.rxg_lgssm_vmp_transition_f32(
             *c.head, c.hp("a_mean0"), c.hp("a_cov0"), c.hp("a_init_mean"), c.hp("a_init_cov"), c.hp("B"), c.hp("m0"),
@@ -569,7 +586,7 @@ class Context:
         xi, W = self.empty(di, n), self.empty(di, di, n)
         st = self.empty(n, dtype=torch.int32)
         self._check(self.lib.rxg_rule_mul_in_f32(self.h, n, do, di, Ap, shared, _fp(mu_out), _fp(S_out), _fp(xi), _fp(W),
-                                                 ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+                                                 _i32(st), L.PTR_DEVICE))
         return xi, W, st
 
     def _pair(self, fn, a, Sa, b, Sb):
@@ -593,7 +610,7 @@ class Context:
         d, n = v.shape
         vo, Mo = torch.empty_like(v), torch.empty_like(M)
         st = self.empty(n, dtype=torch.int32)
-        self._check(fn(self.h, n, d, _fp(v), _fp(M), _fp(vo), _fp(Mo), ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+        self._check(fn(self.h, n, d, _fp(v), _fp(M), _fp(vo), _fp(Mo), _i32(st), L.PTR_DEVICE))
         return vo, Mo, st
 
     def meancov_to_wmp(self, mu, S):
@@ -612,7 +629,7 @@ class Context:
         mu, S = self.empty(d, n), self.empty(d, d, n)
         st = self.empty(n, dtype=torch.int32)
         self._check(self.lib.rxg_marginal_gaussian_f32(self.h, n, d, k, xs, ws, _fp(mu), _fp(S),
-                                                       ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+                                                       _i32(st), L.PTR_DEVICE))
         return mu, S, st
 
     def _six(self, fn, a, b, c, d_):
@@ -657,7 +674,7 @@ class Context:
         out = self.empty(d, d, n)
         st = self.empty(n, dtype=torch.int32)
         self._check(self.lib.rxg_wishart_mean_f32(self.h, n, d, _fp(df), _fp(iS), _fp(out),
-                                                  ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+                                                  _i32(st), L.PTR_DEVICE))
         return out, st
 
     def mv_iid_wishart_vmp(self, y, iterations=10, mu0=None, Lambda0=None, nu0=None, inv_scale0=None, init_E_P=None):
@@ -676,7 +693,7 @@ class Context:
         st = self.empty(batch, dtype=torch.int32)
         self._check(self.lib.rxg_mv_iid_wishart_vmp_f32(self.h, d, N, batch, iterations, keep[0][1], keep[1][1], float(nu0),
                                                         keep[2][1], keep[3][1], _fp(y), _fp(mm), _fp(mc), _fp(df), _fp(iS),
-                                                        ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+                                                        _i32(st), L.PTR_DEVICE))
         return dict(m_mean=mm, m_cov=mc, df=df, inv_scale=iS, status=st)
 
     def ar_vmp(self, series, order, iterations=15, gamma_prior=(1.0, 1.0), theta_prior_precision=1.0, init_gamma=(1.0, 1.0),
@@ -687,10 +704,9 @@ class Context:
         tm, tc = self.empty(order, batch), self.empty(order, order, batch)
         gs, gr = self.empty(batch), self.empty(batch)
         fe = self.empty(iterations, batch, dtype=torch.float64) if want_free_energy else None      # fp64 output (see the header)
-        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
         self._check(self.lib.rxg_ar_vmp_f32(self.h, order, N, batch, iterations, gamma_prior[0], gamma_prior[1], theta_prior_precision,
-                                            init_gamma[0], init_gamma[1], _fp(series), _fp(tm), _fp(tc), _fp(gs), _fp(gr), fe_p,
-                                            L.PTR_DEVICE))
+                                            init_gamma[0], init_gamma[1], _fp(series), _fp(tm), _fp(tc), _fp(gs),
+                                            _fp(gr), _f64(fe), L.PTR_DEVICE))
         return dict(theta_mean=tm, theta_cov=tc, gamma_shape=gs, gamma_rate=gr, free_energy=fe)
 
     def lar_vmp(self, y, order, tau, iterations=15, gamma_prior=(1.0, 1.0), theta_prior_precision=1.0, x0_prior_precision=1.0,
@@ -711,10 +727,9 @@ class Context:
         gs, gr = self.empty(iters, batch), self.empty(iters, batch)
         fe = self.empty(iters, batch, dtype=torch.float64) if want_free_energy else None
         st = self.empty(batch, dtype=torch.int32)
-        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
         self._check(self.lib.rxg_lar_vmp_f32(self.h, int(order), T, batch, iters, ctypes.cast(prm, L.fp), _fp(y), _fp(xm), _fp(xc),
-                                             _fp(tm), _fp(tc), _fp(gs), _fp(gr), fe_p,
-                                             ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+                                             _fp(tm), _fp(tc), _fp(gs), _fp(gr), _f64(fe),
+                                             _i32(st), L.PTR_DEVICE))
         return dict(x_mean=xm, x_cov=xc, theta_mean=tm, theta_cov=tc, gamma_shape=gs, gamma_rate=gr, free_energy=fe, status=st)
 
     def gmm_vmp(self, y, alpha0, mu0, V0, nu0, S0, alpha_init, m_init, Vm_init, nu_init, S_init, iterations=10,
@@ -730,16 +745,10 @@ class Context:
             raise ValueError("gmm_vmp: y must be [N, d, batch]")
         N, d, batch = y.shape
         K = int(np.asarray(alpha0).shape[0])
-        shapes = dict(alpha0=(K,), mu0=(K, d), V0=(K, d, d), nu0=(K,), S0=(K, d, d), alpha_init=(K,), m_init=(K, d),
-                      Vm_init=(K, d, d), nu_init=(K,), S_init=(K, d, d))
-        vals = dict(alpha0=alpha0, mu0=mu0, V0=V0, nu0=nu0, S0=S0, alpha_init=alpha_init, m_init=m_init, Vm_init=Vm_init,
-                    nu_init=nu_init, S_init=S_init)
-        keep = {}
-        for k, shp in shapes.items():
-            a = np.asarray(vals[k], dtype=np.float64)
-            if a.shape != shp:
-                raise ValueError(f"gmm_vmp: {k} must have shape {shp} (K = {K}, d = {d}), got {a.shape}")
-            keep[k] = _model32(a)
+        keep = _host_arrays("gmm_vmp", dict(alpha0=(alpha0, (K,)), mu0=(mu0, (K, d)), V0=(V0, (K, d, d)),
+                                            nu0=(nu0, (K,)), S0=(S0, (K, d, d)), alpha_init=(alpha_init, (K,)),
+                                            m_init=(m_init, (K, d)), Vm_init=(Vm_init, (K, d, d)),
+                                            nu_init=(nu_init, (K,)), S_init=(S_init, (K, d, d))), f"K = {K}, d = {d}")
         its = int(iterations)
         al, mm, mc = self.empty(K, batch), self.empty(K, d, batch), self.empty(K, d, d, batch)
         df, iS = self.empty(K, batch), self.empty(K, d, d, batch)
@@ -749,12 +758,11 @@ class Context:
                  hist_m_cov=self.empty(its, K, d, d, batch), hist_w_df=self.empty(its, K, batch),
                  hist_w_inv_scale=self.empty(its, K, d, d, batch)) if keep_each else {}
         st = self.empty(batch, dtype=torch.int32)
-        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
-        self._check(self.lib.rxg_gmm_vmp_f32(self.h, d, K, N, batch, its, *(keep[k][1] for k in shapes), _fp(y), _fp(al),
-                                             _fp(mm), _fp(mc), _fp(df), _fp(iS), fe_p, _fp(z),
+        self._check(self.lib.rxg_gmm_vmp_f32(self.h, d, K, N, batch, its, *(p for _, p in keep.values()), _fp(y),
+                                             _fp(al), _fp(mm), _fp(mc), _fp(df), _fp(iS), _f64(fe), _fp(z),
                                              *(_fp(h.get(k)) for k in ("hist_alpha", "hist_m_mean", "hist_m_cov",
                                                                          "hist_w_df", "hist_w_inv_scale")),
-                                             ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+                                             _i32(st), L.PTR_DEVICE))
         out = dict(alpha=al, m_mean=mm, m_cov=mc, w_df=df, w_inv_scale=iS, free_energy=fe, z_prob=z, status=st)
         out.update(h)
         return out
@@ -767,27 +775,17 @@ class Context:
         with shape [M, K].  Returns ``s_prob[T, K, batch]``, ``s0_prob[K, batch]``, ``A_alpha[K, K, batch]`` /
         ``B_alpha[M, K, batch]`` (None when known), ``free_energy[iterations, batch]`` (fp64), ``status[batch]`` and, with
         ``keep_each``, ``hist_s`` / ``hist_A`` / ``hist_B`` with a leading iteration axis."""
-        if not (x.is_cuda and x.dtype == torch.uint8 and x.is_contiguous() and x.dim() == 2):
-            raise ValueError("hmm_vmp: x must be a contiguous uint8 CUDA tensor [T, batch]")
-        if x.device.index != self.device:
-            raise ValueError(f"hmm_vmp: x lives on cuda:{x.device.index}, this context is bound to cuda:{self.device}")
+        self._io(x, "hmm_vmp: x [T, batch]", dtype=torch.uint8, ndim=2)
         T, batch = x.shape
         K = int(np.asarray(p0).reshape(-1).shape[0])
         B_any = B_known if B_known is not None else B_prior
         if B_any is None:
             raise ValueError("hmm_vmp: pass either B_prior and B_init (B learned) or B_known")
         M = int(np.asarray(B_any).shape[0])
-        vals = dict(p0=(p0, (K,)), A_prior=(A_prior, (K, K)), A_init=(A_init, (K, K)), A_known=(A_known, (K, K)),
-                    B_prior=(B_prior, (M, K)), B_init=(B_init, (M, K)), B_known=(B_known, (M, K)))
-        keep = {}
-        for k, (v, shp) in vals.items():
-            if v is None:
-                keep[k] = (None, L.as_fp(0))
-                continue
-            a = np.asarray(v, dtype=np.float64)
-            if a.shape != shp:
-                raise ValueError(f"hmm_vmp: {k} must have shape {shp} (K = {K}, M = {M}), got {a.shape}")
-            keep[k] = _model32(a)
+        keep = _host_arrays("hmm_vmp", dict(p0=(p0, (K,)), A_prior=(A_prior, (K, K)), A_init=(A_init, (K, K)),
+                                            A_known=(A_known, (K, K)), B_prior=(B_prior, (M, K)),
+                                            B_init=(B_init, (M, K)), B_known=(B_known, (M, K))),
+                            f"K = {K}, M = {M}", nulls=True)
         learn_A, learn_B = A_known is None, B_known is None
         its = int(iterations)
         sp, s0 = self.empty(T, K, batch), self.empty(K, batch)
@@ -800,12 +798,9 @@ class Context:
             h["hist_A"] = self.empty(its, K, K, batch) if learn_A else None
             h["hist_B"] = self.empty(its, M, K, batch) if learn_B else None
         st = self.empty(batch, dtype=torch.int32)
-        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
-        self._check(self.lib.rxg_hmm_vmp_f32(self.h, K, M, T, batch, its, *(keep[k][1] for k in vals),
-                                             ctypes.cast(c_void_p(x.data_ptr()), L.u8p), _fp(sp), _fp(s0), _fp(Aa),
-                                             _fp(Ba), fe_p, _fp(h.get("hist_s")), _fp(h.get("hist_A")),
-                                             _fp(h.get("hist_B")), ctypes.cast(c_void_p(st.data_ptr()), L.i32p),
-                                             L.PTR_DEVICE))
+        self._check(self.lib.rxg_hmm_vmp_f32(self.h, K, M, T, batch, its, *(p for _, p in keep.values()), _u8(x),
+                                             _fp(sp), _fp(s0), _fp(Aa), _fp(Ba), _f64(fe), _fp(h.get("hist_s")),
+                                             _fp(h.get("hist_A")), _fp(h.get("hist_B")), _i32(st), L.PTR_DEVICE))
         out = dict(s_prob=sp, s0_prob=s0, A_alpha=Aa, B_alpha=Ba, free_energy=fe, status=st)
         out.update(h)
         return out
@@ -828,15 +823,7 @@ class Context:
         vals = dict(p0=(p0, (K,)), A_prior=(A_prior, (K, K)), A_init=(A_init, (K, K)), A_known=(A_known, (K, K)),
                     mu0=(mu0, (K, d)), V0=(V0, (K, d, d)), nu0=(nu0, (K,)), S0=(S0, (K, d, d)), m_init=(m_init, (K, d)),
                     Vm_init=(Vm_init, (K, d, d)), nu_init=(nu_init, (K,)), S_init=(S_init, (K, d, d)))
-        keep = {}
-        for k, (v, shp) in vals.items():
-            if v is None:
-                keep[k] = (None, L.as_fp(0))
-                continue
-            a = np.asarray(v, dtype=np.float64)
-            if a.shape != shp:
-                raise ValueError(f"hmm_gauss_vmp: {k} must have shape {shp} (K = {K}, d = {d}), got {a.shape}")
-            keep[k] = _model32(a)
+        keep = _host_arrays("hmm_gauss_vmp", vals, f"K = {K}, d = {d}", nulls=True)
         learn_A = A_known is None
         its = int(iterations)
         sp, s0 = self.empty(T, K, batch), self.empty(K, batch)
@@ -847,12 +834,12 @@ class Context:
                  hist_m_mean=self.empty(its, K, d, batch), hist_m_cov=self.empty(its, K, d, d, batch),
                  hist_w_df=self.empty(its, K, batch), hist_w_inv_scale=self.empty(its, K, d, d, batch)) if keep_each else {}
         st = self.empty(batch, dtype=torch.int32)
-        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
-        self._check(self.lib.rxg_hmm_gauss_vmp_f32(self.h, d, K, T, batch, its, *(keep[k][1] for k in vals), _fp(y), _fp(sp),
-                                                   _fp(s0), _fp(Aa), _fp(mm), _fp(mc), _fp(df), _fp(iS), fe_p,
+        self._check(self.lib.rxg_hmm_gauss_vmp_f32(self.h, d, K, T, batch, its, *(p for _, p in keep.values()), _fp(y),
+                                                   _fp(sp), _fp(s0), _fp(Aa), _fp(mm), _fp(mc), _fp(df), _fp(iS),
+                                                   _f64(fe),
                                                    *(_fp(h.get(k)) for k in ("hist_s", "hist_A", "hist_m_mean", "hist_m_cov",
                                                                                "hist_w_df", "hist_w_inv_scale")),
-                                                   ctypes.cast(c_void_p(st.data_ptr()), L.i32p), L.PTR_DEVICE))
+                                                   _i32(st), L.PTR_DEVICE))
         out = dict(s_prob=sp, s0_prob=s0, A_alpha=Aa, m_mean=mm, m_cov=mc, w_df=df, w_inv_scale=iS, free_energy=fe, status=st)
         out.update(h)
         return out
@@ -868,30 +855,20 @@ class Context:
         if X.dim() != 3:
             raise ValueError("binomial_polya_vmp: X must be [N, p, batch]")
         N, p, batch = X.shape
-        for name, t in (("y", y), ("ntrials", ntrials)):
-            if t is None and name == "ntrials":
-                continue
-            if not (t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and tuple(t.shape) == (N, batch)):
-                raise ValueError(f"binomial_polya_vmp: {name} must be a contiguous int32 CUDA tensor [N, batch] = {(N, batch)}")
-            if t.device.index != self.device:
-                raise ValueError(f"binomial_polya_vmp: {name} lives on cuda:{t.device.index}, this context is bound to "
-                                 f"cuda:{self.device}")
-        keep = {}
-        for k, (v, shp) in dict(xi0=(xi0, (p,)), W0=(W0, (p, p))).items():
-            a = np.asarray(v, dtype=np.float64)
-            if a.shape != shp:
-                raise ValueError(f"binomial_polya_vmp: {k} must have shape {shp} (p = {p}), got {a.shape}")
-            keep[k] = _model32(a)
+        if y is None:
+            raise ValueError("binomial_polya_vmp: y is required")
+        self._io(y, "binomial_polya_vmp: y [N, batch]", dtype=torch.int32, shape=(N, batch))
+        self._io(ntrials, "binomial_polya_vmp: ntrials [N, batch]", dtype=torch.int32, shape=(N, batch))
+        keep = _host_arrays("binomial_polya_vmp", dict(xi0=(xi0, (p,)), W0=(W0, (p, p))), f"p = {p}")
         its = int(iterations)
         mean, cov = self.empty(p, batch), self.empty(p, p, batch)
         fe = self.empty(its, batch, dtype=torch.float64) if want_free_energy else None
         h = dict(hist_mean=self.empty(its, p, batch), hist_cov=self.empty(its, p, p, batch)) if keep_each else {}
         st = self.empty(batch, dtype=torch.int32)
-        i32 = lambda t: ctypes.cast(c_void_p(t.data_ptr() if t is not None else None), L.i32p)
-        fe_p = ctypes.cast(c_void_p(fe.data_ptr() if fe is not None else None), ctypes.POINTER(ctypes.c_double))
-        self._check(self.lib.rxg_binomial_polya_vmp_f32(self.h, p, N, batch, its, keep["xi0"][1], keep["W0"][1], _fp(X), i32(y),
-                                                        i32(ntrials), _fp(mean), _fp(cov), fe_p, _fp(h.get("hist_mean")),
-                                                        _fp(h.get("hist_cov")), i32(st), L.PTR_DEVICE))
+        self._check(self.lib.rxg_binomial_polya_vmp_f32(self.h, p, N, batch, its, keep["xi0"][1], keep["W0"][1], _fp(X),
+                                                        _i32(y), _i32(ntrials), _fp(mean), _fp(cov), _f64(fe),
+                                                        _fp(h.get("hist_mean")), _fp(h.get("hist_cov")), _i32(st),
+                                                        L.PTR_DEVICE))
         out = dict(beta_mean=mean, beta_cov=cov, free_energy=fe, status=st)
         out.update(h)
         return out
@@ -899,18 +876,9 @@ class Context:
     def _multinomial_args(self, who, y, xi0, W0):
         """y: a contiguous int32 CUDA tensor [n, K, batch] on this context's device; the prior (xi0 [D], W0 [D, D], D = K - 1)
         as the fp32 host arrays the C entries take."""
-        if not (isinstance(y, torch.Tensor) and y.is_cuda and y.dtype == torch.int32 and y.is_contiguous() and y.dim() == 3):
-            raise ValueError(f"{who}: y must be a contiguous int32 CUDA tensor [n, K, batch]")
-        if y.device.index != self.device:
-            raise ValueError(f"{who}: y lives on cuda:{y.device.index}, this context is bound to cuda:{self.device}")
+        self._io(y, f"{who}: y [n, K, batch]", dtype=torch.int32, ndim=3)
         D = y.shape[1] - 1
-        keep = {}
-        for k, (v, shp) in dict(xi0=(xi0, (D,)), W0=(W0, (D, D))).items():
-            a = np.asarray(v, dtype=np.float64)
-            if a.shape != shp:
-                raise ValueError(f"{who}: {k} must have shape {shp} (K = {D + 1}), got {a.shape}")
-            keep[k] = _model32(a)
-        return D, keep
+        return D, _host_arrays(who, dict(xi0=(xi0, (D,)), W0=(W0, (D, D))), f"K = {D + 1}")
 
     def multinomial_polya_vmp(self, y, xi0, W0, iterations=1, want_free_energy=True, keep_each=False):
         """Bayesian multinomial regression by mean-field Polya-Gamma VMP over whole data sets
@@ -944,12 +912,8 @@ class Context:
         T, K, batch = y.shape
         if (m is None) != (S is None):
             raise ValueError("multinomial_polya_online: pass the carry m and S together, or neither")
-        if m is not None:
-            for name, t, shp in (("m", m, (D, batch)), ("S", S, (D, D, batch))):
-                if not (t.is_cuda and t.dtype == torch.float64 and t.is_contiguous() and tuple(t.shape) == shp
-                        and t.device.index == self.device):
-                    raise ValueError(f"multinomial_polya_online: {name} must be a contiguous float64 tensor {shp} on "
-                                     f"cuda:{self.device}")
+        self._io(m, "multinomial_polya_online: m [D, batch]", dtype=torch.float64, shape=(D, batch))
+        self._io(S, "multinomial_polya_online: S [D, D, batch]", dtype=torch.float64, shape=(D, D, batch))
         if in_place and m is None:
             raise ValueError("multinomial_polya_online: in_place needs a carry")
         m_out = m if in_place else self.empty(D, batch, dtype=torch.float64)

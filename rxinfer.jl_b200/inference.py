@@ -12,6 +12,7 @@ being silently ignored (SURVEY.md appendix C: those calls must be routed to stoc
 from __future__ import annotations
 
 from dataclasses import dataclass, field
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -166,24 +167,25 @@ class gaussian_mixture:
     w_prior: list
 
 
-class MeanField:
+class _Marker:
+    """An argument that stands for a choice, not a value: every instance of a marker class is equal to every other."""
+
+    def __eq__(self, other):
+        return isinstance(other, type(self))
+
+    def __hash__(self):
+        return hash(type(self))
+
+    def __repr__(self):
+        return f"{type(self).__name__}()"
+
+
+class MeanField(_Marker):
     """``constraints = MeanField()``: the naive mean-field factorisation q(s) prod q(m[k]) prod q(w[k]) prod q(z[i])."""
 
-    def __eq__(self, other):
-        return isinstance(other, MeanField)
 
-    def __hash__(self):
-        return hash(MeanField)
-
-
-class BetheFactorization:
+class BetheFactorization(_Marker):
     """``BetheFactorization()``: the reference's default constraints (no factorisation of the local joints)."""
-
-    def __eq__(self, other):
-        return isinstance(other, BetheFactorization)
-
-    def __hash__(self):
-        return hash(BetheFactorization)
 
 
 def _weights(x, K, what):
@@ -227,6 +229,36 @@ def _precisions(xs, K, what):
     return np.array(nu), np.stack(S)
 
 
+def _emission_arrays(model, init, K):
+    """The NormalMixture emission arrays of the C entries: mu0[K, d], V0[K, d, d] (covariance), nu0[K], S0[K, d, d]
+    (Wishart scale) from ``model.m_prior`` / ``model.w_prior``, and the same for the initial q(m), q(w) of ``init``."""
+    out = {}
+    out["mu0"], out["V0"] = _gaussians(model.m_prior, K, "m_prior")
+    out["m_init"], out["Vm_init"] = _gaussians(init["m"], K, "initialization['m']")
+    out["nu0"], out["S0"] = _precisions(model.w_prior, K, "w_prior")
+    out["nu_init"], out["S_init"] = _precisions(init["w"], K, "initialization['w']")
+    d = out["mu0"].shape[1]
+    for k in ("m_init", "V0", "Vm_init", "S0", "S_init"):
+        if out[k].shape[1] != d:
+            raise ValueError(f"{k}: dimension {out[k].shape[1]}, the means have d = {d}")
+    return out
+
+
+def _component_posteriors(r, each, univariate):
+    """q(m[k]) and q(w[k]) of every NormalMixture component from a result of the C entry: the last iteration's, or
+    with a leading iteration axis (``hist_*``) for ``m`` / ``w`` in ``each``; Normal / Gamma when the model was
+    ``univariate``."""
+    mp = "hist_" if "m" in each else ""
+    wp = "hist_" if "w" in each else ""
+    mm, mc, df, iS = r[mp + "m_mean"], r[mp + "m_cov"], r[wp + "w_df"], r[wp + "w_inv_scale"]
+    K = mm.shape[-3]
+    if univariate:
+        return ([NormalMeanVariance(mm[..., k, 0, :], mc[..., k, 0, 0, :]) for k in range(K)],
+                [GammaShapeRate(df[..., k, :] / 2, iS[..., k, 0, 0, :] / 2) for k in range(K)])
+    return ([MvNormalMeanCovariance(mm[..., k, :, :], mc[..., k, :, :, :]) for k in range(K)],
+            [WishartFast(df[..., k, :], iS[..., k, :, :, :]) for k in range(K)])
+
+
 def gaussian_mixture_arrays(model, initialization):
     """The model and its ``initialization`` in the Dirichlet / MvNormal / Wishart form of the C entry: a dict of host
     arrays alpha0[K], mu0[K, d], V0[K, d, d], nu0[K], S0[K, d, d] and the same for the initial marginals (``*_init``,
@@ -235,14 +267,7 @@ def gaussian_mixture_arrays(model, initialization):
     if not isinstance(initialization, dict) or not {"s", "m", "w"} <= set(initialization):
         raise ValueError("gaussian_mixture needs initialization = {'s': q(s), 'm': [q(m[k])], 'w': [q(w[k])]}")
     out = dict(alpha0=_weights(model.alpha0, K, "alpha0"), alpha_init=_weights(initialization["s"], K, "initialization['s']"))
-    out["mu0"], out["V0"] = _gaussians(model.m_prior, K, "m_prior")
-    out["m_init"], out["Vm_init"] = _gaussians(initialization["m"], K, "initialization['m']")
-    out["nu0"], out["S0"] = _precisions(model.w_prior, K, "w_prior")
-    out["nu_init"], out["S_init"] = _precisions(initialization["w"], K, "initialization['w']")
-    d = out["mu0"].shape[1]
-    for k in ("m_init", "V0", "Vm_init", "S0", "S_init"):
-        if out[k].shape[1] != d:
-            raise ValueError(f"{k}: dimension {out[k].shape[1]}, the means have d = {d}")
+    out.update(_emission_arrays(model, initialization, K))
     out["univariate"] = isinstance(model.alpha0, Beta)
     return out
 
@@ -267,14 +292,8 @@ class hidden_markov_model:
     B: object
 
 
-class HMMConstraints:
+class HMMConstraints(_Marker):
     """``q(s, s_0, A, B) = q(s, s_0) q(A) q(B)`` (hmm_tests.jl:22-24): the chain is kept structured, the matrices apart."""
-
-    def __eq__(self, other):
-        return isinstance(other, HMMConstraints)
-
-    def __hash__(self):
-        return hash(HMMConstraints)
 
 
 def check_hmm_constraints(constraints):
@@ -303,31 +322,39 @@ def hmm_symbols(x, M):
     return sym.contiguous()
 
 
+def _p0(model):
+    return np.asarray(model.p0.p if isinstance(model.p0, Categorical) else model.p0, np.float64).reshape(-1)
+
+
+def _matrix_arguments(model, name, init, K):
+    """``{name}_known`` of a ``PointMass`` probability matrix, or ``{name}_prior`` and ``{name}_init`` of a learned
+    ``DirichletCollection`` (its q from ``init``); the matrix is K x K for A and M x K for B."""
+    v = getattr(model, name)
+    if isinstance(v, PointMass):
+        out = {f"{name}_known": np.asarray(v.value, np.float64)}
+    elif isinstance(v, DirichletCollection):
+        if not isinstance(init.get(name), DirichletCollection):
+            raise ValueError(f"{name} is learned: pass initialization = {{'{name}': DirichletCollection(...)}}, e.g. "
+                             f"vague(DirichletCollection, {np.asarray(v.alpha).shape})")
+        out = {f"{name}_prior": np.asarray(v.alpha, np.float64),
+               f"{name}_init": np.asarray(init[name].alpha, np.float64)}
+        if out[f"{name}_init"].shape != out[f"{name}_prior"].shape:
+            raise ValueError(f"initialization['{name}'] has shape {out[f'{name}_init'].shape}, the prior "
+                             f"{out[f'{name}_prior'].shape}")
+    else:
+        raise TypeError(f"model.{name}: expected DirichletCollection or PointMass, got {type(v).__name__}")
+    shape = next(iter(out.values())).shape
+    if len(shape) != 2 or shape[1] != K or (name == "A" and shape[0] != K):
+        raise ValueError(f"model.{name} has shape {shape}; with K = {K} states A is K x K and B is M x K")
+    return out
+
+
 def hmm_arguments(model, initialization):
     """The keyword arguments of ``Context.hmm_vmp`` for ``model`` and ``initialization``."""
-    p0 = np.asarray(model.p0.p if isinstance(model.p0, Categorical) else model.p0, np.float64).reshape(-1)
-    K = p0.shape[0]
+    p0 = _p0(model)
     init = initialization or {}
-    out = {"p0": p0}
-    for name in ("A", "B"):
-        v = getattr(model, name)
-        if isinstance(v, PointMass):
-            out[f"{name}_known"] = np.asarray(v.value, np.float64)
-            shape = out[f"{name}_known"].shape
-        elif isinstance(v, DirichletCollection):
-            if not isinstance(init.get(name), DirichletCollection):
-                raise ValueError(f"{name} is learned: pass initialization = {{'{name}': DirichletCollection(...)}}, e.g. "
-                                 f"vague(DirichletCollection, {np.asarray(v.alpha).shape})")
-            out[f"{name}_prior"] = np.asarray(v.alpha, np.float64)
-            out[f"{name}_init"] = np.asarray(init[name].alpha, np.float64)
-            shape = out[f"{name}_prior"].shape
-            if out[f"{name}_init"].shape != shape:
-                raise ValueError(f"initialization['{name}'] has shape {out[f'{name}_init'].shape}, the prior {shape}")
-        else:
-            raise TypeError(f"model.{name}: expected DirichletCollection or PointMass, got {type(v).__name__}")
-        if len(shape) != 2 or shape[1] != K or (name == "A" and shape[0] != K):
-            raise ValueError(f"model.{name} has shape {shape}; with K = {K} states A is K x K and B is M x K")
-    return out
+    K = p0.shape[0]
+    return {"p0": p0, **_matrix_arguments(model, "A", init, K), **_matrix_arguments(model, "B", init, K)}
 
 
 @dataclass
@@ -346,53 +373,21 @@ class gaussian_hidden_markov_model:
     w_prior: list
 
 
-class GaussianHMMConstraints:
+class GaussianHMMConstraints(_Marker):
     """``q(s_0, s, A, m, w) = q(s_0, s) q(A) q(m[1]) ... q(m[K]) q(w[1]) ... q(w[K])``: the chain kept structured, the
     transition matrix and every state's mean and precision apart."""
-
-    def __eq__(self, other):
-        return isinstance(other, GaussianHMMConstraints)
-
-    def __hash__(self):
-        return hash(GaussianHMMConstraints)
 
 
 def gaussian_hmm_arguments(model, initialization):
     """The keyword arguments of ``Context.hmm_gauss_vmp`` for ``model`` and ``initialization``: p0[K], the A arguments of
     ``hmm_arguments`` and the emission arrays of ``gaussian_mixture_arrays`` (mu0[K, d], V0[K, d, d], nu0[K], S0[K, d, d]
     and the same for the initial q(m), q(w))."""
-    p0 = np.asarray(model.p0.p if isinstance(model.p0, Categorical) else model.p0, np.float64).reshape(-1)
-    K = p0.shape[0]
+    p0 = _p0(model)
     init = initialization or {}
     if not {"m", "w"} <= set(init):
         raise ValueError("gaussian_hidden_markov_model needs initialization = {'m': [q(m[k])], 'w': [q(w[k])]} (and 'A' "
                          "when A is learned)")
-    out = {"p0": p0}
-    if isinstance(model.A, PointMass):
-        out["A_known"] = np.asarray(model.A.value, np.float64)
-        shape = out["A_known"].shape
-    elif isinstance(model.A, DirichletCollection):
-        if not isinstance(init.get("A"), DirichletCollection):
-            raise ValueError(f"A is learned: pass initialization = {{'A': DirichletCollection(...)}}, e.g. "
-                             f"vague(DirichletCollection, {np.asarray(model.A.alpha).shape})")
-        out["A_prior"] = np.asarray(model.A.alpha, np.float64)
-        out["A_init"] = np.asarray(init["A"].alpha, np.float64)
-        shape = out["A_prior"].shape
-        if out["A_init"].shape != shape:
-            raise ValueError(f"initialization['A'] has shape {out['A_init'].shape}, the prior {shape}")
-    else:
-        raise TypeError(f"model.A: expected DirichletCollection or PointMass, got {type(model.A).__name__}")
-    if shape != (K, K):
-        raise ValueError(f"model.A has shape {shape}; with K = {K} states A is K x K")
-    out["mu0"], out["V0"] = _gaussians(model.m_prior, K, "m_prior")
-    out["m_init"], out["Vm_init"] = _gaussians(init["m"], K, "initialization['m']")
-    out["nu0"], out["S0"] = _precisions(model.w_prior, K, "w_prior")
-    out["nu_init"], out["S_init"] = _precisions(init["w"], K, "initialization['w']")
-    d = out["mu0"].shape[1]
-    for k in ("m_init", "V0", "Vm_init", "S0", "S_init"):
-        if out[k].shape[1] != d:
-            raise ValueError(f"{k}: dimension {out[k].shape[1]}, the means have d = {d}")
-    return out
+    return {"p0": p0, **_matrix_arguments(model, "A", init, p0.shape[0]), **_emission_arrays(model, init, p0.shape[0])}
 
 
 @dataclass
@@ -430,30 +425,12 @@ def vec_order(d):
     return np.array([(r % d) * d + r // d for r in range(d * d)])
 
 
-class KeepLast:
+class KeepLast(_Marker):
     """``predictvars`` / ``returnvars`` marker: keep the result of the last iteration (the reference's ``KeepLast()``)."""
 
-    def __eq__(self, other):
-        return isinstance(other, KeepLast)
 
-    def __hash__(self):
-        return hash(KeepLast)
-
-    def __repr__(self):
-        return "KeepLast()"
-
-
-class KeepEach:
+class KeepEach(_Marker):
     """``KeepEach()``: keep the result of every iteration.  Predictions per iteration are outside the batched hot path."""
-
-    def __eq__(self, other):
-        return isinstance(other, KeepEach)
-
-    def __hash__(self):
-        return hash(KeepEach)
-
-    def __repr__(self):
-        return "KeepEach()"
 
 
 @dataclass
@@ -551,73 +528,69 @@ def _noise_posteriors(r):
             if r[f"df_{name}"] is not None}
 
 
-def _infer_hmm(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars, context,
-               catch_exception):
+def _kept_each(who, returnvars, names, each=None, bare_each=True, by_name=True):
+    """The variables of ``names`` that ``returnvars`` keeps for every iteration.  ``returnvars`` is None or KeepLast()
+    (every variable, last iteration only), KeepEach() (every variable of ``each``, by default all of ``names``; refused
+    unless ``bare_each``) or, with ``by_name``, a dict of KeepLast() / KeepEach() by variable, KeepEach() only for
+    ``each``.  Every other form raises ``NotImplementedError``."""
+    each = set(names if each is None else each)
+    if isinstance(returnvars, dict) and by_name:
+        if set(returnvars) - set(names) or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
+            raise NotImplementedError(f"returnvars={returnvars!r}: KeepLast() of {', '.join(names)}; KeepEach() of "
+                                      f"{', '.join(n for n in names if n in each)}")
+        kept = {k for k, v in returnvars.items() if isinstance(v, KeepEach)}
+        if kept - each:
+            last = sorted(kept - each)
+            raise NotImplementedError(f"returnvars: {', '.join(f'q({k})' for k in last)} kept for the last iteration "
+                                      "only (KeepLast)")
+        return kept
+    if returnvars is None or isinstance(returnvars, KeepLast):
+        return set()
+    if bare_each and isinstance(returnvars, KeepEach):
+        return each
+    forms = ["KeepLast()"] + ["KeepEach()"] * bare_each + [f"a dict over {', '.join(names)}"] * by_name
+    raise NotImplementedError(f"returnvars={returnvars!r}: {who} returns {' or '.join(forms)}")
+
+
+# --------------------------------------------------------------------------- handlers of infer()
+# Every handler takes the model and the keywords of ``infer`` (each keeps the ones it uses) and runs the refusals of its
+# model; they raise.  It returns a streaming engine, or ``run(ctx)``, the device work, which ``infer`` runs under the
+# ``catch_exception`` guard.
+def _infer_hmm(model, *, data, initialization, iterations, free_energy, returnvars, **_):
     """``infer`` of ``hidden_markov_model``: one ``rxg_hmm_vmp_f32`` launch.  ``returnvars`` is KeepLast() / KeepEach() for
     every variable or a dict over ``s``, ``A``, ``B``; ``s_0`` is the last iteration's."""
-    check_hmm_constraints(constraints)
-    if predictvars is not None:
-        raise NotImplementedError("predictvars: predictions of the hidden Markov model are outside the batched hot path")
     if data is None or "x" not in data:
         raise KeyError("hidden_markov_model needs data = {'x': observations}")
-    if isinstance(returnvars, dict):
-        bad = set(returnvars) - {"s", "A", "B", "s_0"}
-        if bad or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
-            raise NotImplementedError(f"returnvars={returnvars!r}: KeepEach() / KeepLast() of s, A, B (and KeepLast() of s_0)")
-        each = {k for k, v in returnvars.items() if isinstance(v, KeepEach)}
-        if "s_0" in each:
-            raise NotImplementedError("returnvars: q(s_0) is kept for the last iteration only (KeepLast)")
-    elif returnvars is None or isinstance(returnvars, (KeepEach, KeepLast)):
-        each = {"s", "A", "B"} if isinstance(returnvars, KeepEach) else set()
-    else:
-        raise NotImplementedError(f"returnvars={returnvars!r}: the hidden Markov model returns KeepEach() or KeepLast()")
+    each = _kept_each("hidden_markov_model", returnvars, ("s", "A", "B", "s_0"), each=("s", "A", "B"))
     args = hmm_arguments(model, initialization)
     M = (args["B_known"] if "B_known" in args else args["B_prior"]).shape[0]
     x = hmm_symbols(torch.as_tensor(data["x"]), M)
-    try:
-        ctx = context or default_context()
-        x = x.to(f"cuda:{ctx.device}").contiguous()
-        r = ctx.hmm_vmp(x, **args, iterations=iterations or 1, want_free_energy=bool(free_energy), keep_each=bool(each))
+
+    def run(ctx):
+        r = ctx.hmm_vmp(x.to(f"cuda:{ctx.device}").contiguous(), **args, iterations=iterations or 1,
+                        want_free_energy=bool(free_energy), keep_each=bool(each))
         _raise_flagged(r["status"], "hidden_markov_model: ", " (BAD_ARG: a symbol >= M; NAN: data impossible under the model)")
         post = {"s": Categorical(r["hist_s"] if "s" in each else r["s_prob"]), "s_0": Categorical(r["s0_prob"])}
         for name in ("A", "B"):
             if r[f"{name}_alpha"] is not None:
                 post[name] = DirichletCollection(r[f"hist_{name}"] if name in each else r[f"{name}_alpha"])
         return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
-    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
-        if catch_exception:
-            return InferenceResult(posteriors={}, model=model, error=e)
-        raise
+    return run
 
 
-def _infer_hmm_gauss(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars, datastream,
-                     context, catch_exception):
-    """``infer`` of ``gaussian_hidden_markov_model``: one ``rxg_hmm_gauss_vmp_f32`` launch.  ``returnvars`` is KeepLast() /
-    KeepEach() for every variable or a dict over ``s``, ``A``, ``m``, ``w`` (and KeepLast() of ``s_0``)."""
+def _check_gaussian_hmm_constraints(constraints):
     if not isinstance(constraints, GaussianHMMConstraints):
         raise ValueError("gaussian_hidden_markov_model runs the structured factorisation q(s_0, s) q(A) q(m[1]) ... q(m[K]) "
                          f"q(w[1]) ... q(w[K]) only; pass constraints = GaussianHMMConstraints() (got {constraints!r})")
-    if predictvars is not None:
-        raise NotImplementedError("predictvars: predictions of the Gaussian hidden Markov model are outside the batched "
-                                  "hot path")
-    if datastream is not None or data is None:
-        raise NotImplementedError("gaussian_hidden_markov_model runs over whole series: pass data = {'y': [T, d, batch]} "
-                                  "(no datastream)")
+
+
+def _infer_hmm_gauss(model, *, data, initialization, iterations, free_energy, returnvars, **_):
+    """``infer`` of ``gaussian_hidden_markov_model``: one ``rxg_hmm_gauss_vmp_f32`` launch.  ``returnvars`` is
+    KeepLast() / KeepEach() for every variable or a dict over ``s``, ``A``, ``m``, ``w`` (and KeepLast() of ``s_0``)."""
     if "y" not in data:
         raise KeyError("gaussian_hidden_markov_model needs data = {'y': observations}")
-    if isinstance(returnvars, dict):
-        bad = set(returnvars) - {"s", "A", "m", "w", "s_0"}
-        if bad or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
-            raise NotImplementedError(f"returnvars={returnvars!r}: KeepEach() / KeepLast() of s, A, m, w (and KeepLast() "
-                                      "of s_0)")
-        each = {k for k, v in returnvars.items() if isinstance(v, KeepEach)}
-        if "s_0" in each:
-            raise NotImplementedError("returnvars: q(s_0) is kept for the last iteration only (KeepLast)")
-    elif returnvars is None or isinstance(returnvars, (KeepEach, KeepLast)):
-        each = {"s", "A", "m", "w"} if isinstance(returnvars, KeepEach) else set()
-    else:
-        raise NotImplementedError(f"returnvars={returnvars!r}: the Gaussian hidden Markov model returns KeepEach() or "
-                                  "KeepLast()")
+    each = _kept_each("gaussian_hidden_markov_model", returnvars, ("s", "A", "m", "w", "s_0"),
+                      each=("s", "A", "m", "w"))
     args = gaussian_hmm_arguments(model, initialization)
     d = args["mu0"].shape[1]
     y = torch.as_tensor(data["y"])
@@ -625,32 +598,19 @@ def _infer_hmm_gauss(model, data, constraints, initialization, iterations, free_
     if y.dim() != 3 or y.shape[1] != d:
         raise ValueError(f"data['y'] must be [T, d = {d}, batch] (or [T, batch] at d = 1), got {tuple(y.shape)}")
     univariate = isinstance(model.m_prior[0], NormalMeanVariance) and isinstance(model.w_prior[0], GammaShapeRate)
-    try:
-        ctx = context or default_context()
-        y = y.to(device=f"cuda:{ctx.device}", dtype=torch.float32).contiguous()
-        r = ctx.hmm_gauss_vmp(y, **args, iterations=iterations or 1, want_free_energy=bool(free_energy),
-                              keep_each=bool(each))
+
+    def run(ctx):
+        r = ctx.hmm_gauss_vmp(y.to(device=f"cuda:{ctx.device}", dtype=torch.float32).contiguous(), **args,
+                              iterations=iterations or 1, want_free_energy=bool(free_energy), keep_each=bool(each))
         _raise_flagged(r["status"], "gaussian_hidden_markov_model: ",
                        " (BAD_ARG: a non-finite datum other than an all-NaN step; NAN: a vanished normaliser; NOT_SPD: "
                        "an update met a non-SPD matrix)")
         post = {"s": Categorical(r["hist_s"] if "s" in each else r["s_prob"]), "s_0": Categorical(r["s0_prob"])}
         if r["A_alpha"] is not None:
             post["A"] = DirichletCollection(r["hist_A"] if "A" in each else r["A_alpha"])
-        mp = "hist_" if "m" in each else ""                      # KeepEach: a leading iteration axis
-        wp = "hist_" if "w" in each else ""
-        mm, mc, df, iS = r[mp + "m_mean"], r[mp + "m_cov"], r[wp + "w_df"], r[wp + "w_inv_scale"]
-        K = mm.shape[-3]
-        if univariate:
-            post["m"] = [NormalMeanVariance(mm[..., k, 0, :], mc[..., k, 0, 0, :]) for k in range(K)]
-            post["w"] = [GammaShapeRate(df[..., k, :] / 2, iS[..., k, 0, 0, :] / 2) for k in range(K)]
-        else:
-            post["m"] = [MvNormalMeanCovariance(mm[..., k, :, :], mc[..., k, :, :, :]) for k in range(K)]
-            post["w"] = [WishartFast(df[..., k, :], iS[..., k, :, :, :]) for k in range(K)]
+        post["m"], post["w"] = _component_posteriors(r, each, univariate)
         return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
-    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
-        if catch_exception:
-            return InferenceResult(posteriors={}, model=model, error=e)
-        raise
+    return run
 
 
 @dataclass
@@ -664,15 +624,9 @@ class binomial_regression:
     prior_precision: object
 
 
-def _infer_binomial(model, data, initialization, iterations, free_energy, returnvars, predictvars, datastream, context,
-                    catch_exception):
+def _infer_binomial(model, *, data, initialization, iterations, free_energy, returnvars, **_):
     """``infer`` of ``binomial_regression``: one ``rxg_binomial_polya_vmp_f32`` launch.  ``returnvars`` is KeepLast() /
     KeepEach() of ``β``; ``free_energy=True`` gives F after every iteration."""
-    if predictvars is not None:
-        raise NotImplementedError("predictvars: predictions of y are outside the batched hot path")
-    if datastream is not None or data is None:
-        raise NotImplementedError("binomial_regression runs over whole data sets: pass data = {'X', 'y', 'n_trials'} "
-                                  "(no datastream)")
     if initialization is not None:
         raise NotImplementedError("binomial_regression starts from the prior: initialization is not used")
     if "X" not in data or "y" not in data:
@@ -680,14 +634,7 @@ def _infer_binomial(model, data, initialization, iterations, free_energy, return
     bad = set(data) - {"X", "y", "n_trials"}
     if bad:
         raise ValueError(f"binomial_regression: unknown data {sorted(bad)} (X, y, n_trials)")
-    if isinstance(returnvars, dict):
-        if set(returnvars) - {"β"} or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
-            raise NotImplementedError(f"returnvars={returnvars!r}: KeepEach() / KeepLast() of β")
-        each = isinstance(returnvars.get("β"), KeepEach)
-    elif returnvars is None or isinstance(returnvars, (KeepEach, KeepLast)):
-        each = isinstance(returnvars, KeepEach)
-    else:
-        raise NotImplementedError(f"returnvars={returnvars!r}: binomial_regression returns KeepEach() or KeepLast() of β")
+    each = bool(_kept_each("binomial_regression", returnvars, ("β",)))
     X = torch.as_tensor(data["X"])
     single = X.dim() == 2
     X = X[None] if single else X
@@ -706,8 +653,8 @@ def _infer_binomial(model, data, initialization, iterations, free_energy, return
 
     y = counts("y")
     n = counts("n_trials") if data.get("n_trials") is not None else None
-    try:
-        ctx = context or default_context()
+
+    def run(ctx):
         dev = f"cuda:{ctx.device}"
         r = ctx.binomial_polya_vmp(X.to(device=dev, dtype=torch.float32).permute(1, 2, 0).contiguous(),
                                    y.to(dev).T.contiguous(), model.prior_xi, model.prior_precision,
@@ -720,10 +667,7 @@ def _infer_binomial(model, data, initialization, iterations, free_energy, return
         if single:
             mean, cov, fe = mean[..., 0], cov[..., 0], (fe[:, 0] if fe is not None else None)
         return InferenceResult(posteriors={"β": MvNormalMeanCovariance(mean, cov)}, model=model, free_energy=fe)
-    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
-        if catch_exception:
-            return InferenceResult(posteriors={}, model=model, error=e)
-        raise
+    return run
 
 
 @dataclass
@@ -744,17 +688,6 @@ class multinomial_regression_online:
     chunks are int32 counts [Tc, K, batch]; ``data = {"y": [batch, T, K]}`` (or [T, K]) gives a completed engine."""
 
 
-def _returns_each(returnvars, name, who):
-    """KeepEach() / KeepLast() of one variable, bare or as {name: ...}: True for KeepEach."""
-    if isinstance(returnvars, dict):
-        if set(returnvars) - {name} or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
-            raise NotImplementedError(f"returnvars={returnvars!r}: KeepEach() / KeepLast() of {name}")
-        return isinstance(returnvars.get(name), KeepEach)
-    if returnvars is None or isinstance(returnvars, (KeepEach, KeepLast)):
-        return isinstance(returnvars, KeepEach)
-    raise NotImplementedError(f"returnvars={returnvars!r}: {who} returns KeepEach() or KeepLast() of {name}")
-
-
 def _counts(v, what):
     """Whole-number counts as an int32 tensor; a float array must hold whole numbers."""
     v = torch.as_tensor(v)
@@ -766,15 +699,9 @@ def _counts(v, what):
     return v.to(torch.int32)
 
 
-def _infer_multinomial(model, data, initialization, iterations, free_energy, returnvars, predictvars, datastream,
-                       context, catch_exception):
+def _infer_multinomial(model, *, data, initialization, iterations, free_energy, returnvars, **_):
     """``infer`` of ``multinomial_regression``: one ``rxg_multinomial_polya_vmp_f32`` call.  ``returnvars`` is
     KeepLast() / KeepEach() of ``ψ``; ``free_energy=True`` gives F after every iteration."""
-    if predictvars is not None:
-        raise NotImplementedError("predictvars: predictions of y are outside the batched hot path")
-    if datastream is not None or data is None:
-        raise NotImplementedError("multinomial_regression runs over whole data sets: pass data = {'y'} (the online form "
-                                  "is multinomial_regression_online)")
     if initialization is not None:
         raise NotImplementedError("multinomial_regression starts from the prior: initialization is not used")
     if "y" not in data:
@@ -782,14 +709,14 @@ def _infer_multinomial(model, data, initialization, iterations, free_energy, ret
     bad = set(data) - {"y"}
     if bad:
         raise ValueError(f"multinomial_regression: unknown data {sorted(bad)} (y)")
-    each = _returns_each(returnvars, "ψ", "multinomial_regression")
+    each = bool(_kept_each("multinomial_regression", returnvars, ("ψ",)))
     y = _counts(data["y"], "data['y']")
     single = y.dim() == 2
     y = y[None] if single else y
     if y.dim() != 3:
         raise ValueError(f"data['y'] must be [batch, n, K] (or [n, K]), got {tuple(y.shape)}")
-    try:
-        ctx = context or default_context()
+
+    def run(ctx):
         r = ctx.multinomial_polya_vmp(y.to(f"cuda:{ctx.device}").permute(1, 2, 0).contiguous(), model.prior_xi,
                                       model.prior_precision, iterations=iterations or 1,
                                       want_free_energy=bool(free_energy), keep_each=each)
@@ -800,14 +727,11 @@ def _infer_multinomial(model, data, initialization, iterations, free_energy, ret
         if single:
             mean, cov, fe = mean[..., 0], cov[..., 0], (fe[:, 0] if fe is not None else None)
         return InferenceResult(posteriors={"ψ": MvNormalMeanCovariance(mean, cov)}, model=model, free_energy=fe)
-    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
-        if catch_exception:
-            return InferenceResult(posteriors={}, model=model, error=e)
-        raise
+    return run
 
 
-def _infer_multinomial_online(model, data, initialization, autoupdates, iterations, free_energy, returnvars, predictvars,
-                              keephistory, historyvars, datastream, autostart, batch, context):
+def _infer_multinomial_online(model, *, data, initialization, autoupdates, iterations, free_energy, returnvars,
+                              predictvars, keephistory, historyvars, datastream, autostart, batch, context, **_):
     """``infer`` of ``multinomial_regression_online``: an ``RxInferenceEngine`` of kind "multinomial" (the carry q(ψ) in
     fp64 on the device).  With ``data`` the whole stream is one chunk and the engine is returned completed."""
     if predictvars is not None or returnvars is not None:
@@ -839,35 +763,23 @@ def _infer_multinomial_online(model, data, initialization, autoupdates, iteratio
                              initialization=init)
 
 
-def _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
-                       datastream, context, catch_exception):
+def _check_hgf_offline_constraints(constraints):
+    if not isinstance(constraints, MeanField):
+        raise ValueError(f"hgf_offline runs the naive mean-field factorisation only; pass constraints = MeanField() "
+                         f"(got {constraints!r})")
+
+
+def _infer_hgf_offline(model, *, data, initialization, iterations, free_energy, returnvars, **_):
     """``infer`` of ``hgf_offline``: one ``rxg_hgf_vmp_learn_f32`` launch.  ``returnvars``: KeepLast() for x, z (and x_0),
     KeepEach() or KeepLast() for κ, ω.  A chain whose GH products collapse (DESIGN 3.19) is flagged RXG_ERR_NAN in
     ``result.status[batch]`` and its posteriors are not meaningful; the call does not raise for it, since at large batches
     a few such chains are expected and the others' results stand."""
-    if not isinstance(constraints, MeanField):
-        raise ValueError(f"hgf_offline runs the naive mean-field factorisation only; pass constraints = MeanField() "
-                         f"(got {constraints!r})")
-    if predictvars is not None:
-        raise NotImplementedError("predictvars: predictions of the HGF are outside the batched hot path")
-    if datastream is not None or data is None:
-        raise NotImplementedError("hgf_offline runs over whole series: pass data = {'y': [T, batch]} (no datastream)")
     if "y" not in data:
         raise KeyError("hgf_offline needs data = {'y': observations}")
-    if isinstance(returnvars, dict):
-        bad = set(returnvars) - {"x", "z", "x_0", "κ", "ω"}
-        if bad or not all(isinstance(v, (KeepEach, KeepLast)) for v in returnvars.values()):
-            raise NotImplementedError(f"returnvars={returnvars!r}: KeepLast() of x, z, x_0 and KeepEach() / KeepLast() of κ, ω")
-        each = {k for k, v in returnvars.items() if isinstance(v, KeepEach)}
-        if each - {"κ", "ω"}:
-            raise NotImplementedError("returnvars: q(x), q(z), q(x_0) are kept for the last iteration only (KeepLast)")
-    elif returnvars is None or isinstance(returnvars, KeepLast):
-        each = set()
-    else:
-        raise NotImplementedError(f"returnvars={returnvars!r}: pass KeepLast() or a dict with KeepEach() for κ, ω only")
+    each = _kept_each("hgf_offline", returnvars, ("x", "z", "x_0", "κ", "ω"), each=("κ", "ω"), bare_each=False)
     args = hgf_offline_arguments(model, initialization)
-    try:
-        ctx = context or default_context()
+
+    def run(ctx):
         y = torch.as_tensor(data["y"]).to(device=f"cuda:{ctx.device}", dtype=torch.float32).contiguous()
         if y.dim() != 2:
             raise ValueError(f"data['y'] must be [T, batch], got {tuple(y.shape)}")
@@ -879,10 +791,274 @@ def _infer_hgf_offline(model, data, constraints, initialization, iterations, fre
             q = r["hist_kw"] if name in each else r["kw"]     # KeepEach: a leading iteration axis
             post[name] = NormalMeanVariance(q[..., i, 0, :], q[..., i, 1, :])
         return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"], status=r["status"])
-    except Exception as e:           # reference: catch_exception=true returns a partial result with .error
-        if catch_exception:
-            return InferenceResult(posteriors={}, model=model, error=e)
-        raise
+    return run
+
+
+_WISHART_LGSSMS = (linear_gaussian_ssm_wishart_precision, linear_gaussian_ssm_wishart_noise,
+                   linear_gaussian_ssm_continuous_transition)
+
+
+def _series(run):
+    """The handler of a model observed as ``data['y']``, or through a streaming engine when there is no ``data``: the
+    checks these models share, then ``run(model, ctx, y, mask=..., inputs=..., predict=..., horizon=..., **keywords)``
+    under the guard."""
+    def handler(model, **kw):
+        data = kw["data"]
+        if isinstance(model, _WISHART_LGSSMS):
+            if data is not None and "u" in data:
+                raise NotImplementedError("data['u']: input sequences on the Wishart-precision LGSSM are outside the "
+                                          "batched hot path (a constant offset is model.u)")
+            if isinstance(kw["returnvars"], dict) and isinstance(kw["returnvars"].get("x"), KeepEach):
+                raise NotImplementedError("returnvars: q(x) is kept for the last iteration only (KeepLast) on the "
+                                          "batched path")
+            if data is None:
+                raise ValueError("the Wishart-precision LGSSM needs `data` (it has no streaming form)")
+        horizon = getattr(model, "horizon", 0) if isinstance(model, linear_gaussian_ssm_smoothing) else 0
+        if isinstance(model, linear_gaussian_ssm_filtering) and horizon:
+            raise NotImplementedError("horizon > 0 belongs to the smoothing LGSSM")
+        predict = None
+        if kw["predictvars"] is not None or horizon > 0:
+            predict = _predict_keys(kw["predictvars"] if kw["predictvars"] is not None else {}, model, data)
+        if data is None:
+            if kw["datastream"] is None and kw["autoupdates"] is None:
+                raise ValueError("either `data` or `datastream` (or `autoupdates` for a push-driven engine) is "
+                                 "required")
+            if kw["batch"] is None:
+                raise ValueError("streaming inference needs `batch` (number of lock-step datastreams)")
+            from .streaming import RxInferenceEngine
+            return RxInferenceEngine(kw["context"] or default_context(), model, batch=kw["batch"],
+                                     iterations=kw["iterations"], keephistory=kw["keephistory"],
+                                     historyvars=kw["historyvars"], free_energy=kw["free_energy"],
+                                     datastream=kw["datastream"], autostart=kw["autostart"],
+                                     cov_shared_out=kw["cov_shared_out"])
+        if "y" not in data:
+            raise KeyError("data must contain the observations under key 'y'")   # reference: missing data key error
+        y = data["y"]
+        # known per-step inputs x[t] ~ A x[t-1] + u[t]: data["u"] is a host [T(+H), d] sequence shared by every chain or
+        # a CUDA [T(+H), d, batch] tensor (one sequence per chain)
+        inputs = data.get("u")
+        if inputs is not None and getattr(model, "u", None) is not None:
+            raise ValueError("the model has a constant offset u and data carries an input sequence 'u': fold the "
+                             "constant into the sequence")
+        if inputs is not None and not isinstance(model, linear_gaussian_ssm_smoothing):
+            raise NotImplementedError(f"data['u']: input sequences belong to the LGSSM, not {type(model).__name__}")
+        if inputs is not None and horizon > 0 and inputs.shape[0] != y.shape[0] + horizon:
+            raise ValueError(f"data['u'] needs T + horizon = {y.shape[0] + horizon} rows (the forecasts use the inputs "
+                             f"of the forecast steps), got {inputs.shape[0]}")
+        return lambda ctx: run(model, ctx, y, mask=data.get("ymask"), inputs=inputs, predict=predict, horizon=horizon,
+                               **kw)
+    return handler
+
+
+@_series
+def _infer_lgssm_filtering(model, ctx, y, *, mask, inputs, free_energy, cov_shared_out, **_):
+    r = ctx.lgssm(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], u=model.u, inputs=inputs,
+                  smooth=False, mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain,
+                  transition_first=True, cov_shared_out=cov_shared_out)
+    q = MvNormalMeanCovariance(r["mean"], r["cov"])
+    return InferenceResult(posteriors={}, history={"x_t": q}, free_energy=r["neg_log_evidence"], model=model)
+
+
+@_series
+def _infer_lgssm_smoothing(model, ctx, y, *, mask, inputs, predict, horizon, iterations, free_energy, cov_shared_out,
+                           **_):
+    if iterations not in (None, 1):
+        raise NotImplementedError("iterations > 1 on a tree-structured BP model is a no-op in the reference; "
+                                  "KeepEach() results are outside the hot path")
+    if predict is not None:
+        r = ctx.lgssm_predict(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], horizon=horizon,
+                              u=model.u, inputs=inputs, mask=mask, want_evidence=free_energy,
+                              per_chain_model=model.per_chain, cov_shared_out=cov_shared_out,
+                              transition_first=model.prior_on_previous_state, want_status=True)
+        # e.g. a chain whose D_t = Q - B S_s B' is not SPD has no usable prediction
+        _raise_flagged(r["status"], "predictions: ", " (NOT_SPD: Q - B S_s B' is not SPD, the observations dominate "
+                                                     "beyond the fp32 posterior covariances)")
+        T = y.shape[0]
+        mean, cov = r["mean"], r["cov"]
+        if horizon > 0:          # posteriors["x"] covers x[1..T+H], as model_1's x covers n + 2 states
+            mean, cov = torch.cat([mean, r["fc_mean"]]), torch.cat([cov, r["fc_cov"]])
+        preds = {}
+        if "y" in predict:
+            preds["y"] = MvNormalMeanCovariance(r["pred_mean"][:T], r["pred_cov"][:T])
+        if "o" in predict:
+            preds["o"] = MvNormalMeanCovariance(r["pred_mean"][T:], r["pred_cov"][T:])
+        return InferenceResult(posteriors={"x": MvNormalMeanCovariance(mean, cov)}, predictions=preds,
+                               free_energy=r["neg_log_evidence"], model=model)
+    r = ctx.lgssm(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], u=model.u, inputs=inputs,
+                  smooth=True, mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain,
+                  cov_shared_out=cov_shared_out, transition_first=model.prior_on_previous_state)
+    return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"])},
+                           free_energy=r["neg_log_evidence"], model=model)
+
+
+@_series
+def _infer_hgf(model, ctx, y, *, iterations, free_energy, **_):
+    out = ctx.hgf_filter(y, iters=iterations or 1, kappa=model.real_k, omega=model.real_w,
+                         z_variance=model.z_variance, y_variance=model.y_variance, init=model.init,
+                         want_free_energy=bool(free_energy))
+    fe = None
+    if free_energy:      # free_energy_history of the streaming engine: average over the data, per iteration
+        out, fe_all = out
+        fe = fe_all.mean(dim=0)
+    return InferenceResult(posteriors={}, model=model, free_energy=fe,
+                           history={"xt": NormalMeanVariance(out[:, 0], out[:, 1]),
+                                    "zt": NormalMeanVariance(out[:, 2], out[:, 3])})
+
+
+@_series
+def _infer_kalman_gamma(model, ctx, y, *, iterations, free_energy, **_):
+    out, fe = ctx.stream_vmp_gamma(y, iters=iterations or 1, w=model.transition_precision, init=model.init,
+                                   want_free_energy=bool(free_energy))
+    return InferenceResult(posteriors={}, model=model, free_energy=None if fe is None else fe.mean(dim=0),
+                           history={"x_t": NormalMeanVariance(out[:, 0], out[:, 1]),
+                                    "τ": GammaShapeRate(out[:, 2], out[:, 3])})
+
+
+@_series
+def _infer_lgssm_gamma(model, ctx, y, *, iterations, free_energy, **_):
+    r = ctx.lgssm_vmp_gamma(y, iterations=iterations or 1, a=model.a, v_proc=model.v_proc, prior=model.x0,
+                            gamma_prior=model.gamma_prior, init_E_tau=model.init_E_tau,
+                            want_free_energy=bool(free_energy))
+    return InferenceResult(posteriors={"x": NormalMeanVariance(r["mean"], r["var"]),
+                                       "τ": GammaShapeRate(r["shape"], r["rate"])}, model=model,
+                           free_energy=r["free_energy"])
+
+
+@_series
+def _infer_wishart_precision(model, ctx, y, *, mask, iterations, free_energy, **_):
+    r = ctx.lgssm_vmp_wishart(y, model.A, model.B, model.P, model.x0[0], model.x0[1], iterations=iterations or 1,
+                              w_prior=(model.w_prior.df, model.w_prior.inv_scale()), init_E_W=model.w_init.mean(),
+                              u=model.u, mask=mask, transition_first=model.prior_on_previous_state,
+                              want_free_energy=bool(free_energy))
+    _raise_flagged(r["status"])
+    # returnvars of the reference's call under `iterations`: x = KeepLast() here, w = KeepEach() (iteration axis)
+    return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]),
+                                       "w": WishartFast(r["df"], r["inv_scale"])},
+                           model=model, free_energy=r["free_energy"])
+
+
+@_series
+def _infer_wishart_noise(model, ctx, y, *, mask, iterations, free_energy, **_):
+    r = ctx.lgssm_vmp_noise(y, model.A, model.B, model.x0[0], model.x0[1], **_noise_kwargs(model), u=model.u,
+                            mask=mask, transition_first=model.prior_on_previous_state,
+                            iterations=iterations or 1, want_free_energy=bool(free_energy))
+    _raise_flagged(r["status"])
+    # x = KeepLast(), w_p / w_q = KeepEach() (leading iteration axis) for the learned precisions
+    return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]), **_noise_posteriors(r)},
+                           model=model, free_energy=r["free_energy"])
+
+
+@_series
+def _infer_continuous_transition(model, ctx, y, *, mask, iterations, free_energy, **_):
+    kw = _noise_kwargs(model)
+    if model.a_init is None:
+        raise ValueError("a_init: q(a) needs an initial (mean, covariance) (an uninformed q(a) makes the first "
+                         "sweep meaningless)")
+    d = np.asarray(model.x0[1]).shape[-1]
+    pm = vec_order(d)
+    rowmajor = lambda mc: (np.asarray(mc[0], np.float64).reshape(-1)[pm],
+                           np.asarray(mc[1], np.float64)[np.ix_(pm, pm)])
+    r = ctx.lgssm_vmp_transition(y, model.B, model.x0[0], model.x0[1], a_prior=rowmajor(model.a_prior),
+                                 a_init=rowmajor(model.a_init), **kw, u=model.u, mask=mask,
+                                 transition_first=model.prior_on_previous_state, iterations=iterations or 1,
+                                 want_free_energy=bool(free_energy))
+    _raise_flagged(r["status"])
+    # x = KeepLast(); a, w_p / w_q = KeepEach() (leading iteration axis); a over vec(A) in column-major order
+    pt = torch.as_tensor(pm, device=r["a_mean"].device)
+    its_, nb = r["a_mean"].shape[0], r["a_mean"].shape[-1]
+    a_mu = r["a_mean"].reshape(its_, d * d, nb)[:, pt]
+    a_S = r["a_cov"][:, pt][:, :, pt]
+    return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]),
+                                       "a": MvNormalMeanCovariance(a_mu, a_S), **_noise_posteriors(r)},
+                           model=model, free_energy=r["free_energy"])
+
+
+@_series
+def _infer_mixture(model, ctx, y, *, constraints, initialization, iterations, free_energy, returnvars, **_):
+    check_mean_field(constraints)
+    each = _kept_each("gaussian_mixture", returnvars, ("s", "m", "w"), by_name=False)
+    arr = gaussian_mixture_arrays(model, initialization)
+    yy = y[:, None] if y.dim() == 2 else y          # univariate data may come as [N, batch]
+    if yy.shape[1] != arr["mu0"].shape[1]:
+        raise ValueError(f"data['y'] has d = {yy.shape[1]}, the model's means d = {arr['mu0'].shape[1]}")
+    r = ctx.gmm_vmp(yy.contiguous(), *(arr[k] for k in ("alpha0", "mu0", "V0", "nu0", "S0", "alpha_init", "m_init",
+                                                         "Vm_init", "nu_init", "S_init")),
+                    iterations=iterations or 1, want_free_energy=bool(free_energy), want_z=True, keep_each=bool(each))
+    _raise_flagged(r["status"], "gaussian_mixture: ", " (NOT_SPD: an update met a non-SPD matrix)")
+    al = r["hist_alpha" if each else "alpha"]       # KeepEach: a leading iteration axis on every posterior
+    post = {"s": Beta(al[..., 0, :], al[..., 1, :]) if arr["univariate"] else Dirichlet(al)}
+    post["m"], post["w"] = _component_posteriors(r, each, arr["univariate"])
+    post["z"] = Categorical(r["z_prob"])
+    return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
+
+
+@_series
+def _infer_lar(model, ctx, y, *, iterations, free_energy, **_):
+    yy = y[:, 0] if y.dim() == 3 else y
+    r = ctx.lar_vmp(yy.contiguous(), model.order, model.tau, iterations=iterations or 1, gamma_prior=model.gamma_prior,
+                    theta_prior_precision=model.theta_prior_precision, x0_prior_precision=model.x0_prior_precision,
+                    init_gamma=model.init_gamma, init_theta_precision=model.init_theta_precision,
+                    want_free_energy=bool(free_energy))
+    # returnvars of the reference's call: x = KeepLast(), gamma / theta = KeepEach() (leading iteration axis)
+    return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["x_mean"], r["x_cov"]),
+                                       "γ": GammaShapeRate(r["gamma_shape"], r["gamma_rate"]),
+                                       "θ": MvNormalMeanCovariance(r["theta_mean"], r["theta_cov"])},
+                           model=model, free_energy=r["free_energy"])
+
+
+@_series
+def _infer_unrecognised(model, ctx, y, **_):
+    raise NotImplementedError(f"model pattern {type(model).__name__} is not on the batched hot path")
+
+
+class _Model(NamedTuple):
+    """What ``infer`` knows of one model besides its handler: the refusals it states once for the model."""
+    handler: object
+    takes_constraints: bool = False          # `constraints` is a keyword of the model (else it is refused)
+    check_constraints: object = None         # checked before every other refusal (the mixture checks its own, guarded)
+    refuses: tuple = ()                      # streaming keywords refused with NotImplementedError
+    refusal_note: str = ""                   # appended to that refusal
+    predictions_of: str = None               # predictvars refused: "predictions of <this> are outside ..."
+    whole_data: str = None                   # datastream refused: "<model> <this>"
+    context_guarded: bool = False            # the context lookup is under the catch_exception guard
+
+
+_STREAMING = ("autoupdates", "keephistory", "historyvars", "batch", "cov_shared_out")
+_WISHART_LGSSM = "the Wishart-precision LGSSM"
+
+_MODELS = {
+    linear_gaussian_ssm_filtering: _Model(_infer_lgssm_filtering),
+    linear_gaussian_ssm_smoothing: _Model(_infer_lgssm_smoothing),
+    hgf: _Model(_infer_hgf),
+    kalman_gamma_streaming: _Model(_infer_kalman_gamma),
+    univariate_lgssm_gamma_precision: _Model(_infer_lgssm_gamma),
+    linear_gaussian_ssm_wishart_precision: _Model(_infer_wishart_precision, predictions_of=_WISHART_LGSSM),
+    linear_gaussian_ssm_wishart_noise: _Model(_infer_wishart_noise, predictions_of=_WISHART_LGSSM),
+    linear_gaussian_ssm_continuous_transition: _Model(_infer_continuous_transition, predictions_of=_WISHART_LGSSM),
+    gaussian_mixture: _Model(_infer_mixture, takes_constraints=True),
+    latent_autoregressive: _Model(_infer_lar),
+    hidden_markov_model: _Model(_infer_hmm, takes_constraints=True, check_constraints=check_hmm_constraints,
+                                predictions_of="the hidden Markov model", context_guarded=True),
+    gaussian_hidden_markov_model: _Model(_infer_hmm_gauss, takes_constraints=True,
+                                         check_constraints=_check_gaussian_hmm_constraints,
+                                         predictions_of="the Gaussian hidden Markov model",
+                                         whole_data="runs over whole series: pass data = {'y': [T, d, batch]} "
+                                                    "(no datastream)", context_guarded=True),
+    hgf_offline: _Model(_infer_hgf_offline, takes_constraints=True, check_constraints=_check_hgf_offline_constraints,
+                        predictions_of="the HGF",
+                        whole_data="runs over whole series: pass data = {'y': [T, batch]} (no datastream)",
+                        context_guarded=True),
+    binomial_regression: _Model(_infer_binomial, refuses=_STREAMING, predictions_of="y",
+                                whole_data="runs over whole data sets: pass data = {'X', 'y', 'n_trials'} "
+                                           "(no datastream)", context_guarded=True),
+    multinomial_regression: _Model(_infer_multinomial, refuses=_STREAMING,
+                                   refusal_note=" (the online form is multinomial_regression_online)",
+                                   predictions_of="y",
+                                   whole_data="runs over whole data sets: pass data = {'y'} (the online form is "
+                                              "multinomial_regression_online)", context_guarded=True),
+    multinomial_regression_online: _Model(_infer_multinomial_online, refuses=("cov_shared_out",)),
+}
+_UNRECOGNISED = _Model(_infer_unrecognised)
 
 
 def infer(*, model, iterations=None, free_energy=False, returnvars=None, options=None,
@@ -896,9 +1072,8 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
     With ``datastream=`` (an iterable of time-chunks, or ``None`` + ``autoupdates`` for a push-driven
     engine) the call returns an ``RxInferenceEngine`` (streaming.py), as the reference does when
     ``autoupdates`` is given (/root/reference/src/inference/inference.jl:577-733 dispatch)."""
-    constraints = (kwargs.pop("constraints", None) if isinstance(model, (gaussian_mixture, hidden_markov_model, hgf_offline,
-                                                                         gaussian_hidden_markov_model))
-                   else None)
+    spec = next((_MODELS[t] for t in type(model).__mro__ if t in _MODELS), _UNRECOGNISED)
+    constraints = kwargs.pop("constraints", None) if spec.takes_constraints else None
     for k in kwargs:
         if k in _UNSUPPORTED:
             raise NotImplementedError(
@@ -911,217 +1086,28 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
             raise NotImplementedError(f"options {sorted(bad)} are outside the batched hot path")
     if data is not None and datastream is not None:
         raise ValueError("`data` and `datastream` are mutually exclusive")    # reference: inference.jl argument check
-    if isinstance(model, binomial_regression):
-        if autoupdates is not None or keephistory is not None or historyvars is not None or batch is not None or cov_shared_out:
-            raise NotImplementedError("binomial_regression: autoupdates, keephistory, historyvars, batch and cov_shared_out "
-                                      "are outside the batched hot path")
-        return _infer_binomial(model, data, initialization, iterations, free_energy, returnvars, predictvars, datastream,
-                               context, catch_exception)
-    if isinstance(model, multinomial_regression):
-        if autoupdates is not None or keephistory is not None or historyvars is not None or batch is not None or cov_shared_out:
-            raise NotImplementedError("multinomial_regression: autoupdates, keephistory, historyvars, batch and "
-                                      "cov_shared_out are outside the batched hot path (the online form is "
-                                      "multinomial_regression_online)")
-        return _infer_multinomial(model, data, initialization, iterations, free_energy, returnvars, predictvars,
-                                  datastream, context, catch_exception)
-    if isinstance(model, multinomial_regression_online):
-        if cov_shared_out:
-            raise NotImplementedError("multinomial_regression_online: cov_shared_out is outside the batched hot path")
-        return _infer_multinomial_online(model, data, initialization, autoupdates, iterations, free_energy, returnvars,
-                                         predictvars, keephistory, historyvars, datastream, autostart, batch, context)
-    if isinstance(model, hgf_offline):
-        return _infer_hgf_offline(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
-                                  datastream, context, catch_exception)
-    if isinstance(model, gaussian_hidden_markov_model):
-        return _infer_hmm_gauss(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
-                                datastream, context, catch_exception)
-    if isinstance(model, hidden_markov_model):
-        return _infer_hmm(model, data, constraints, initialization, iterations, free_energy, returnvars, predictvars,
-                          context, catch_exception)
-    if isinstance(model, (linear_gaussian_ssm_wishart_precision, linear_gaussian_ssm_wishart_noise,
-                          linear_gaussian_ssm_continuous_transition)):
-        if predictvars is not None:
-            raise NotImplementedError("predictvars: predictions of the Wishart-precision LGSSM are outside the batched hot path")
-        if data is not None and "u" in data:
-            raise NotImplementedError("data['u']: input sequences on the Wishart-precision LGSSM are outside the batched hot "
-                                      "path (a constant offset is model.u)")
-        if isinstance(returnvars, dict) and isinstance(returnvars.get("x"), KeepEach):
-            raise NotImplementedError("returnvars: q(x) is kept for the last iteration only (KeepLast) on the batched path")
-        if data is None:
-            raise ValueError("the Wishart-precision LGSSM needs `data` (it has no streaming form)")
-    horizon = getattr(model, "horizon", 0) if isinstance(model, linear_gaussian_ssm_smoothing) else 0
-    if isinstance(model, linear_gaussian_ssm_filtering) and horizon:
-        raise NotImplementedError("horizon > 0 belongs to the smoothing LGSSM")
-    predict = None
-    if predictvars is not None or horizon > 0:
-        predict = _predict_keys(predictvars if predictvars is not None else {}, model, data)
-    if data is None:
-        if datastream is None and autoupdates is None:
-            raise ValueError("either `data` or `datastream` (or `autoupdates` for a push-driven engine) is required")
-        if batch is None:
-            raise ValueError("streaming inference needs `batch` (number of lock-step datastreams)")
-        from .streaming import RxInferenceEngine
-        return RxInferenceEngine(context or default_context(), model, batch=batch, iterations=iterations,
-                                 keephistory=keephistory, historyvars=historyvars, free_energy=free_energy,
-                                 datastream=datastream, autostart=autostart, cov_shared_out=cov_shared_out)
-    if "y" not in data:
-        raise KeyError("data must contain the observations under key 'y'")   # reference: missing data key error
-    y = data["y"]
-    # known per-step inputs x[t] ~ A x[t-1] + u[t]: data["u"] is a host [T(+H), d] sequence shared by every chain or a
-    # CUDA [T(+H), d, batch] tensor (one sequence per chain)
-    inputs = data.get("u")
-    if inputs is not None and getattr(model, "u", None) is not None:
-        raise ValueError("the model has a constant offset u and data carries an input sequence 'u': fold the constant "
-                         "into the sequence")
-    if inputs is not None and not isinstance(model, (linear_gaussian_ssm_smoothing, linear_gaussian_ssm_filtering)):
-        raise NotImplementedError(f"data['u']: input sequences belong to the LGSSM, not {type(model).__name__}")
-    if inputs is not None and horizon > 0 and inputs.shape[0] != y.shape[0] + horizon:
-        raise ValueError(f"data['u'] needs T + horizon = {y.shape[0] + horizon} rows (the forecasts use the inputs of "
-                         f"the forecast steps), got {inputs.shape[0]}")
-    ctx = context or default_context()
-    mask = data.get("ymask")
+    if spec.check_constraints is not None:
+        spec.check_constraints(constraints)
+    given = dict(autoupdates=autoupdates is not None, keephistory=keephistory is not None,
+                 historyvars=historyvars is not None, batch=batch is not None, cov_shared_out=bool(cov_shared_out))
+    if any(given[k] for k in spec.refuses):
+        names = " and ".join(filter(None, (", ".join(spec.refuses[:-1]), spec.refuses[-1])))
+        raise NotImplementedError(f"{type(model).__name__}: {names} {'are' if len(spec.refuses) > 1 else 'is'} outside "
+                                  f"the batched hot path{spec.refusal_note}")
+    if spec.predictions_of is not None and predictvars is not None:
+        raise NotImplementedError(f"predictvars: predictions of {spec.predictions_of} are outside the batched hot path")
+    if spec.whole_data is not None and (datastream is not None or data is None):
+        raise NotImplementedError(f"{type(model).__name__} {spec.whole_data}")
+    run = spec.handler(model, data=data, constraints=constraints, initialization=initialization, iterations=iterations,
+                       free_energy=free_energy, returnvars=returnvars, predictvars=predictvars, datastream=datastream,
+                       autoupdates=autoupdates, keephistory=keephistory, historyvars=historyvars, autostart=autostart,
+                       batch=batch, cov_shared_out=cov_shared_out, context=context)
+    if not callable(run):
+        return run                                   # a streaming engine
+    if not spec.context_guarded:
+        context = context or default_context()       # looked up before the guard, so a missing device raises
     try:
-        if isinstance(model, linear_gaussian_ssm_filtering):
-            r = ctx.lgssm(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], u=model.u, inputs=inputs,
-                          smooth=False, mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain, transition_first=True,
-                          cov_shared_out=cov_shared_out)
-            q = MvNormalMeanCovariance(r["mean"], r["cov"])
-            return InferenceResult(posteriors={}, history={"x_t": q}, free_energy=r["neg_log_evidence"], model=model)
-        if isinstance(model, linear_gaussian_ssm_smoothing):
-            if iterations not in (None, 1):
-                raise NotImplementedError("iterations > 1 on a tree-structured BP model is a no-op in the reference; "
-                                          "KeepEach() results are outside the hot path")
-            if predict is not None:
-                r = ctx.lgssm_predict(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], horizon=horizon,
-                                      u=model.u, inputs=inputs, mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain,
-                                      cov_shared_out=cov_shared_out, transition_first=model.prior_on_previous_state,
-                                      want_status=True)
-                # e.g. a chain whose D_t = Q - B S_s B' is not SPD has no usable prediction
-                _raise_flagged(r["status"], "predictions: ", " (NOT_SPD: Q - B S_s B' is not SPD, the observations dominate "
-                                                             "beyond the fp32 posterior covariances)")
-                T = y.shape[0]
-                mean, cov = r["mean"], r["cov"]
-                if horizon > 0:          # posteriors["x"] covers x[1..T+H], as model_1's x covers n + 2 states
-                    mean, cov = torch.cat([mean, r["fc_mean"]]), torch.cat([cov, r["fc_cov"]])
-                preds = {}
-                if "y" in predict:
-                    preds["y"] = MvNormalMeanCovariance(r["pred_mean"][:T], r["pred_cov"][:T])
-                if "o" in predict:
-                    preds["o"] = MvNormalMeanCovariance(r["pred_mean"][T:], r["pred_cov"][T:])
-                return InferenceResult(posteriors={"x": MvNormalMeanCovariance(mean, cov)}, predictions=preds,
-                                       free_energy=r["neg_log_evidence"], model=model)
-            r = ctx.lgssm(y, model.A, model.B, model.P, model.Q, model.x0[0], model.x0[1], u=model.u, inputs=inputs, smooth=True,
-                          mask=mask, want_evidence=free_energy, per_chain_model=model.per_chain, cov_shared_out=cov_shared_out,
-                          transition_first=model.prior_on_previous_state)
-            return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"])},
-                                   free_energy=r["neg_log_evidence"], model=model)
-        if isinstance(model, hgf):
-            out = ctx.hgf_filter(y, iters=iterations or 1, kappa=model.real_k, omega=model.real_w,
-                                 z_variance=model.z_variance, y_variance=model.y_variance, init=model.init,
-                                 want_free_energy=bool(free_energy))
-            fe = None
-            if free_energy:      # free_energy_history of the streaming engine: average over the data, per iteration
-                out, fe_all = out
-                fe = fe_all.mean(dim=0)
-            return InferenceResult(posteriors={}, model=model, free_energy=fe,
-                                   history={"xt": NormalMeanVariance(out[:, 0], out[:, 1]),
-                                            "zt": NormalMeanVariance(out[:, 2], out[:, 3])})
-        if isinstance(model, kalman_gamma_streaming):
-            out, fe = ctx.stream_vmp_gamma(y, iters=iterations or 1, w=model.transition_precision, init=model.init,
-                                           want_free_energy=bool(free_energy))
-            return InferenceResult(posteriors={}, model=model, free_energy=None if fe is None else fe.mean(dim=0),
-                                   history={"x_t": NormalMeanVariance(out[:, 0], out[:, 1]),
-                                            "τ": GammaShapeRate(out[:, 2], out[:, 3])})
-        if isinstance(model, univariate_lgssm_gamma_precision):
-            r = ctx.lgssm_vmp_gamma(y, iterations=iterations or 1, a=model.a, v_proc=model.v_proc, prior=model.x0,
-                                    gamma_prior=model.gamma_prior, init_E_tau=model.init_E_tau,
-                                    want_free_energy=bool(free_energy))
-            return InferenceResult(posteriors={"x": NormalMeanVariance(r["mean"], r["var"]),
-                                               "τ": GammaShapeRate(r["shape"], r["rate"])}, model=model,
-                                   free_energy=r["free_energy"])
-        if isinstance(model, linear_gaussian_ssm_wishart_precision):
-            r = ctx.lgssm_vmp_wishart(y, model.A, model.B, model.P, model.x0[0], model.x0[1], iterations=iterations or 1,
-                                      w_prior=(model.w_prior.df, model.w_prior.inv_scale()), init_E_W=model.w_init.mean(),
-                                      u=model.u, mask=mask, transition_first=model.prior_on_previous_state,
-                                      want_free_energy=bool(free_energy))
-            _raise_flagged(r["status"])
-            # returnvars of the reference's call under `iterations`: x = KeepLast() here, w = KeepEach() (iteration axis)
-            return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]),
-                                               "w": WishartFast(r["df"], r["inv_scale"])},
-                                   model=model, free_energy=r["free_energy"])
-        if isinstance(model, linear_gaussian_ssm_wishart_noise):
-            r = ctx.lgssm_vmp_noise(y, model.A, model.B, model.x0[0], model.x0[1], **_noise_kwargs(model), u=model.u,
-                                    mask=mask, transition_first=model.prior_on_previous_state,
-                                    iterations=iterations or 1, want_free_energy=bool(free_energy))
-            _raise_flagged(r["status"])
-            # x = KeepLast(), w_p / w_q = KeepEach() (leading iteration axis) for the learned precisions
-            return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]), **_noise_posteriors(r)},
-                                   model=model, free_energy=r["free_energy"])
-        if isinstance(model, linear_gaussian_ssm_continuous_transition):
-            kw = _noise_kwargs(model)
-            if model.a_init is None:
-                raise ValueError("a_init: q(a) needs an initial (mean, covariance) (an uninformed q(a) makes the first "
-                                 "sweep meaningless)")
-            d = np.asarray(model.x0[1]).shape[-1]
-            pm = vec_order(d)
-            rowmajor = lambda mc: (np.asarray(mc[0], np.float64).reshape(-1)[pm],
-                                   np.asarray(mc[1], np.float64)[np.ix_(pm, pm)])
-            r = ctx.lgssm_vmp_transition(y, model.B, model.x0[0], model.x0[1], a_prior=rowmajor(model.a_prior),
-                                         a_init=rowmajor(model.a_init), **kw, u=model.u, mask=mask,
-                                         transition_first=model.prior_on_previous_state, iterations=iterations or 1,
-                                         want_free_energy=bool(free_energy))
-            _raise_flagged(r["status"])
-            # x = KeepLast(); a, w_p / w_q = KeepEach() (leading iteration axis); a over vec(A) in column-major order
-            pt = torch.as_tensor(pm, device=r["a_mean"].device)
-            its_, nb = r["a_mean"].shape[0], r["a_mean"].shape[-1]
-            a_mu = r["a_mean"].reshape(its_, d * d, nb)[:, pt]
-            a_S = r["a_cov"][:, pt][:, :, pt]
-            return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"]),
-                                               "a": MvNormalMeanCovariance(a_mu, a_S), **_noise_posteriors(r)},
-                                   model=model, free_energy=r["free_energy"])
-        if isinstance(model, gaussian_mixture):
-            check_mean_field(constraints)
-            if predictvars is not None:
-                raise NotImplementedError("predictvars: predictions of the Gaussian mixture are outside the batched hot path")
-            keep_each = isinstance(returnvars, KeepEach)
-            if returnvars is not None and not isinstance(returnvars, (KeepEach, KeepLast)):
-                raise NotImplementedError(f"returnvars={returnvars!r}: the Gaussian mixture returns KeepEach() or KeepLast()")
-            arr = gaussian_mixture_arrays(model, initialization)
-            yy = y[:, None] if y.dim() == 2 else y          # univariate data may come as [N, batch]
-            if yy.shape[1] != arr["mu0"].shape[1]:
-                raise ValueError(f"data['y'] has d = {yy.shape[1]}, the model's means d = {arr['mu0'].shape[1]}")
-            r = ctx.gmm_vmp(yy.contiguous(), *(arr[k] for k in ("alpha0", "mu0", "V0", "nu0", "S0", "alpha_init", "m_init",
-                                                                 "Vm_init", "nu_init", "S_init")),
-                            iterations=iterations or 1, want_free_energy=bool(free_energy), want_z=True, keep_each=keep_each)
-            bad = r["status"] != 0
-            if bool(bad.any()):
-                raise L.RxGaussError(L.RXG_ERR_NOT_SPD, f"{int(bad.sum())} of {bad.numel()} chains flagged NOT_SPD")
-            pre = "hist_" if keep_each else ""           # KeepEach: a leading iteration axis on every posterior
-            al, mm, mc = r[pre + "alpha"], r[pre + "m_mean"], r[pre + "m_cov"]
-            df, iS = r[pre + "w_df"], r[pre + "w_inv_scale"]
-            K = int(model.K)
-            if arr["univariate"]:
-                post = {"s": Beta(al[..., 0, :], al[..., 1, :]),
-                        "m": [NormalMeanVariance(mm[..., k, 0, :], mc[..., k, 0, 0, :]) for k in range(K)],
-                        "w": [GammaShapeRate(df[..., k, :] / 2, iS[..., k, 0, 0, :] / 2) for k in range(K)]}
-            else:
-                post = {"s": Dirichlet(al),
-                        "m": [MvNormalMeanCovariance(mm[..., k, :, :], mc[..., k, :, :, :]) for k in range(K)],
-                        "w": [WishartFast(df[..., k, :], iS[..., k, :, :, :]) for k in range(K)]}
-            post["z"] = Categorical(r["z_prob"])
-            return InferenceResult(posteriors=post, model=model, free_energy=r["free_energy"])
-        if isinstance(model, latent_autoregressive):
-            yy = y[:, 0] if y.dim() == 3 else y
-            r = ctx.lar_vmp(yy.contiguous(), model.order, model.tau, iterations=iterations or 1, gamma_prior=model.gamma_prior,
-                            theta_prior_precision=model.theta_prior_precision, x0_prior_precision=model.x0_prior_precision,
-                            init_gamma=model.init_gamma, init_theta_precision=model.init_theta_precision,
-                            want_free_energy=bool(free_energy))
-            # returnvars of the reference's call: x = KeepLast(), gamma / theta = KeepEach() (leading iteration axis)
-            return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["x_mean"], r["x_cov"]),
-                                               "γ": GammaShapeRate(r["gamma_shape"], r["gamma_rate"]),
-                                               "θ": MvNormalMeanCovariance(r["theta_mean"], r["theta_cov"])},
-                                   model=model, free_energy=r["free_energy"])
-        raise NotImplementedError(f"model pattern {type(model).__name__} is not on the batched hot path")
+        return run(context or default_context())
     except Exception as e:           # reference: catch_exception=true returns a partial result with .error
         if catch_exception:
             return InferenceResult(posteriors={}, model=model, error=e)
