@@ -620,7 +620,6 @@ lgssm_block_sweep(const float* __restrict__ fwdT, const float* __restrict__ bwdT
     const int cg = tid % (NB / 2), rg = tid / (NB / 2);
     const int64_t b0 = (int64_t)blockIdx.x * NB;
     const int nb = (int)((batch - b0) < NB ? (batch - b0) : NB);
-    const bool even = (batch % 2) == 0;         // 8-byte alignment of the paired global stores
 
     auto load_W = [&](float* dst, const float* src, int K2) {
         for (int p = tid; p < K2 * D / 4; p += NT) cpa16(dst + 4 * p, src + 4 * p);
@@ -657,8 +656,8 @@ lgssm_block_sweep(const float* __restrict__ fwdT, const float* __restrict__ bwdT
             const int row = 4 * rg + r;
             *reinterpret_cast<float2*>(Zb[q ^ 1] + row * NB + 2 * cg) = make_float2(acc[r][0], acc[r][1]);
             float* g = mean + ((size_t)t * D + row) * batch + b0 + 2 * cg;
-            if (even && 2 * cg + 1 < nb) *reinterpret_cast<float2*>(g) = make_float2(acc[r][0], acc[r][1]);
-            else { if (2 * cg < nb) g[0] = acc[r][0]; if (2 * cg + 1 < nb) g[1] = acc[r][1]; }
+            if (2 * cg < nb) g[0] = acc[r][0];          // scalar stores: the caller's mean need not be 8-byte aligned
+            if (2 * cg + 1 < nb) g[1] = acc[r][1];
         }
         __syncthreads();
     }
@@ -685,8 +684,8 @@ lgssm_block_sweep(const float* __restrict__ fwdT, const float* __restrict__ bwdT
             const int row = 4 * rg + rr;
             *reinterpret_cast<float2*>(Zb[q ^ 1] + (D + row) * NB + 2 * cg) = make_float2(acc[rr][0], acc[rr][1]);
             float* g = mean + ((size_t)t * D + row) * batch + b0 + 2 * cg;
-            if (even && 2 * cg + 1 < nb) *reinterpret_cast<float2*>(g) = make_float2(acc[rr][0], acc[rr][1]);
-            else { if (2 * cg < nb) g[0] = acc[rr][0]; if (2 * cg + 1 < nb) g[1] = acc[rr][1]; }
+            if (2 * cg < nb) g[0] = acc[rr][0];
+            if (2 * cg + 1 < nb) g[1] = acc[rr][1];
         }
         __syncthreads();
     }
