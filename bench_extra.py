@@ -641,10 +641,11 @@ def main():
             del y
 
     if "stream" in which:
-        # what HBM delivers to a dependency-free streaming kernel for a given read : write mix (the sweep kernel moves
-        # 2.14 GB in and 5.25 GB out per launch, i.e. ~2 : 5)
+        # what HBM delivers to a dependency-free streaming kernel for a given read : write mix (the headline cluster sweep
+        # reads y once and writes means and covariances: 1.05 GB in and 5.24 GB out per launch, i.e. ~1 : 5; the lock-step
+        # kernel's checkpoint variant moves ~2 : 5)
         n = 1 << 28                                            # 1 GiB per row: far beyond L2
-        for nr, nw in ((1, 1), (2, 5), (0, 4), (4, 1)):
+        for nr, nw in ((1, 1), (1, 5), (2, 5), (0, 4), (4, 1)):
             src = torch.randn(max(nr, 1), n, device="cuda")[:nr] if nr else torch.empty(0, n, device="cuda")
             dst = torch.empty(nw, n, device="cuda")
             ms = timed(lambda: ctx.selftest_stream(src, dst), warm=3, reps=5)

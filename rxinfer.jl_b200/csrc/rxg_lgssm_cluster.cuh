@@ -11,15 +11,19 @@
 // One thread-block cluster of CL_CTAS CTAs owns 32 consecutive chains (lane = chain) for all T steps; CTA r owns the
 // time slice [r S, (r + 1) S), S = SPC L, and its CL_WARPS warps take its SPC sub-segments round robin.  Per CTA:
 //   load     y of the slice (S x m x 32 floats) and the slice's F, K, E, G records into shared memory with cp.async:
-//            the only read of y.
+//            the only read of y.  While those copies are in flight the CTA writes its span of the per-chain
+//            covariances (store_cov_span; PEER: in pass D instead).
 //   pass A   the zero-carry forward recursion of every sub-segment                           -> c
 //   scan     forward carries in two levels: inside the CTA through shared memory, across the cluster through
 //            distributed shared memory (each CTA's slice offset, read by the later CTAs between two cluster barriers)
 //   pass B   the forward recursion from the true carry; mu_f[t] overwrites y_t in shared memory (m >= d)
 //   pass C   the zero-carry backward recursion of every sub-segment over the stored mu_f    -> b
 //   scan     backward carries, the same two levels in the other direction
-//   pass D   the backward recursion from the true carry; smoothed means and broadcast covariances are the only HBM
-//            writes (streaming stores)
+//   pass D   the backward recursion from the true carry; stores the smoothed means (streaming stores)
+// The covariances are chain independent (every cov[t][i][j][.] is Sigma_s[t][i][j]), so they need not follow the chain
+// tiles: CTA k writes the k-th contiguous span of the flattened buffer as 16-byte streaming stores.  Written per tile in
+// pass D instead, they were 128-byte pieces 256 KiB apart from CTAs that drift apart in time (the pattern of
+// rxg_lgssm_seg.cuh's header, DESIGN 3.8), two thirds of the kernel's bytes.
 // HBM traffic per (chain, step) is 4 (m + d + d^2) bytes, the algorithmic 96 B at d = m = 4 (lgssm_shared_kernel's
 // checkpoint variant: ~115 B, it reads y twice and writes / reads a checkpoint per 12 steps).  The only synchronisation
 // is __syncthreads and the cluster barrier; the hardware co-schedules the CTAs of a cluster.
@@ -102,6 +106,40 @@ __device__ __forceinline__ void affine_step(const float* Mx, float (&v)[D], cons
     for (int i = 0; i < D; ++i) v[i] = n[i];
 }
 
+// This CTA's span of the per-chain covariances.  Every chain's copy of cov[t][i][j][.] is the table entry
+// Sigma_s[t][i][j] (the SS record of bwd_tab), so the bytes may be written in any order: CTA k owns the contiguous
+// float4s [k D^2 T, (k + 1) D^2 T) of the flattened cov[T][D][D][batch] (the grid has batch / 32 * CL_CTAS CTAs, so the
+// spans tile the buffer; batch % 32 == 0, so a float4 never straddles a row).  Thread-strided 16-byte streaming stores;
+// each thread tracks its row incrementally (one 64-bit division per thread) and reloads the entry only when its row
+// changes: at most twice at 65 536 chains, where a span covers at most two 256 KiB rows.
+template <int D, int M>
+__device__ __forceinline__ void store_cov_span(const float* __restrict__ bwd_tab, float* __restrict__ cov, int64_t batch,
+                                               int T) {
+    using TB = Tab<D, M>;
+    constexpr int NT = 32 * CL_WARPS;
+    const int n4 = (int)(batch / 4);                       // float4s per row
+    const int span = D * D * T;                            // float4s per CTA
+    const int64_t base = (int64_t)blockIdx.x * span;
+    float4* out = reinterpret_cast<float4*>(cov) + base;
+    const int step_rows = NT / n4, step_cols = NT % n4;
+    int i = (int)threadIdx.x;
+    const int64_t q = base + i;
+    int row = (int)(q / n4), col = (int)(q - (int64_t)row * n4);
+    int cur = -1;
+    float4 v = {};
+    for (; i < span; i += NT) {
+        if (row != cur) {
+            cur = row;
+            const float s = bwd_tab[(size_t)(row / (D * D)) * TB::BWD_REC + TB::SS_OFF + row % (D * D)];
+            v = make_float4(s, s, s, s);
+        }
+        __stcs(out + i, v);
+        row += step_rows;
+        col += step_cols;
+        if (col >= n4) { col -= n4; ++row; }
+    }
+}
+
 // PEER: the smoothed posteriors are also stored to the peer ranks' gathered buffers (fused all-gather, rxg_peer.cu),
 // so that a fused gather returns the bits of the plain sweep.
 template <int D, int M, bool PEER>
@@ -152,6 +190,7 @@ lgssm_cluster_sweep_kernel(const float* __restrict__ fwd_tab, const float* __res
         for (int p = tid; p < CL_CTAS * (CT::REC / 4); p += 32 * CL_WARPS)
             cp_async16(s_slice + p * 4, cl_tab + (size_t)CL_CTAS * spc * CT::REC + p * 4);
         cp_async_commit();
+        if (!PEER && write_cov) store_cov_span<D, M>(bwd_tab, cov, batch, T);
         cp_async_wait<0>();
     }
     __syncthreads();
@@ -347,13 +386,15 @@ lgssm_cluster_sweep_kernel(const float* __restrict__ fwd_tab, const float* __res
                     v[i][0] = nv[i];
                     __stcs(mean + ((int64_t)t * D + i) * batch + b, nv[i]);
                 }
-                float Sst[pad4(D * D)];
-                if (write_cov) {
-                    load_uniform<pad4(D * D)>(bwd_tab + (size_t)t * TB::BWD_REC + TB::SS_OFF, Sst);
+                if constexpr (PEER) {
+                    float Sst[pad4(D * D)];
+                    if (write_cov) {
+                        load_uniform<pad4(D * D)>(bwd_tab + (size_t)t * TB::BWD_REC + TB::SS_OFF, Sst);
 #pragma unroll
-                    for (int i = 0; i < D * D; ++i) __stcs(cov + ((int64_t)t * D * D + i) * batch + b, Sst[i]);
+                        for (int i = 0; i < D * D; ++i) __stcs(cov + ((int64_t)t * D * D + i) * batch + b, Sst[i]);
+                    }
+                    peer_store<D, 1>(po, write_cov, t, batch, b, v, Sst);
                 }
-                if (PEER) peer_store<D, 1>(po, write_cov, t, batch, b, v, Sst);
             }
         }
     }
