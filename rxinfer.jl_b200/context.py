@@ -544,45 +544,59 @@ class Context:
         return dict(mean=c.mean, cov=c.cov, a_mean=a_mean, a_cov=a_cov, **c.out, free_energy=c.fe, status=c.st)
 
     # ------------------------------------------------------------------ per-rule kernels
-    def _mat(self, M):
-        """PointMass matrix operand: host array => shared; CUDA tensor [r,c,n] => per message."""
+    def _mat(self, M, name, rows, cols, n):
+        """PointMass matrix operand [rows, cols] (None: taken from M): a host array or a CUDA tensor [rows, cols] is one
+        matrix shared by every message (shared = 1; a host array is copied to the device), a CUDA tensor [rows, cols, n]
+        one matrix per message (shared = 0).  Returns (kept tensor, pointer, shared, (rows, cols))."""
         if isinstance(M, torch.Tensor) and M.is_cuda:
-            self._dev(M)
-            return M, _fp(M), 0
-        t = torch.as_tensor(np.ascontiguousarray(np.asarray(M, dtype=np.float32)), device=f"cuda:{self.device}")
-        return t, _fp(t), 1
+            self._io(M, name)
+            shared = M.dim() == 2
+            r, c = M.shape[:2] if M.dim() in (2, 3) else (None, None)
+            want = (rows or r, cols or c) + (() if shared else (n,))
+            if tuple(M.shape) != want:
+                raise ValueError(f"{name}: expected a shared CUDA matrix {want[:2]} or one per message {want[:2] + (n,)}, "
+                                 f"got {tuple(M.shape)}")
+            return M, _fp(M), int(shared), want[:2]
+        a = np.ascontiguousarray(np.asarray(M.cpu() if isinstance(M, torch.Tensor) else M, dtype=np.float32))
+        if a.ndim != 2 or (rows is not None and a.shape[0] != rows) or (cols is not None and a.shape[1] != cols):
+            raise ValueError(f"{name}: expected a host matrix {(rows, cols)} shared by every message, got {a.shape} "
+                             f"(a matrix per message is a CUDA tensor [rows, cols, n])")
+        t = torch.as_tensor(a, device=f"cuda:{self.device}")
+        return t, _fp(t), 1, a.shape
+
+    def _msgs(self, v, name, *mats):
+        """A batch of messages: ``v`` [d, n] and the [d, d, n] matrices ``mats`` (name, tensor); returns (d, n)."""
+        self._io(v, name, ndim=2)
+        d, n = v.shape
+        for nm, M in mats:
+            self._io(M, nm, shape=(d, d, n))
+        return d, n
 
     def rule_add_cov(self, mu, S, Sigma, which="out"):
-        self._dev(mu, S)
-        d, n = mu.shape
-        keep, Sp, shared = self._mat(Sigma)
-        mo, So = torch.empty_like(mu), torch.empty_like(S)
+        d, n = self._msgs(mu, "mu", ("S", S))
+        keep, Sp, shared, _ = self._mat(Sigma, "Sigma", d, d, n)
+        mo, So = torch.empty_like(mu), self.empty(d, d, n)
         fn = self.lib.rxg_rule_mvnormal_meancov_out_f32 if which == "out" else self.lib.rxg_rule_mvnormal_meancov_mean_f32
         self._check(fn(self.h, n, d, _fp(mu), _fp(S), Sp, shared, _fp(mo), _fp(So), L.PTR_DEVICE))
         return mo, So
 
     def rule_mean_from_data(self, y, Sigma):
-        self._dev(y)
-        d, n = y.shape
-        keep, Sp, shared = self._mat(Sigma)
+        d, n = self._msgs(y, "y")
+        keep, Sp, shared, _ = self._mat(Sigma, "Sigma", d, d, n)
         mo, So = torch.empty_like(y), self.empty(d, d, n)
         self._check(self.lib.rxg_rule_mvnormal_meancov_mean_data_f32(self.h, n, d, _fp(y), Sp, shared, _fp(mo), _fp(So), L.PTR_DEVICE))
         return mo, So
 
     def rule_mul_out(self, A, mu, S):
-        self._dev(mu, S)
-        di, n = mu.shape
-        keep, Ap, shared = self._mat(A)
-        do = keep.shape[0]
+        di, n = self._msgs(mu, "mu", ("S", S))
+        keep, Ap, shared, (do, _) = self._mat(A, "A", None, di, n)
         mo, So = self.empty(do, n), self.empty(do, do, n)
         self._check(self.lib.rxg_rule_mul_out_f32(self.h, n, do, di, Ap, shared, _fp(mu), _fp(S), _fp(mo), _fp(So), L.PTR_DEVICE))
         return mo, So
 
     def rule_mul_in(self, A, mu_out, S_out):
-        self._dev(mu_out, S_out)
-        do, n = mu_out.shape
-        keep, Ap, shared = self._mat(A)
-        di = keep.shape[1]
+        do, n = self._msgs(mu_out, "mu_out", ("S_out", S_out))
+        keep, Ap, shared, (_, di) = self._mat(A, "A", do, None, n)
         xi, W = self.empty(di, n), self.empty(di, di, n)
         st = self.empty(n, dtype=torch.int32)
         self._check(self.lib.rxg_rule_mul_in_f32(self.h, n, do, di, Ap, shared, _fp(mu_out), _fp(S_out), _fp(xi), _fp(W),
@@ -590,9 +604,9 @@ class Context:
         return xi, W, st
 
     def _pair(self, fn, a, Sa, b, Sb):
-        self._dev(a, Sa, b, Sb)
-        d, n = a.shape
-        o, So = torch.empty_like(a), torch.empty_like(Sa)
+        d, n = self._msgs(a, "first vector", ("first matrix", Sa), ("second matrix", Sb))
+        self._io(b, "second vector", shape=(d, n))
+        o, So = torch.empty_like(a), self.empty(d, d, n)
         self._check(fn(self.h, n, d, _fp(a), _fp(Sa), _fp(b), _fp(Sb), _fp(o), _fp(So), L.PTR_DEVICE))
         return o, So
 
@@ -606,9 +620,8 @@ class Context:
         return self._pair(self.lib.rxg_prod_gaussian_f32, xi1, W1, xi2, W2)
 
     def _conv(self, fn, v, M):
-        self._dev(v, M)
-        d, n = v.shape
-        vo, Mo = torch.empty_like(v), torch.empty_like(M)
+        d, n = self._msgs(v, "vector", ("matrix", M))
+        vo, Mo = torch.empty_like(v), self.empty(d, d, n)
         st = self.empty(n, dtype=torch.int32)
         self._check(fn(self.h, n, d, _fp(v), _fp(M), _fp(vo), _fp(Mo), _i32(st), L.PTR_DEVICE))
         return vo, Mo, st
@@ -620,10 +633,15 @@ class Context:
         return self._conv(self.lib.rxg_wmp_to_meancov_f32, xi, W)
 
     def marginal_gaussian(self, msgs):
-        d, n = msgs[0][0].shape
+        """Product of the k (xi [d, n], W [d, d, n]) messages ``msgs``, as (mean, covariance, status)."""
+        msgs = list(msgs)
+        if not msgs:
+            raise ValueError("marginal_gaussian: needs at least one (xi, W) message")
         k = len(msgs)
-        for xi, W in msgs:
-            self._dev(xi, W)
+        d, n = self._msgs(msgs[0][0], "xi[0]", ("W[0]", msgs[0][1]))
+        for q, (xi, W) in enumerate(msgs):
+            self._io(xi, f"xi[{q}]", shape=(d, n))
+            self._io(W, f"W[{q}]", shape=(d, d, n))
         xs = (L.fp * k)(*[_fp(x) for x, _ in msgs])
         ws = (L.fp * k)(*[_fp(w) for _, w in msgs])
         mu, S = self.empty(d, n), self.empty(d, d, n)
@@ -647,30 +665,40 @@ class Context:
 
     def rule_normal_precision_tau_joint(self, m_joint, V_joint):
         """Structured tau rule: q(out, mu) jointly Gaussian, m_joint[2, n], V_joint[2, 2, n]."""
-        self._dev(m_joint, V_joint)
+        self._io(m_joint, "m_joint", ndim=2)
         n = m_joint.shape[-1]
+        self._io(m_joint, "m_joint", shape=(2, n))
+        self._io(V_joint, "V_joint", shape=(2, 2, n))
         sh, rt = self.empty(n), self.empty(n)
         self._check(self.lib.rxg_rule_normal_precision_tau_joint_f32(self.h, n, _fp(m_joint), _fp(V_joint), _fp(sh), _fp(rt), L.PTR_DEVICE))
         return sh, rt
 
     def rule_mvnormal_precision_lambda(self, m_out, V_out, m_mu, V_mu):
-        self._dev(m_out, V_out, m_mu, V_mu)
-        d, n = m_out.shape
+        d, n = self._msgs(m_out, "m_out", ("V_out", V_out), ("V_mu", V_mu))
+        self._io(m_mu, "m_mu", shape=(d, n))
         df, iS = self.empty(n), self.empty(d, d, n)
         self._check(self.lib.rxg_rule_mvnormal_precision_lambda_f32(self.h, n, d, _fp(m_out), _fp(V_out), _fp(m_mu), _fp(V_mu),
                                                                     _fp(df), _fp(iS), L.PTR_DEVICE))
         return df, iS
 
+    def _wishart(self, pairs):
+        """Wishart messages (df [n], inverse scale [d, d, n]) in ``pairs`` (name, df, iS); returns (d, n)."""
+        iS0 = pairs[0][2]
+        self._io(iS0, f"{pairs[0][0]}: inverse scale", ndim=3)
+        d, n = iS0.shape[0], iS0.shape[-1]
+        for name, df, iS in pairs:
+            self._io(df, f"{name}: df", shape=(n,))
+            self._io(iS, f"{name}: inverse scale", shape=(d, d, n))
+        return d, n
+
     def prod_wishart(self, df1, iS1, df2, iS2):
-        self._dev(df1, iS1, df2, iS2)
-        d, n = iS1.shape[0], iS1.shape[-1]
+        d, n = self._wishart([("first", df1, iS1), ("second", df2, iS2)])
         df, iS = self.empty(n), self.empty(d, d, n)
         self._check(self.lib.rxg_prod_wishart_f32(self.h, n, d, _fp(df1), _fp(iS1), _fp(df2), _fp(iS2), _fp(df), _fp(iS), L.PTR_DEVICE))
         return df, iS
 
     def wishart_mean(self, df, iS):
-        self._dev(df, iS)
-        d, n = iS.shape[0], iS.shape[-1]
+        d, n = self._wishart([("wishart", df, iS)])
         out = self.empty(d, d, n)
         st = self.empty(n, dtype=torch.int32)
         self._check(self.lib.rxg_wishart_mean_f32(self.h, n, d, _fp(df), _fp(iS), _fp(out),

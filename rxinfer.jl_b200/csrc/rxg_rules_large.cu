@@ -20,7 +20,7 @@
 
 namespace rxg {
 
-constexpr int RL_MSGS = 8;          // messages (= warps) per CTA of k_cholinv_warp (6 at d > 57, see cholinv_warp)
+constexpr int RL_MSGS = 8;          // messages (= warps) per CTA of k_cholinv_warp (6 at d > 58, see cholinv_warp)
 
 // o[r][i] = (a ? a[r][i] : 0) + sb * (b ? (b_bcast ? b[r] : b[r][i]) : 0)
 __global__ void __launch_bounds__(256)
@@ -267,7 +267,7 @@ int left_gemm_per_slice(rxg_ctx* ctx, int M, int K, int64_t N, const float* A, c
     return RXG_OK;
 }
 static int cholinv_warp(rxg_ctx* ctx, int64_t n, int d, int k, const RuleList& in, float* vo, float* Mo, int32_t* status) {
-    // 8 messages per CTA (one 32-byte sector per element) unless that leaves room for only one CTA per SM (d > 57): then 6,
+    // 8 messages per CTA (one 32-byte sector per element) unless that leaves room for only one CTA per SM (d > 58): then 6,
     // so that two CTAs = 12 warps share an SM -- the kernel is latency bound
     const size_t per_msg = ((size_t)d * (d + 1) + 3 * d) * sizeof(float);
     const int nm = (RL_MSGS * per_msg > 113 * 1024) ? 6 : RL_MSGS;

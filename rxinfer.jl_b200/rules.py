@@ -14,10 +14,19 @@ class RuleMethodError(NotImplementedError):
     pass
 
 
+def _meancov(msg):
+    """(mu [d, n], Sigma [d, d, n]) of a mean-covariance message: a covariance [d, d] shared by the batch (the form
+    ``MvNormalMeanCovariance`` documents) is expanded to one per message, the layout every rule kernel reads."""
+    mu, S = msg.mu, msg.Sigma
+    if S.dim() == 2 and mu.dim() == 2:
+        S = S.unsqueeze(-1).expand(*S.shape, mu.shape[-1]).contiguous()
+    return mu, S
+
+
 def _mc(ctx, msg):
     """mean_cov(msg): converts a (xi, W) message with one cholinv, like the reference."""
     if isinstance(msg, MvNormalMeanCovariance):
-        return msg.mu, msg.Sigma
+        return _meancov(msg)
     if isinstance(msg, MvNormalWeightedMeanPrecision):
         mu, S, _ = ctx.wmp_to_meancov(msg.xi, msg.W)
         return mu, S
@@ -27,7 +36,7 @@ def _mc(ctx, msg):
 def _wmp(ctx, msg):
     if isinstance(msg, MvNormalWeightedMeanPrecision):
         return msg.xi, msg.W
-    xi, W, _ = ctx.meancov_to_wmp(msg.mu, msg.Sigma)
+    xi, W, _ = ctx.meancov_to_wmp(*_meancov(msg))
     return xi, W
 
 
@@ -66,8 +75,7 @@ def call_rule(ctx, node: str, edge: str, **kw):
             return GammaShapeRate(*ctx.rule_normal_precision_tau(mo, vo, mm, vm))
         if edge == "τ" and "q_out_μ" in kw:
             # structured: q(out, mu) jointly Gaussian (MvNormalMeanCovariance with d = 2)
-            j = kw["q_out_μ"]
-            return GammaShapeRate(*ctx.rule_normal_precision_tau_joint(j.mu, j.Sigma))
+            return GammaShapeRate(*ctx.rule_normal_precision_tau_joint(*_mc(ctx, kw["q_out_μ"])))
         if edge == "out" and "q_τ" in kw and "m_μ" in kw:
             # (m_μ::Normal, q_τ): belief-propagation message on the mean edge -> N(m_μ, v_μ + 1/E[τ])
             src = kw["m_μ"]
