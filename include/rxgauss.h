@@ -691,6 +691,54 @@ int rxg_lgssm_smooth_gather_f32(rxg_ctx*, int d, int m, int T, int64_t batch_loc
                                 float* const* gathered_mean, float* const* gathered_cov,
                                 float* neg_log_evidence, int32_t* status, unsigned flags);
 
+/* ------------------------------------------------------------------ Delta node (nonlinear maps) ----------
+ * z := f(x) between Gaussian nodes with meta Linearization() or Unscented(alpha, beta, kappa)
+ * [ref: docs/src/manuals/inference/delta-node.md; paper/example.jl].  The user supplies CUDA C++ source defining
+ *   template <class S> __device__ void f(const S* x, S* z);   (transition, R^d -> R^d)
+ *   template <class S> __device__ void g(const S* x, S* y);   (optional observation map, R^d -> R^m)
+ * calling math functions unqualified (sin, cos, tan, exp, log, sqrt, tanh, atan, atan2, pow, fabs).  The library
+ * compiles it at run time with NVRTC, loaded with dlopen once per process by the first compile: the path in
+ * RXG_NVRTC as rxg_create read it for the context that compiles first, else libnvrtc.so.12 (rxg_delta_check_source
+ * always uses the soname); later overrides are ignored once NVRTC is loaded.  The source is compiled
+ * with the library's Delta header, for sm_90a and exactly one (d, m), d and m in 1..8.  Linearization runs in fp32
+ * (Jacobians by forward-mode dual numbers); Unscented in fp64 (2d + 1 sigma points; ut = {alpha, beta, kappa} or
+ * NULL for ReactiveMP's Unscented() defaults {1e-3, 2, 0}).  Without NVRTC the entries return RXG_ERR_UNSUPPORTED;
+ * a compile error returns RXG_ERR_BAD_ARG with the compiler log in `log` (and in rxg_last_error).
+ * A model belongs to its context: the context caches one module per (source, names, d, m, method, ut), so a second
+ * create of the same model compiles nothing, and rxg_destroy unloads them all.
+ * Model constants (row-major host arrays) are shared by every chain; data are device arrays (RXG_PTR_DEVICE is
+ * required).  Per-chain status: RXG_ERR_NOT_SPD (a predicted or innovation covariance is not SPD), RXG_ERR_NAN.  */
+typedef struct rxg_delta_model rxg_delta_model;
+#define RXG_DELTA_LINEARIZATION 0
+#define RXG_DELTA_UNSCENTED 1
+/* Compile check without a context or a GPU: RXG_OK, or RXG_ERR_BAD_ARG with the NVRTC log (which also carries the
+ * ptxas register / spill report of both kernels on success).                                                       */
+int rxg_delta_check_source(const char* source, const char* f_name, const char* g_name, int d, int m, int method,
+                           const double ut[3], char* log, size_t log_cap);
+int rxg_delta_model_create(rxg_ctx*, const char* source, const char* f_name, const char* g_name, int d, int m,
+                           int method, const double ut[3], rxg_delta_model** out, char* log, size_t log_cap);
+/* NVRTC compilations this context has run (a cached create adds none)                                             */
+long long rxg_delta_compile_count(const rxg_ctx*);
+/* Whole series, one fused launch: x[1] ~ N(m0, S0), x[t] = f(x[t-1]) + N(0, P), y[t] ~ N(B x[t], Q) (g NULL) or
+ * N(g(x[t]), Q) (B may be NULL); the EKF / UKF forward pass then the ERTS / URTS backward pass, the transition
+ * linearised at the filtered marginals.  y[T][m][batch]; ymask[T][batch] (1 = observed) or NULL;
+ * post_mean[T][d][batch], post_cov[T][d][d][batch]; filt_mean / filt_cov (same shapes) or NULL; status[batch] or NULL. */
+int rxg_delta_smooth_f32(rxg_ctx*, const rxg_delta_model* model, int T, int64_t batch, const float* m0,
+                         const float* S0, const float* P, const float* B, const float* Q, const float* y,
+                         const uint8_t* ymask, float* post_mean, float* post_cov, float* filt_mean, float* filt_cov,
+                         int32_t* status, unsigned flags);
+/* Streaming filter, one time-chunk of Tc data.  Carry q(x) = carry_mean[d][batch], carry_cov[d][d][batch] (device,
+ * updated in place); every datum pushes it through f (+ P) and then updates it by y.  Known noise: Q (carry_tau and
+ * filt_tau NULL).  Learned precision (m = 1, B the observation row, no g, Q NULL): y ~ N(B x, 1/tau), q(x) q(tau),
+ * carry_tau[2][batch] = (shape, rate) of q(tau), which is both the next datum's Gamma prior and its initial q(tau),
+ * and `iters` VMP iterations per datum; filt_tau[Tc][2][batch] or NULL.  filt_mean[Tc][d][batch] /
+ * filt_cov[Tc][d][d][batch] or NULL.  The carry is rounded to fp32 after every datum, so splitting a stream into
+ * chunks gives the same result, bit for bit, as one call.                                                           */
+int rxg_delta_filter_chunk_f32(rxg_ctx*, const rxg_delta_model* model, int Tc, int64_t batch, const float* P,
+                               const float* B, const float* Q, int iters, const float* y, const uint8_t* ymask,
+                               float* carry_mean, float* carry_cov, float* carry_tau, float* filt_mean, float* filt_cov,
+                               float* filt_tau, int32_t* status, unsigned flags);
+
 #ifdef __cplusplus
 }
 #endif

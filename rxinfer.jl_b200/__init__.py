@@ -22,7 +22,8 @@ def __getattr__(name):   # lazy: these import torch
                 "linear_gaussian_ssm_continuous_transition", "gaussian_mixture", "MeanField", "BetheFactorization",
                 "hidden_markov_model", "HMMConstraints", "hgf_offline", "gaussian_hidden_markov_model",
                 "GaussianHMMConstraints", "binomial_regression", "multinomial_regression",
-                "multinomial_regression_online",
+                "multinomial_regression_online", "CudaFunction", "Linearization", "Unscented",
+                "nonlinear_gaussian_ssm_smoothing", "nonlinear_gaussian_ssm_filtering", "nonlinear_gamma_streaming",
                 "default_context",
                 "KeepLast", "KeepEach"):
         from . import inference

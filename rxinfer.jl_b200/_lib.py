@@ -27,6 +27,7 @@ COV_REPLICATE = 1 << 6
 MASK_SHARED = 1 << 7
 U_SEQ_SHARED = 1 << 8      # u is one input sequence for every chain, a host array [rows, d]
 U_SEQ_CHAIN = 1 << 9       # u is a per-chain input sequence, a device array [rows, d, batch]
+RXG_DELTA_LINEARIZATION, RXG_DELTA_UNSCENTED = 0, 1
 
 fp = POINTER(c_float)
 u8p = POINTER(c_uint8)
@@ -128,6 +129,15 @@ SIGNATURES = {
     "rxg_peer_allgather_f32": (c_int, [c_void_p, c_int64, fp, POINTER(fp), c_uint]),
     "rxg_lgssm_smooth_gather_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, fp, fp, fp, fp, fp, fp, fp, fp, u8p,
                                             POINTER(fp), POINTER(fp), fp, i32p, c_uint]),
+    "rxg_delta_check_source": (c_int, [c_char_p, c_char_p, c_char_p, c_int, c_int, c_int, POINTER(c_double), c_char_p,
+                                       c_size_t]),
+    "rxg_delta_model_create": (c_int, [c_void_p, c_char_p, c_char_p, c_char_p, c_int, c_int, c_int, POINTER(c_double),
+                                       POINTER(c_void_p), c_char_p, c_size_t]),
+    "rxg_delta_compile_count": (c_longlong, [c_void_p]),
+    "rxg_delta_smooth_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, fp, fp, fp, fp, fp, fp, u8p, fp, fp, fp, fp, i32p,
+                                     c_uint]),
+    "rxg_delta_filter_chunk_f32": (c_int, [c_void_p, c_void_p, c_int, c_int64, fp, fp, fp, c_int, fp, u8p, fp, fp, fp, fp,
+                                           fp, fp, i32p, c_uint]),
 }
 
 
@@ -147,11 +157,28 @@ def _missing_entry(name):
     return call
 
 
+def _preload_nvrtc():
+    """The Delta node compiles user functions with NVRTC, which the library opens as libnvrtc.so.12 on first use.  When
+    the NVRTC wheel that PyTorch depends on is installed, load its copy globally so that this soname resolves even
+    where no CUDA toolkit is on the loader's path."""
+    import importlib.util
+    try:
+        spec = importlib.util.find_spec("nvidia.cuda_nvrtc")
+    except (ImportError, ValueError):
+        return
+    for base in (spec.submodule_search_locations or []) if spec else []:
+        path = os.path.join(base, "lib", "libnvrtc.so.12")
+        if os.path.exists(path):
+            ctypes.CDLL(path, mode=ctypes.RTLD_GLOBAL)
+            return
+
+
 def load():
     """Load the in-tree shared library.  Raises (never falls back) if it has not been built."""
     global _lib
     if _lib is not None:
         return _lib
+    _preload_nvrtc()
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python rxinfer.jl_b200/build.py` "

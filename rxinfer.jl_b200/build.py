@@ -20,10 +20,10 @@ UNITS = ([("rxg_lgssm.cu", f"rxg_lgssm_d{d}m{m}", (f"-DRXG_INST_D={d}", f"-DRXG_
           ("rxg_lgssm_large.cu", "rxg_lgssm.cu", "rxg_umma_sweep.cu", "rxg_api.cu", "rxg_peer.cu", "rxg_rules.cu", "rxg_hgf.cu",
            "rxg_lgssm_general.cu", "rxg_lgssm_generic.cu", "rxg_lar.cu", "rxg_rules_large.cu", "rxg_predict.cu",
            "rxg_lgssm_vmp.cu", "rxg_mixture.cu", "rxg_hmm.cu", "rxg_hgf_learn.cu", "rxg_hmm_gauss.cu", "rxg_polya.cu",
-           "rxg_multinomial.cu")] +
+           "rxg_multinomial.cu", "rxg_delta.cu")] +
          [("rxg_hostfill.cpp", "rxg_hostfill", ())])        # plain C++ (g++): host-side covariance broadcast
 SOURCES = sorted({u[0] for u in UNITS})
-HEADERS = ["rxg_internal.h", "rxg_linalg.cuh", "rxg_gain.cuh", "rxg_lgssm_common.cuh", "rxg_chain_step.cuh", "rxg_lgssm_shared.cuh", "rxg_lgssm_seg.cuh", "rxg_lgssm_cluster.cuh", "rxg_sweep_select.h", "rxg_umma.cuh", "rxg_lar.cuh", "rxg_hmm.cuh", "rxg_hgf_learn.cuh", "rxg_hmm_gauss.cuh", "rxg_normal_wishart.cuh", "rxg_polya.cuh", "rxg_multinomial.cuh", os.path.join("..", "..", "include", "rxgauss.h")]
+HEADERS = ["rxg_internal.h", "rxg_linalg.cuh", "rxg_gain.cuh", "rxg_lgssm_common.cuh", "rxg_chain_step.cuh", "rxg_lgssm_shared.cuh", "rxg_lgssm_seg.cuh", "rxg_lgssm_cluster.cuh", "rxg_sweep_select.h", "rxg_umma.cuh", "rxg_lar.cuh", "rxg_hmm.cuh", "rxg_hgf_learn.cuh", "rxg_hmm_gauss.cuh", "rxg_normal_wishart.cuh", "rxg_polya.cuh", "rxg_multinomial.cuh", "rxg_delta.cuh", os.path.join("..", "..", "include", "rxgauss.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-mavx2", "-Xcompiler", "-pthread", "--expt-relaxed-constexpr", "-Xptxas", "-v",
@@ -35,6 +35,22 @@ def _nvcc():
         if cand and os.path.exists(cand):
             return cand
     raise RuntimeError("nvcc not found: librxgauss cannot be built (there is no CPU fallback)")
+
+
+def embed_delta_header(objdir: str) -> str:
+    """rxg_delta.cuh as the byte array ``rxg_delta_header_src`` (NUL-terminated) in an object of its own: the library
+    compiles it, with the user's functions, at run time (rxg_delta.cu)."""
+    with open(os.path.join(CSRC, "rxg_delta.cuh"), "rb") as f:
+        data = f.read() + b"\0"
+    src = os.path.join(objdir, "rxg_delta_header.cpp")
+    rows = ",\n".join(",".join(str(b - 256 if b > 127 else b) for b in data[i:i + 32]) for i in range(0, len(data), 32))
+    with open(src, "w") as f:
+        f.write(f"extern const char rxg_delta_header_src[] = {{\n{rows}\n}};\n")
+    obj = os.path.join(objdir, "rxg_delta_header.o")
+    r = subprocess.run(["g++", "-O0", "-fPIC", "-c", src, "-o", obj], capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError(f"compiling the embedded Delta header failed:\n{r.stderr}")
+    return obj
 
 
 def _stale():
@@ -73,6 +89,7 @@ def build(force: bool = False, verbose: bool = False, extra_flags=(), lib: str =
 
     with cf.ThreadPoolExecutor(max_workers=min(len(UNITS), os.cpu_count() or 4)) as ex:
         objs = list(ex.map(compile_one, UNITS))
+    objs.append(embed_delta_header(objdir))
     tmp = lib + ".tmp"      # link next to the target and rename: a concurrent reader never sees a partial file
     cmd = [nvcc, "-shared", "-o", tmp, *objs, "-ldl", "-lpthread", "-Xcompiler", "-fPIC"]
     r = subprocess.run(cmd, capture_output=True, text=True)

@@ -54,6 +54,17 @@ def _host_arrays(who, arrays, dims, nulls=False):
     return keep
 
 
+def delta_mask(mask, T, batch, device, who):
+    """The Delta kernels read ymask[t][b] for every step and chain: a mask must be [T, batch] exactly (checked on the
+    host, before anything is copied or launched).  Returns it as contiguous uint8 on ``device``, or None."""
+    if mask is None:
+        return None
+    shape = tuple(mask.shape) if hasattr(mask, "shape") else tuple(np.shape(mask))
+    if shape != (T, batch):
+        raise ValueError(f"{who}: mask must be [T, batch] = {(T, batch)} (1 = observed), got {shape}")
+    return torch.as_tensor(mask, device=device).to(torch.uint8).contiguous()
+
+
 class Context:
     """``rxg_ctx`` bound to a CUDA device.  Launches go to torch's current stream on that device
     (so ``torch.cuda.Event`` timing and stream ordering with torch ops are meaningful)."""
@@ -321,6 +332,75 @@ class Context:
         self._check(self.lib.rxg_lgssm_filter_chunk_f32(self.h, d, m, T, batch, *ptrs, _fp(prev_mean), cc, _fp(y),
                                                         _fp(mean), _fp(cov), _fp(nle), flags))
         return dict(mean=mean, cov=cov, neg_log_evidence=nle)
+
+    # ------------------------------------------------------------------ Delta node (user functions, NVRTC)
+    def delta_model(self, source, f_name, d, m, method, g_name=None, ut=None):
+        """``rxg_delta_model_create``: compile (or find in this context's cache) the module of the user functions
+        ``f_name`` (R^d -> R^d) and ``g_name`` (R^d -> R^m, or None) defined in the CUDA ``source``; ``method`` is
+        ``L.RXG_DELTA_LINEARIZATION`` or ``L.RXG_DELTA_UNSCENTED`` with ``ut = (alpha, beta, kappa)`` or None for the
+        defaults.  A compile error raises ``RxGaussError`` carrying the NVRTC log."""
+        log = ctypes.create_string_buffer(1 << 16)
+        h = c_void_p()
+        uta = (ctypes.c_double * 3)(*ut) if ut is not None else None
+        rc = self.lib.rxg_delta_model_create(self.h, source.encode(), f_name.encode(), g_name.encode() if g_name else None,
+                                             int(d), int(m), int(method), uta, ctypes.byref(h), log, len(log))
+        self._check(rc)
+        return SimpleNamespace(h=h, d=int(d), m=int(m), method=int(method), has_g=g_name is not None)
+
+    @property
+    def delta_compiles(self) -> int:
+        """NVRTC compilations this context has run (a cached ``delta_model`` adds none)."""
+        return int(self.lib.rxg_delta_compile_count(self.h))
+
+    def _delta_consts(self, model, **arrays):
+        d, m = model.d, model.m
+        shapes = {"m0": (d,), "S0": (d, d), "P": (d, d), "B": (m, d), "Q": (m, m)}
+        return _host_arrays("delta", {k: (v, shapes[k]) for k, v in arrays.items()}, f"d = {d}, m = {m}", nulls=True)
+
+    def delta_smooth(self, model, y, m0, S0, P, Q, B=None, mask=None, want_filtered=False):
+        """``rxg_delta_smooth_f32``: y[T, m, batch] (CUDA fp32), mask[T, batch] (uint8 / bool) or None.  Returns mean
+        [T, d, batch], cov [T, d, d, batch], status [batch] and, with ``want_filtered``, filt_mean / filt_cov."""
+        self._io(y, "delta_smooth: y [T, m, batch]", ndim=3)
+        T, m, batch = y.shape
+        if m != model.m:
+            raise ValueError(f"delta_smooth: y has m = {m}, the model m = {model.m}")
+        d = model.d
+        k = self._delta_consts(model, m0=m0, S0=S0, P=P, B=B, Q=Q)
+        mk = delta_mask(mask, T, batch, y.device, "delta_smooth")
+        mean, cov = self.empty(T, d, batch), self.empty(T, d, d, batch)
+        fm = self.empty(T, d, batch) if want_filtered else None
+        fc = self.empty(T, d, d, batch) if want_filtered else None
+        st = self.empty(batch, dtype=torch.int32)
+        self._check(self.lib.rxg_delta_smooth_f32(self.h, model.h, T, batch, k["m0"][1], k["S0"][1], k["P"][1], k["B"][1],
+                                                  k["Q"][1], _fp(y), _u8(mk), _fp(mean), _fp(cov), _fp(fm), _fp(fc),
+                                                  _i32(st), L.PTR_DEVICE))
+        return dict(mean=mean, cov=cov, filt_mean=fm, filt_cov=fc, status=st)
+
+    def delta_filter_chunk(self, model, y, P, carry_mean, carry_cov, Q=None, B=None, carry_tau=None, iters=1, mask=None,
+                           want_history=True):
+        """``rxg_delta_filter_chunk_f32``: one time-chunk y[Tc, m, batch] of the streaming filter.  The carry
+        ``carry_mean[d, batch]`` / ``carry_cov[d, d, batch]`` (and ``carry_tau[2, batch]`` = (shape, rate) of a learned
+        precision, m = 1, ``B`` the observation row, no ``Q``) are CUDA fp32 tensors updated in place.  Returns the
+        chunk's filtered mean / cov (and tau [Tc, 2, batch]) when ``want_history``, and status [batch]."""
+        self._io(y, "delta_filter_chunk: y [Tc, m, batch]", ndim=3)
+        T, m, batch = y.shape
+        if m != model.m:
+            raise ValueError(f"delta_filter_chunk: y has m = {m}, the model m = {model.m}")
+        d = model.d
+        for t, name, shp in ((carry_mean, "carry_mean", (d, batch)), (carry_cov, "carry_cov", (d, d, batch)),
+                             (carry_tau, "carry_tau", (2, batch))):
+            self._io(t, f"delta_filter_chunk: {name}", shape=shp)
+        k = self._delta_consts(model, P=P, B=B, Q=Q)
+        mk = delta_mask(mask, T, batch, y.device, "delta_filter_chunk")
+        fm = self.empty(T, d, batch) if want_history else None
+        fc = self.empty(T, d, d, batch) if want_history else None
+        ft = self.empty(T, 2, batch) if want_history and carry_tau is not None else None
+        st = self.empty(batch, dtype=torch.int32)
+        self._check(self.lib.rxg_delta_filter_chunk_f32(self.h, model.h, T, batch, k["P"][1], k["B"][1], k["Q"][1],
+                                                        int(iters), _fp(y), _u8(mk), _fp(carry_mean), _fp(carry_cov),
+                                                        _fp(carry_tau), _fp(fm), _fp(fc), _fp(ft), _i32(st),
+                                                        L.PTR_DEVICE))
+        return dict(mean=fm, cov=fc, tau=ft, status=st)
 
     HGF_LEARN_PRIOR = (1.0, 1.0, 0.0, 1.0, 0.0, 1.0, 0.0, 1.0)   # hgf_1: kappa, omega, x_0, z[1] ~ N(mean, variance)
     HGF_LEARN_INIT = (1.0, 1.0, 0.0, 1.0, 0.0, 1.0, 0.0, 1.0)    # initial q(kappa), q(omega), q(z), q(x)

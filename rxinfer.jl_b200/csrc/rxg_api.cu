@@ -153,6 +153,10 @@ static int numa_node_count() {
     return n;
 }
 
+namespace rxg {
+void delta_ctx_init(const rxg_ctx* ctx);       // rxg_delta.cu: the NVRTC path override and the Delta module cache
+void delta_ctx_release(const rxg_ctx* ctx);
+}
 
 extern "C" {
 
@@ -186,6 +190,7 @@ int rxg_create(rxg_ctx** out, int device, unsigned flags) {
         {RXG_OPT_GATHER_MODE, "RXG_GATHER_MODE"}, {RXG_OPT_POLYA_PATH, "RXG_POLYA_PATH"}};
     for (const auto& e : kEnv)
         if (const char* v = getenv(e.env)) ctx->opt[e.id] = atoll(v);
+    rxg::delta_ctx_init(ctx);      // RXG_NVRTC
     *out = ctx;
     return RXG_OK;
 }
@@ -209,6 +214,7 @@ int rxg_destroy(rxg_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     rxg_comm_destroy_internal(ctx);
+    rxg::delta_ctx_release(ctx);
     if (ctx->ws) cudaFree(ctx->ws);
     if (ctx->stage) cudaFree(ctx->stage);
     if (ctx->d_bad) cudaFree(ctx->d_bad);

@@ -495,6 +495,169 @@ def _predict_keys(predictvars, model, data):
     return keys
 
 
+# --------------------------------------------------------------------------- Delta node (nonlinear maps)
+@dataclass
+class CudaFunction:
+    """A user function for a Delta node: CUDA C++ ``source`` defining
+    ``template <class S> __device__ void <name>(const S* x, S* z)`` from R^d_in to R^d_out, with math functions called
+    unqualified (the library instantiates it with dual numbers for Linearization and with double for Unscented)."""
+    source: str
+    name: str
+    d_in: int
+    d_out: int
+
+
+class Linearization(_Marker):
+    """``Linearization()``: the Delta node's messages from the first-order Taylor expansion at the incoming mean
+    (Jacobians by forward-mode dual numbers, fp32)."""
+
+
+@dataclass(frozen=True)
+class Unscented:
+    """``Unscented(alpha=, beta=, kappa=)``: the unscented transform with 2d + 1 sigma points (fp64); the defaults are
+    ReactiveMP's."""
+    alpha: float = 1e-3
+    beta: float = 2.0
+    kappa: float = 0.0
+
+
+@dataclass
+class nonlinear_gaussian_ssm_smoothing:
+    """``x[1] ~ x0; x[t] ~ N(f(x[t-1]), P); y[t] ~ N(B x[t], Q)`` or ``N(g(x[t]), Q)``, the Delta node ``f`` (and ``g``)
+    approximated as ``meta`` says [ref: test/models/nonlinear/].  ``x0 = (mean, cov)``."""
+    f: CudaFunction
+    P: np.ndarray
+    Q: np.ndarray
+    x0: tuple
+    B: np.ndarray = None
+    g: CudaFunction = None
+
+
+@dataclass
+class nonlinear_gaussian_ssm_filtering(nonlinear_gaussian_ssm_smoothing):
+    """The one-step model with ``@autoupdates`` of ``mean_cov(q(x_t))``: every datum pushes the carry through f (and
+    P) before its observation; ``x0`` initialises the carry."""
+
+
+@dataclass
+class nonlinear_gamma_streaming:
+    """The paper's pendulum (paper/example.jl): ``previous_state ~ MvNormal(prior)``, ``state ~ f(previous_state)``,
+    ``noise ~ Gamma(shape, scale)``, ``observation ~ Normal(dot(c, state), precision = noise)`` with
+    ``q(state, noise) = q(state) q(noise)`` and the priors autoupdated from q(state) and q(noise).  ``state0 = (mean,
+    cov)`` and ``noise0 = (shape, scale)`` are the initial marginals (and the first datum's priors); ``P`` an optional
+    process noise added to the Delta node's message (the paper has none)."""
+    f: CudaFunction
+    c: np.ndarray
+    state0: tuple = ((0.5, 0.0), ((0.01, 0.0), (0.0, 0.01)))
+    noise0: tuple = (1.0, 100.0)
+    P: np.ndarray = None
+
+
+_DELTA_MODELS = (nonlinear_gaussian_ssm_smoothing, nonlinear_gamma_streaming)
+
+
+def delta_method(model, meta):
+    """The one approximation ``meta`` assigns to the model's Delta nodes: (method code, (alpha, beta, kappa) or None)."""
+    if not isinstance(meta, dict):
+        raise ValueError("meta: expected a dict {'f': Linearization() or Unscented(...), 'g': ...}")
+    nodes = ["f"] + (["g"] if getattr(model, "g", None) is not None else [])
+    bad = set(meta) - set(nodes)
+    if bad:
+        raise ValueError(f"meta: {sorted(bad)} are not Delta nodes of {type(model).__name__} (its nodes: {nodes})")
+    methods = []
+    for n in nodes:
+        m = meta.get(n)
+        if not isinstance(m, (Linearization, Unscented)):
+            # the reference refuses a Delta node without an approximation method between Gaussian nodes
+            raise ValueError(f"meta: the Delta node {n!r} needs an approximation method: Linearization() or Unscented()")
+        methods.append(m)
+    if any(m != methods[0] for m in methods[1:]):
+        raise NotImplementedError("meta: f and g with different approximation methods are outside the batched hot path")
+    m = methods[0]
+    if isinstance(m, Linearization):
+        return L.RXG_DELTA_LINEARIZATION, None
+    return L.RXG_DELTA_UNSCENTED, (float(m.alpha), float(m.beta), float(m.kappa))
+
+
+def delta_module(ctx, model, meta):
+    """The compiled module of the model's Delta nodes (cached by the context)."""
+    method, ut = delta_method(model, meta)
+    f, g = model.f, getattr(model, "g", None)
+    d = f.d_in
+    if f.d_out != d:
+        raise ValueError(f"f maps R^{f.d_in} to R^{f.d_out}: a transition maps R^d to R^d")
+    m = 1
+    if g is not None:
+        if g.d_in != d:
+            raise ValueError(f"g takes R^{g.d_in}, the state is R^{d}")
+        m = g.d_out
+    elif getattr(model, "B", None) is not None:
+        m = np.atleast_2d(np.asarray(model.B)).shape[0]
+    elif not isinstance(model, nonlinear_gamma_streaming):
+        raise ValueError("the observation needs B (linear) or g (a CudaFunction)")
+    source = f.source if g is None or g.source == f.source else f.source + "\n" + g.source
+    return ctx.delta_model(source, f.name, d, m, method, g_name=None if g is None else g.name, ut=ut)
+
+
+def _check_delta_constraints(constraints):
+    if not isinstance(constraints, MeanField):
+        raise NotImplementedError("nonlinear_gamma_streaming runs under q(state, noise) = q(state) q(noise): pass "
+                                  "constraints = MeanField()")
+
+
+def _infer_delta(model, *, data, meta, initialization, free_energy, iterations, returnvars, predictvars, datastream,
+                 autoupdates, keephistory, historyvars, autostart, batch, context, **_):
+    if initialization is not None:
+        where = "state0 = (mean, cov) and noise0 = (shape, scale)" if isinstance(model, nonlinear_gamma_streaming) \
+            else "x0 = (mean, cov)"
+        raise NotImplementedError(f"initialization: {type(model).__name__} takes its initial marginals as model fields "
+                                  f"({where})")
+    if returnvars is not None and not isinstance(returnvars, KeepLast):
+        raise NotImplementedError("returnvars: the nonlinear state-space models return the last marginals (KeepLast()); "
+                                  "per-iteration results are outside the batched hot path")
+    if free_energy:
+        raise NotImplementedError("free_energy: the Delta node's energy term under Linearization / Unscented is not "
+                                  "restated on the batched path")
+    if predictvars is not None:
+        raise NotImplementedError("predictvars: predictions of the nonlinear state-space models are outside the "
+                                  "batched hot path")
+    if meta is None:
+        raise ValueError("meta: the Delta nodes need an approximation method, e.g. meta = {'f': Linearization()}")
+    delta_method(model, meta)           # refuse a bad meta before anything runs
+    smoothing = type(model) is nonlinear_gaussian_ssm_smoothing
+    if smoothing and iterations not in (None, 1):
+        raise NotImplementedError("iterations > 1 on the tree-structured smoother repeats the same schedule")
+    if data is None:
+        if smoothing:
+            raise ValueError("nonlinear_gaussian_ssm_smoothing runs over whole series: pass data = {'y': [T, m, batch]}")
+        if datastream is None and autoupdates is None:
+            raise ValueError("either `data` or `datastream` (or `autoupdates` for a push-driven engine) is required")
+        if batch is None:
+            raise ValueError("streaming inference needs `batch` (number of lock-step datastreams)")
+        from .streaming import RxInferenceEngine
+        return RxInferenceEngine(context or default_context(), model, batch=batch, iterations=iterations,
+                                 keephistory=keephistory, historyvars=historyvars, datastream=datastream,
+                                 autostart=autostart, meta=meta)
+    if "y" not in data:
+        raise KeyError("data must contain the observations under key 'y'")
+
+    def run(ctx):
+        y = torch.as_tensor(data["y"], device=f"cuda:{ctx.device}", dtype=torch.float32).contiguous()
+        mask = data.get("ymask")
+        mod = delta_module(ctx, model, meta)
+        if smoothing:
+            r = ctx.delta_smooth(mod, y, model.x0[0], model.x0[1], model.P, model.Q, B=model.B, mask=mask)
+            _raise_flagged(r["status"], "nonlinear_gaussian_ssm_smoothing: ",
+                           " (NOT_SPD: a predicted or innovation covariance is not SPD; NAN: a non-finite value)")
+            return InferenceResult(posteriors={"x": MvNormalMeanCovariance(r["mean"], r["cov"])}, model=model)
+        from .streaming import RxInferenceEngine
+        eng = RxInferenceEngine(ctx, model, batch=y.shape[-1], iterations=iterations, keephistory=y.shape[0],
+                                historyvars=historyvars, datastream=None, autostart=False, meta=meta)
+        eng.push(y if mask is None else {"y": y, "ymask": mask})
+        return InferenceResult(posteriors={}, history=eng.history, model=model)
+    return run
+
+
 def _raise_flagged(status, prefix="", suffix=""):
     """Raise ``RxGaussError`` when the kernel flagged some chains: RXG_ERR_NOT_SPD if any chain is NOT_SPD, else the first
     flagged chain's code; the message counts the chains and names the codes."""
@@ -1021,6 +1184,7 @@ class _Model(NamedTuple):
     predictions_of: str = None               # predictvars refused: "predictions of <this> are outside ..."
     whole_data: str = None                   # datastream refused: "<model> <this>"
     context_guarded: bool = False            # the context lookup is under the catch_exception guard
+    takes_meta: bool = False                 # `meta` is a keyword of the model (its Delta nodes' approximations)
 
 
 _STREAMING = ("autoupdates", "keephistory", "historyvars", "batch", "cov_shared_out")
@@ -1057,6 +1221,11 @@ _MODELS = {
                                    whole_data="runs over whole data sets: pass data = {'y'} (the online form is "
                                               "multinomial_regression_online)", context_guarded=True),
     multinomial_regression_online: _Model(_infer_multinomial_online, refuses=("cov_shared_out",)),
+    nonlinear_gaussian_ssm_smoothing: _Model(_infer_delta, takes_meta=True, refuses=_STREAMING,
+                                             refusal_note=" (the streaming form is nonlinear_gaussian_ssm_filtering)"),
+    nonlinear_gaussian_ssm_filtering: _Model(_infer_delta, takes_meta=True, refuses=("cov_shared_out",)),
+    nonlinear_gamma_streaming: _Model(_infer_delta, takes_meta=True, takes_constraints=True,
+                                      check_constraints=_check_delta_constraints, refuses=("cov_shared_out",)),
 }
 _UNRECOGNISED = _Model(_infer_unrecognised)
 
@@ -1074,6 +1243,7 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
     ``autoupdates`` is given (/root/reference/src/inference/inference.jl:577-733 dispatch)."""
     spec = next((_MODELS[t] for t in type(model).__mro__ if t in _MODELS), _UNRECOGNISED)
     constraints = kwargs.pop("constraints", None) if spec.takes_constraints else None
+    meta = kwargs.pop("meta", None) if spec.takes_meta else None
     for k in kwargs:
         if k in _UNSUPPORTED:
             raise NotImplementedError(
@@ -1101,7 +1271,7 @@ def infer(*, model, iterations=None, free_energy=False, returnvars=None, options
     run = spec.handler(model, data=data, constraints=constraints, initialization=initialization, iterations=iterations,
                        free_energy=free_energy, returnvars=returnvars, predictvars=predictvars, datastream=datastream,
                        autoupdates=autoupdates, keephistory=keephistory, historyvars=historyvars, autostart=autostart,
-                       batch=batch, cov_shared_out=cov_shared_out, context=context)
+                       batch=batch, cov_shared_out=cov_shared_out, context=context, meta=meta)
     if not callable(run):
         return run                                   # a streaming engine
     if not spec.context_guarded:

@@ -318,6 +318,23 @@ lgssm_smooth_gather(ctx, d, m, T, bl, A, B, P, Q, m0, S0, u, y, mask, gm::Vector
     check(ctx, ccall((:rxg_lgssm_smooth_gather_f32, LIB), Cint,
         (Ptr{Cvoid}, Cint, Cint, Cint, Int64, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{UInt8}, Ptr{F32P}, Ptr{F32P}, F32P, Ptr{Int32}, Cuint),
         ctx.handle, d, m, T, bl, A, B, P, Q, m0, S0, u, y, mask, gm, gc, nle, st, fl))
+# Delta node: user CUDA functions compiled at run time (NVRTC); `method` 0 = Linearization, 1 = Unscented
+delta_check_source(src, f, g, d, m, method, ut, log, cap) =
+    ccall((:rxg_delta_check_source, LIB), Cint, (Cstring, Cstring, Ptr{UInt8}, Cint, Cint, Cint, Ptr{Cdouble}, Ptr{UInt8}, Csize_t),
+        src, f, g, d, m, method, ut, log, cap)
+delta_model_create(ctx, src, f, g, d, m, method, ut, out, log, cap) =
+    check(ctx, ccall((:rxg_delta_model_create, LIB), Cint,
+        (Ptr{Cvoid}, Cstring, Cstring, Ptr{UInt8}, Cint, Cint, Cint, Ptr{Cdouble}, Ptr{Ptr{Cvoid}}, Ptr{UInt8}, Csize_t),
+        ctx.handle, src, f, g, d, m, method, ut, out, log, cap))
+delta_compile_count(ctx) = ccall((:rxg_delta_compile_count, LIB), Clonglong, (Ptr{Cvoid},), ctx.handle)
+delta_smooth(ctx, model, T, b, m0, S0, P, B, Q, y, mask, pm, pc, fm, fc, st, fl) =
+    check(ctx, ccall((:rxg_delta_smooth_f32, LIB), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Int64, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{UInt8}, F32P, F32P, F32P, F32P, Ptr{Int32}, Cuint),
+        ctx.handle, model, T, b, m0, S0, P, B, Q, y, mask, pm, pc, fm, fc, st, fl))
+delta_filter_chunk(ctx, model, T, b, P, B, Q, iters, y, mask, cm, cc, ct, fm, fc, ft, st, fl) =
+    check(ctx, ccall((:rxg_delta_filter_chunk_f32, LIB), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Cint, Int64, F32P, F32P, F32P, Cint, F32P, Ptr{UInt8}, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Int32}, Cuint),
+        ctx.handle, model, T, b, P, B, Q, iters, y, mask, cm, cc, ct, fm, fc, ft, st, fl))
 end # module Lib
 
 # ---------------------------------------------------------------------------------------------- 2. device arrays and batched messages

@@ -25,7 +25,7 @@ class RxInferenceEngine:
     ``Subject``-style datastream).  ``autostart=True`` consumes an iterable datastream immediately."""
 
     def __init__(self, ctx, model, *, batch, iterations=1, keephistory=None, historyvars=None, free_energy=False,
-                 datastream=None, autostart=True, cov_shared_out=False, initialization=None):
+                 datastream=None, autostart=True, cov_shared_out=False, initialization=None, meta=None):
         from . import inference as I
         self.ctx, self.model, self.batch = ctx, model, int(batch)
         self.iterations = int(iterations or 1)
@@ -54,6 +54,23 @@ class RxInferenceEngine:
             m0 = torch.as_tensor(np.asarray(model.x0[0], np.float32), device=f"cuda:{ctx.device}")
             self._prev_mean = m0[:, None].expand(-1, self.batch).contiguous()      # q(x_t) initialisation, broadcast
             self._carry_cov = np.ascontiguousarray(np.asarray(model.x0[1], np.float32)).copy()
+        elif isinstance(model, (I.nonlinear_gaussian_ssm_filtering, I.nonlinear_gamma_streaming)):
+            # the Delta-node filter: the carry q(x) (and q(noise)) is per chain, [d, batch] / [d, d, batch] on the device
+            gamma = isinstance(model, I.nonlinear_gamma_streaming)
+            self._kind = "delta"
+            names = ("state", "noise") if gamma else ("x_t",)
+            self._module = I.delta_module(ctx, model, meta)
+            mean, cov = model.state0 if gamma else model.x0
+            dev = f"cuda:{ctx.device}"
+            m0 = torch.as_tensor(np.asarray(mean, np.float32), device=dev)
+            S0 = torch.as_tensor(np.asarray(cov, np.float32), device=dev)
+            self._mean = m0[:, None].expand(-1, self.batch).contiguous()
+            self._cov = S0[:, :, None].expand(-1, -1, self.batch).contiguous()
+            self._tau = None
+            if gamma:      # Gamma(shape, scale) of the paper -> (shape, rate)
+                shape, scale = model.noise0
+                self._tau = torch.tensor([[float(shape)], [1.0 / float(scale)]], dtype=torch.float32,
+                                         device=dev).expand(-1, self.batch).contiguous()
         elif isinstance(model, I.multinomial_regression_online):
             self._kind = "multinomial"
             names = ("ψ",)
@@ -99,13 +116,16 @@ class RxInferenceEngine:
     # -------------------------------------------------------------- one tick = one chunk (streaming.jl:344-430)
     def push(self, chunk):
         """Consume one chunk; returns the chunk's marginals (dict name -> batched distribution)."""
-        inputs = None
+        inputs = mask = None
         if isinstance(chunk, dict):      # {"y": [Tc, m, batch], "u": the chunk's known inputs ([Tc, d] or [Tc, d, batch])}
+            # (the Delta-node engine also takes "ymask": [Tc, batch], 1 = observed)
             if self._kind != "lgssm" and "u" in chunk:
                 raise NotImplementedError("input sequences belong to the LGSSM streaming engine")
-            chunk, inputs = chunk["y"], chunk.get("u")
+            chunk, inputs, mask = chunk["y"], chunk.get("u"), chunk.get("ymask")
         if self._kind == "multinomial":
             return self._push_multinomial(chunk)
+        if self._kind == "delta":
+            return self._push_delta(chunk, mask)
         if self._kind == "lgssm":
             mo = self.model
             r = self.ctx.lgssm_filter_chunk(chunk, mo.A, mo.B, mo.P, mo.Q, self._prev_mean, self._carry_cov, u=mo.u,
@@ -159,6 +179,30 @@ class RxInferenceEngine:
         self._keep(out)
         return out
 
+    def _push_delta(self, chunk, mask):
+        """One chunk y[Tc, m, batch] (or [Tc, batch] when m = 1) of the Delta-node filter: one
+        ``rxg_delta_filter_chunk_f32`` call, the carry updated in place.  A chunk that flags a chain raises."""
+        from .inference import _raise_flagged
+        mo = self.model
+        y = chunk[:, None] if chunk.dim() == 2 else chunk
+        d = self._module.d
+        P = np.zeros((d, d)) if getattr(mo, "P", None) is None else mo.P
+        if self._tau is not None:
+            r = self.ctx.delta_filter_chunk(self._module, y.contiguous(), P, self._mean, self._cov,
+                                            B=np.asarray(mo.c, np.float64).reshape(1, -1), carry_tau=self._tau,
+                                            iters=self.iterations, mask=mask)
+        else:
+            r = self.ctx.delta_filter_chunk(self._module, y.contiguous(), P, self._mean, self._cov, Q=mo.Q, B=mo.B,
+                                            mask=mask)
+        _raise_flagged(r["status"], f"{type(mo).__name__}: ", " (NOT_SPD: a predicted or innovation covariance is not "
+                                                              "SPD; NAN: a non-finite value)")
+        self.ticks += int(y.shape[0])
+        out = {("state" if self._tau is not None else "x_t"): MvNormalMeanCovariance(r["mean"], r["cov"])}
+        if self._tau is not None:
+            out["noise"] = GammaShapeRate(r["tau"][:, 0], r["tau"][:, 1])
+        self._keep(out)
+        return out
+
     def _keep(self, out):
         if self.keephistory:
             for name in self.historyvars:
@@ -176,6 +220,11 @@ class RxInferenceEngine:
         """Most recent marginals (the reference exposes observables; here: the last tick's values)."""
         if self._kind == "lgssm":
             return {"x_t": (self._prev_mean, self._carry_cov.copy())}
+        if self._kind == "delta":            # per-chain carry, [d, batch] / [d, d, batch] (and (shape, rate) [batch])
+            q = {("state" if self._tau is not None else "x_t"): MvNormalMeanCovariance(self._mean, self._cov)}
+            if self._tau is not None:
+                q["noise"] = GammaShapeRate(self._tau[0], self._tau[1])
+            return q
         if self._kind == "multinomial":      # fp64 carry, [D, batch] / [D, D, batch]
             return {"ψ": None if self._carry is None else MvNormalMeanCovariance(*self._carry)}
         if self._kind == "vmpgamma":
