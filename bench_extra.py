@@ -17,6 +17,7 @@ the per-rule kernels, one JSON line each.  Device-resident data, CUDA events, >=
                                              times, data-pass bandwidth and fp64 FMA rate)
   python bench_extra.py --which hgf_learn    (opt-in: HGF with learned kappa, omega, T = 1000, 20 iterations)
   python bench_extra.py --which delta        (opt-in: Delta node: the paper's pendulum stream, the d = 4 tracker smoother)
+  python bench_extra.py --which gamma_mixture (opt-in: Gamma-mixture VMP with point-mass shapes, K = 2 and K = 8)
 """
 from __future__ import annotations
 
@@ -385,6 +386,43 @@ def bench_gmm(ctx, peak):
         torch.cuda.empty_cache()
 
 
+def bench_gamma_mixture(ctx, peak):
+    """Gamma-mixture VMP with point-mass shapes (rxg_gamma_mixture_vmp_f32), N = 250 points per data set, 50 iterations,
+    65 536 data sets, free energy on; time from CUDA events around the call (host validation and the constant upload
+    included, both O(K)), median of repeated calls.  Per datum and iteration the data pass reads 4 B of y and issues
+    K + 3 MUFU operations (K exp, log y, log and reciprocal of the normaliser), K + 3 fp32 -> fp64 conversions (also
+    16 / clock / SM) and 3 K + 1 fp64 adds / FMAs; the estimated bound is the largest of the HBM, MUFU + conversion and
+    fp64 times (clock-rate estimates at the 1.98 GHz boost clock, not measurements)."""
+    gname, plim = gpu_name_and_power_limit()
+    torch.manual_seed(23)
+    N, nb, its = 250, 65536, 50
+    sm = torch.cuda.get_device_properties(0).multi_processor_count
+    clk = 1.98e9
+    for K in (2, 8):
+        shapes = torch.linspace(3.0, 60.0, K, device="cuda")
+        means = torch.logspace(-1.0, 0.5, K, device="cuda")
+        lab = torch.randint(0, K, (N, nb), device="cuda")
+        y = torch.distributions.Gamma(shapes[lab], shapes[lab] / means[lab]).sample().contiguous()
+        one = np.ones(K)
+        args = (one, one, 0.1 * one, one, one, one, one, np.linspace(0.5, 5.0, K), one)
+        r = ctx.gamma_mixture_vmp(y, *args, iterations=its)
+        flagged = int((r["status"] != 0).sum())
+        runs = [timed(lambda: ctx.gamma_mixture_vmp(y, *args, iterations=its), warm=2, reps=3) for _ in range(3)]
+        ms = float(np.median(runs))
+        n = N * nb * its
+        t = {"hbm": 4 * n / (peak * 1e9), "mufu_cvt": 2 * (K + 3) * n / (16 * sm * clk),
+             "fp64": (3 * K + 1) * n / (64 * sm * clk)}
+        bound = max(t, key=t.get)
+        print(json.dumps({"what": "Gamma-mixture VMP (gamma_mixture_vmp_kernel), free energy on", "K": K, "N": N,
+                          "batch": nb, "iterations": its, "ms": ms, "ms_runs": runs, "ms_per_iteration": ms / its,
+                          "bytes_per_iteration": 4 * N * nb, "achieved_GBs": 4 * n / ms / 1e6,
+                          "estimated_bound": bound, "bound_ms": {k: v * 1e3 for k, v in t.items()},
+                          "frac_of_bound": t[bound] * 1e3 / ms, "flagged_chains": flagged, "peak_hbm_gbs": peak,
+                          "gpu": gname, "power_limit": plim}), flush=True)
+        del y
+        torch.cuda.empty_cache()
+
+
 def bench_hmm(ctx, peak):
     """Hidden Markov model VMP (rxg_hmm_vmp_f32), T = 1000 steps, 20 iterations, 65 536 chains, A and B learned, free
     energy on; time from CUDA events around the call (host validation and the constant upload included, both O(M K)).
@@ -690,6 +728,8 @@ def main():
         bench_hmm_gauss(ctx, peak)
     if "delta" in which:
         bench_delta(ctx)
+    if "gamma_mixture" in which:
+        bench_gamma_mixture(ctx, peak)
     mod = notebook_model_f32()
     kw = dict(A=mod["A"], B=mod["B"], P=mod["P"], Q=mod["Q"], m0=mod["m0"], S0=mod["S0"])
     T, batch = 1000, 65536

@@ -274,6 +274,30 @@ int rxg_gmm_vmp_f32(rxg_ctx*, int d, int K, int N, int64_t batch, int iterations
                     float* m_mean, float* m_cov, float* w_df, float* w_inv_scale, double* free_energy, float* z_prob,
                     float* hist_alpha, float* hist_m_mean, float* hist_m_cov, float* hist_w_df, float* hist_w_inv_scale,
                     int32_t* status, unsigned flags);
+/* Fused mean-field VMP of the Gamma mixture model with point-mass shapes, `batch` independent data sets, all iterations
+ *   in one launch: s ~ Dirichlet(alpha_s), a[k] ~ Gamma(a_shape0[k], a_rate0[k]), b[k] ~ Gamma(b_shape0[k], b_rate0[k])
+ *   (shape, rate), z[i] ~ Categorical(s), y[i] ~ GammaMixture(z[i], a, b) (component k: Gamma(shape a[k], rate b[k])),
+ *   q(z) q(a) q(b) q(s) with q(a[k]) a point mass (PointMassFormConstraint, Newton's method from a_start[k] in fp64),
+ *   initialised to Dirichlet(alpha_init), Gamma(b_shape_init[k], b_rate_init[k]) and a uniform q(z)
+ *   [ref: test/models/mixtures/gamma_mixture_tests.jl:7-40, :45-76].  Priors, initial marginals and starting points are
+ *   HOST arrays shared by every chain: alpha_s[K], a_shape0[K], a_rate0[K], b_shape0[K], b_rate0[K], alpha_init[K],
+ *   b_shape_init[K], b_rate_init[K], a_start[K].  y[N][batch].  Outputs of the last iteration: alpha[K][batch] (q(s)),
+ *   a_hat[K][batch] (the point masses), b_shape[K][batch], b_rate[K][batch] (q(b[k])).  Optional (NULL = not wanted):
+ *   free_energy[iterations][batch] (fp64, the free energy after every iteration, the point masses' entropy left out),
+ *   z_prob[N][K][batch] (q(z) of the last iteration), the KeepEach histories hist_a[iterations][K][batch],
+ *   hist_b_shape[iterations][K][batch], hist_b_rate[iterations][K][batch], status[batch] (RXG_ERR_BAD_ARG for a chain
+ *   with a datum <= 0 or not finite, whose outputs are then NaN; RXG_ERR_NAN for a chain whose Newton iteration did not
+ *   reach a relative step of 1e-12 within 100 steps).  Per iteration: the point masses a (with the previous q(b)), q(b),
+ *   q(s), then q(z) from the new marginals; q(s) is formed before it is first read, so alpha_init does not enter.
+ *   2 <= K <= 8 and every a_shape0 >= 1 (the shape objective is then concave), else RXG_ERR_UNSUPPORTED; N, batch,
+ *   iterations >= 1 and every host parameter positive and finite, else RXG_ERR_BAD_ARG.  Device pointers
+ *   (RXG_ERR_UNSUPPORTED otherwise).                                                                                  */
+int rxg_gamma_mixture_vmp_f32(rxg_ctx*, int K, int N, int64_t batch, int iterations, const float* alpha_s,
+                              const float* a_shape0, const float* a_rate0, const float* b_shape0, const float* b_rate0,
+                              const float* alpha_init, const float* b_shape_init, const float* b_rate_init,
+                              const float* a_start, const float* y, float* alpha, float* a_hat, float* b_shape,
+                              float* b_rate, double* free_energy, float* z_prob, float* hist_a, float* hist_b_shape,
+                              float* hist_b_rate, int32_t* status, unsigned flags);
 /* Fused structured VMP of the hidden Markov model, `batch` independent chains, all iterations in one launch:
  *   A ~ DirichletCollection(A_prior) (K x K, column j = p(s_t | s_{t-1} = j)), B ~ DirichletCollection(B_prior) (M x K,
  *   column j = p(x_t | s_t = j)), s_0 ~ Categorical(p0), s[t] ~ DiscreteTransition(s[t-1], A), x[t] ~

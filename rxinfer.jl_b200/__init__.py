@@ -24,7 +24,7 @@ def __getattr__(name):   # lazy: these import torch
                 "GaussianHMMConstraints", "binomial_regression", "multinomial_regression",
                 "multinomial_regression_online", "CudaFunction", "Linearization", "Unscented",
                 "nonlinear_gaussian_ssm_smoothing", "nonlinear_gaussian_ssm_filtering", "nonlinear_gamma_streaming",
-                "default_context",
+                "gamma_mixture", "GammaMixtureConstraints", "default_context",
                 "KeepLast", "KeepEach"):
         from . import inference
         return getattr(inference, name)

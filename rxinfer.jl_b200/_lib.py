@@ -73,6 +73,8 @@ SIGNATURES = {
     "rxg_lar_vmp_f32": (c_int, [c_void_p, c_int, c_int, c_int64, c_int, fp, fp, fp, fp, fp, fp, fp, fp, POINTER(c_double), i32p, c_uint]),
     "rxg_gmm_vmp_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, c_int, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp,
                                 fp, fp, POINTER(c_double), fp, fp, fp, fp, fp, fp, i32p, c_uint]),
+    "rxg_gamma_mixture_vmp_f32": (c_int, [c_void_p, c_int, c_int, c_int64, c_int, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp,
+                                          fp, fp, fp, fp, POINTER(c_double), fp, fp, fp, fp, i32p, c_uint]),
     "rxg_hmm_vmp_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, c_int, fp, fp, fp, fp, fp, fp, fp, u8p, fp, fp, fp, fp,
                                 POINTER(c_double), fp, fp, fp, i32p, c_uint]),
     "rxg_hmm_gauss_vmp_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int64, c_int, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp,

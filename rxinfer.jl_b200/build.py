@@ -20,10 +20,10 @@ UNITS = ([("rxg_lgssm.cu", f"rxg_lgssm_d{d}m{m}", (f"-DRXG_INST_D={d}", f"-DRXG_
           ("rxg_lgssm_large.cu", "rxg_lgssm.cu", "rxg_umma_sweep.cu", "rxg_api.cu", "rxg_peer.cu", "rxg_rules.cu", "rxg_hgf.cu",
            "rxg_lgssm_general.cu", "rxg_lgssm_generic.cu", "rxg_lar.cu", "rxg_rules_large.cu", "rxg_predict.cu",
            "rxg_lgssm_vmp.cu", "rxg_mixture.cu", "rxg_hmm.cu", "rxg_hgf_learn.cu", "rxg_hmm_gauss.cu", "rxg_polya.cu",
-           "rxg_multinomial.cu", "rxg_delta.cu")] +
+           "rxg_multinomial.cu", "rxg_delta.cu", "rxg_gamma_mixture.cu")] +
          [("rxg_hostfill.cpp", "rxg_hostfill", ())])        # plain C++ (g++): host-side covariance broadcast
 SOURCES = sorted({u[0] for u in UNITS})
-HEADERS = ["rxg_internal.h", "rxg_linalg.cuh", "rxg_gain.cuh", "rxg_lgssm_common.cuh", "rxg_chain_step.cuh", "rxg_lgssm_shared.cuh", "rxg_lgssm_seg.cuh", "rxg_lgssm_cluster.cuh", "rxg_sweep_select.h", "rxg_umma.cuh", "rxg_lar.cuh", "rxg_hmm.cuh", "rxg_hgf_learn.cuh", "rxg_hmm_gauss.cuh", "rxg_normal_wishart.cuh", "rxg_polya.cuh", "rxg_multinomial.cuh", "rxg_delta.cuh", os.path.join("..", "..", "include", "rxgauss.h")]
+HEADERS = ["rxg_internal.h", "rxg_linalg.cuh", "rxg_gain.cuh", "rxg_lgssm_common.cuh", "rxg_chain_step.cuh", "rxg_lgssm_shared.cuh", "rxg_lgssm_seg.cuh", "rxg_lgssm_cluster.cuh", "rxg_sweep_select.h", "rxg_umma.cuh", "rxg_lar.cuh", "rxg_hmm.cuh", "rxg_hgf_learn.cuh", "rxg_hmm_gauss.cuh", "rxg_normal_wishart.cuh", "rxg_polya.cuh", "rxg_multinomial.cuh", "rxg_delta.cuh", "rxg_gamma_mixture.cuh", os.path.join("..", "..", "include", "rxgauss.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-mavx2", "-Xcompiler", "-pthread", "--expt-relaxed-constexpr", "-Xptxas", "-v",

@@ -875,6 +875,39 @@ class Context:
         out.update(h)
         return out
 
+    GAMMA_MIXTURE_KEYS = ("alpha_s", "a_shape0", "a_rate0", "b_shape0", "b_rate0", "alpha_init", "b_shape_init",
+                          "b_rate_init", "a_start")
+
+    def gamma_mixture_vmp(self, y, alpha_s, a_shape0, a_rate0, b_shape0, b_rate0, alpha_init, b_shape_init, b_rate_init,
+                          a_start, iterations=10, want_free_energy=True, want_z=False, keep_each=False):
+        """Fused mean-field VMP of the Gamma mixture model with point-mass shapes (``rxg_gamma_mixture_vmp_f32``);
+        y[N, batch] on the device.  Priors, initial marginals and the shapes' starting points are host arrays [K] shared
+        by every chain, in the order of ``GAMMA_MIXTURE_KEYS`` (Gamma parameters as shape / rate).  Returns the last
+        iteration's ``alpha[K, batch]`` (q(s)), ``a_hat[K, batch]``, ``b_shape[K, batch]``, ``b_rate[K, batch]``,
+        ``free_energy[iterations, batch]`` (fp64), ``z_prob[N, K, batch]`` (with ``want_z``), ``status[batch]`` and, with
+        ``keep_each``, ``hist_a`` / ``hist_b_shape`` / ``hist_b_rate`` with a leading iteration axis."""
+        self._dev(y)
+        if y.dim() != 2:
+            raise ValueError("gamma_mixture_vmp: y must be [N, batch]")
+        N, batch = y.shape
+        K = int(np.asarray(alpha_s).reshape(-1).shape[0])
+        vals = (alpha_s, a_shape0, a_rate0, b_shape0, b_rate0, alpha_init, b_shape_init, b_rate_init, a_start)
+        keep = _host_arrays("gamma_mixture_vmp", {k: (v, (K,)) for k, v in zip(self.GAMMA_MIXTURE_KEYS, vals)},
+                            f"K = {K}")
+        its = int(iterations)
+        al, ah, bs, br = (self.empty(K, batch) for _ in range(4))
+        fe = self.empty(its, batch, dtype=torch.float64) if want_free_energy else None
+        z = self.empty(N, K, batch) if want_z else None
+        h = {k: self.empty(its, K, batch) for k in ("hist_a", "hist_b_shape", "hist_b_rate")} if keep_each else {}
+        st = self.empty(batch, dtype=torch.int32)
+        self._check(self.lib.rxg_gamma_mixture_vmp_f32(self.h, K, N, batch, its, *(p for _, p in keep.values()), _fp(y),
+                                                       _fp(al), _fp(ah), _fp(bs), _fp(br), _f64(fe), _fp(z),
+                                                       *(_fp(h.get(k)) for k in ("hist_a", "hist_b_shape", "hist_b_rate")),
+                                                       _i32(st), L.PTR_DEVICE))
+        out = dict(alpha=al, a_hat=ah, b_shape=bs, b_rate=br, free_energy=fe, z_prob=z, status=st)
+        out.update(h)
+        return out
+
     def hmm_vmp(self, x, p0, A_prior=None, A_init=None, A_known=None, B_prior=None, B_init=None, B_known=None,
                 iterations=1, want_free_energy=True, keep_each=False):
         """Fused structured VMP of the hidden Markov model (``rxg_hmm_vmp_f32``); x[T, batch] uint8 symbols on the device

@@ -15,8 +15,12 @@ import torch
 
 @dataclass
 class PointMass:
-    """Constant / datum (factorised out by default, /root/reference/src/model/model.jl:198,222)."""
+    """Constant / datum (factorised out by default, /root/reference/src/model/model.jl:198,222), or a marginal under a
+    point-mass form constraint."""
     value: object
+
+    def mean(self):
+        return self.value
 
 
 @dataclass

@@ -834,6 +834,122 @@ def _infer_binomial(model, *, data, initialization, iterations, free_energy, ret
 
 
 @dataclass
+class gamma_mixture:
+    """Gamma mixture model (RxInfer test/models/mixtures/gamma_mixture_tests.jl:7-40): ``s ~ prior_s``,
+    ``as[k] ~ Gamma(shape, rate of priors_as[k])``, ``bs[k] ~ Gamma(shape, rate of priors_bs[k])``, ``z[i] ~
+    Categorical(s)``, ``y[i] ~ GammaMixture(switch = z[i], a = as, b = bs)`` (component k: Gamma(shape as[k], rate
+    bs[k])), fitted by mean-field VMP with point-mass shapes (DESIGN 3.24).  ``prior_s`` is a ``Dirichlet``, the priors
+    ``GammaShapeRate``; every shape prior needs shape >= 1.  Run with ``constraints = GammaMixtureConstraints(a_start)``,
+    ``initialization = {"s": Dirichlet, "z": vague(Categorical, K), "bs": GammaShapeRate or a list of K}`` and
+    ``data = {"y": [N, batch]}`` (one data set may come as [N])."""
+    K: int
+    prior_s: object
+    priors_as: list
+    priors_bs: list
+
+
+@dataclass(frozen=True)
+class GammaMixtureConstraints:
+    """``q(z, as, bs, s) = q(z)q(as)q(bs)q(s)`` with every q(as[k]) and q(bs[k]) apart and ``q(as)::
+    PointMassFormConstraint(starting_point = a_start)`` (gamma_mixture_tests.jl:35-42): the shapes are MAP points, found
+    by Newton's method from ``a_start`` (a number, or one per component)."""
+    a_start: object = 1.0
+
+
+def _check_gamma_mixture_constraints(constraints):
+    if not isinstance(constraints, GammaMixtureConstraints):
+        raise ValueError("gamma_mixture runs q(z) q(as) q(bs) q(s) with q(as)::PointMassFormConstraint only: the Gamma "
+                         "shape has no conjugate posterior, so q(as) must be a point mass; pass constraints = "
+                         f"GammaMixtureConstraints(a_start=...) (got {constraints!r})")
+
+
+def _gamma_params(xs, K, what):
+    xs = list(xs) if isinstance(xs, (list, tuple)) else [xs] * K
+    if len(xs) != K:
+        raise ValueError(f"{what}: {len(xs)} marginals for K = {K} components")
+    if not all(isinstance(x, GammaShapeRate) for x in xs):
+        raise TypeError(f"{what}: expected GammaShapeRate, got {[type(x).__name__ for x in xs]}")
+    return np.array([float(x.a) for x in xs]), np.array([float(x.b) for x in xs])
+
+
+def gamma_mixture_arguments(model, constraints, initialization):
+    """The host arrays [K] of ``Context.gamma_mixture_vmp`` (``Context.GAMMA_MIXTURE_KEYS``) from the model, its
+    constraints and ``initialization``; refuses what the batched path does not run."""
+    K = int(model.K)
+    if not 2 <= K <= 8:
+        raise NotImplementedError(f"gamma_mixture: K = {K} components; the batched path runs 2 <= K <= 8")
+    if not isinstance(model.prior_s, Dirichlet):
+        raise TypeError(f"prior_s: expected Dirichlet, got {type(model.prior_s).__name__}")
+    out = dict(alpha_s=_weights(model.prior_s, K, "prior_s"))
+    out["a_shape0"], out["a_rate0"] = _gamma_params(model.priors_as, K, "priors_as")
+    out["b_shape0"], out["b_rate0"] = _gamma_params(model.priors_bs, K, "priors_bs")
+    if (out["a_shape0"] < 1.0).any():
+        raise NotImplementedError(f"priors_as: shape {out['a_shape0'].min()} < 1; the batched path needs every shape prior "
+                                  ">= 1, where the point-mass objective is concave and its maximiser unique")
+    a0 = np.broadcast_to(np.asarray(constraints.a_start, np.float64).reshape(-1), (K,)).copy() \
+        if np.size(constraints.a_start) in (1, K) else None
+    if a0 is None or not (np.isfinite(a0) & (a0 > 0)).all():
+        raise ValueError(f"GammaMixtureConstraints: a_start must be one positive number or {K}, got {constraints.a_start!r}")
+    out["a_start"] = a0
+    if not isinstance(initialization, dict) or not {"s", "bs"} <= set(initialization):
+        raise ValueError("gamma_mixture needs initialization = {'s': Dirichlet, 'z': vague(Categorical, K), 'bs': "
+                         "GammaShapeRate or a list}")
+    bad = set(initialization) - {"s", "z", "bs"}
+    if bad:
+        raise ValueError(f"initialization: {sorted(bad)} are not initialised on this model (s, z, bs; as has its "
+                         "starting point in the constraints)")
+    if not isinstance(initialization["s"], Dirichlet):
+        raise TypeError(f"initialization['s']: expected Dirichlet, got {type(initialization['s']).__name__}")
+    out["alpha_init"] = _weights(initialization["s"], K, "initialization['s']")
+    z = initialization.get("z")
+    if z is not None:
+        p = np.asarray(z.p if isinstance(z, Categorical) else np.nan, np.float64).reshape(-1)
+        if not isinstance(z, Categorical) or p.shape != (K,) or not np.allclose(p, 1.0 / K, rtol=0, atol=1e-12):
+            raise NotImplementedError("initialization['z']: the batched path starts from the uniform q(z) = "
+                                      f"vague(Categorical, {K})")
+    out["b_shape_init"], out["b_rate_init"] = _gamma_params(initialization["bs"], K, "initialization['bs']")
+    for k, v in out.items():
+        if not (np.isfinite(v) & (v > 0)).all():
+            raise ValueError(f"gamma_mixture: {k} must be positive and finite, got {v}")
+    return out
+
+
+def _infer_gamma_mixture(model, *, data, constraints, initialization, iterations, free_energy, returnvars, **_):
+    """``infer`` of ``gamma_mixture``: one ``rxg_gamma_mixture_vmp_f32`` launch.  ``returnvars`` is KeepLast() /
+    KeepEach() or a dict over ``s``, ``z``, ``as``, ``bs``, KeepEach() for ``as`` and ``bs`` (a leading iteration
+    axis)."""
+    if "y" not in data:
+        raise KeyError("gamma_mixture needs data = {'y': [N, batch]}")
+    bad = set(data) - {"y"}
+    if bad:
+        raise ValueError(f"gamma_mixture: unknown data {sorted(bad)} (y)")
+    each = _kept_each("gamma_mixture", returnvars, ("s", "z", "as", "bs"), each=("as", "bs"))
+    args = gamma_mixture_arguments(model, constraints, initialization)
+    y = torch.as_tensor(data["y"])
+    single = y.dim() == 1
+    y = y[:, None] if single else y
+    if y.dim() != 2:
+        raise ValueError(f"data['y'] must be [N, batch] (or [N]), got {tuple(y.shape)}")
+    K = int(model.K)
+
+    def run(ctx):
+        r = ctx.gamma_mixture_vmp(y.to(device=f"cuda:{ctx.device}", dtype=torch.float32).contiguous(),
+                                  *(args[k] for k in Context.GAMMA_MIXTURE_KEYS), iterations=iterations or 1,
+                                  want_free_energy=bool(free_energy), want_z=True, keep_each=bool(each))
+        _raise_flagged(r["status"], "gamma_mixture: ", " (BAD_ARG: a datum <= 0 or not finite; NAN: a shape's Newton "
+                                                       "iteration did not converge)")
+        a = r["hist_a"] if "as" in each else r["a_hat"]
+        bs, br = (r["hist_b_shape"], r["hist_b_rate"]) if "bs" in each else (r["b_shape"], r["b_rate"])
+        sq = (lambda t: t[..., 0]) if single else (lambda t: t)          # one data set: no batch axis
+        post = {"s": Dirichlet(sq(r["alpha"])), "z": Categorical(sq(r["z_prob"])),
+                "as": [PointMass(sq(a[..., k, :])) for k in range(K)],
+                "bs": [GammaShapeRate(sq(bs[..., k, :]), sq(br[..., k, :])) for k in range(K)]}
+        fe = r["free_energy"]
+        return InferenceResult(posteriors=post, model=model, free_energy=None if fe is None else sq(fe))
+    return run
+
+
+@dataclass
 class multinomial_regression:
     """Bayesian multinomial regression (RxInfer test/models/regression/multinomialreg_tests.jl, offline item):
     ``ψ ~ MvNormalWeightedMeanPrecision(prior_xi, prior_precision)``, ``y[i] ~ MultinomialPolya(N_i, ψ)`` with N_i the sum
@@ -1221,6 +1337,10 @@ _MODELS = {
                                    whole_data="runs over whole data sets: pass data = {'y'} (the online form is "
                                               "multinomial_regression_online)", context_guarded=True),
     multinomial_regression_online: _Model(_infer_multinomial_online, refuses=("cov_shared_out",)),
+    gamma_mixture: _Model(_infer_gamma_mixture, takes_constraints=True, check_constraints=_check_gamma_mixture_constraints,
+                          refuses=_STREAMING, predictions_of="y",
+                          whole_data="runs over whole data sets: pass data = {'y': [N, batch]} (no datastream)",
+                          context_guarded=True),
     nonlinear_gaussian_ssm_smoothing: _Model(_infer_delta, takes_meta=True, refuses=_STREAMING,
                                              refusal_note=" (the streaming form is nonlinear_gaussian_ssm_filtering)"),
     nonlinear_gaussian_ssm_filtering: _Model(_infer_delta, takes_meta=True, refuses=("cov_shared_out",)),

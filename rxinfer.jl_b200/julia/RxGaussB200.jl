@@ -249,6 +249,12 @@ gmm_vmp(ctx, d, K, N, batch, its, a0, mu0, V0, nu0, S0, ai, mi, Vi, nui, Si, y, 
         ctx.handle, d, K, N, batch, its, a0, mu0, V0, nu0, S0, ai, mi, Vi, nui, Si, y, al, mm, mc, df, iS, fe, z, hal, hmm, hmc, hdf,
         hiS, st, fl))
 
+gamma_mixture_vmp(ctx, K, N, batch, its, als, ash, art, bsh, brt, ai, bshi, brti, a0, y, al, ah, bs, br, fe, z, ha, hbs, hbr, st, fl) =
+    check(ctx, ccall((:rxg_gamma_mixture_vmp_f32, LIB), Cint,
+        (Ptr{Cvoid}, Cint, Cint, Int64, Cint, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P, F32P,
+         Ptr{Float64}, F32P, F32P, F32P, F32P, Ptr{Int32}, Cuint),
+        ctx.handle, K, N, batch, its, als, ash, art, bsh, brt, ai, bshi, brti, a0, y, al, ah, bs, br, fe, z, ha, hbs, hbr, st, fl))
+
 hgf_vmp_learn(ctx, T, batch, its, prior, zp, yv, init, y, x0, xz, kw, hkw, fe, st, fl) =
     check(ctx, ccall((:rxg_hgf_vmp_learn_f32, LIB), Cint,
         (Ptr{Cvoid}, Cint, Int64, Cint, F32P, Cfloat, Cfloat, F32P, F32P, F32P, F32P, F32P, F32P, Ptr{Float64}, Ptr{Int32}, Cuint),
